@@ -134,20 +134,30 @@ struct Struct {
   int m;                      // inequality rows of THIS scene (== P.m, or 4 nc_s / nc_s on the engine path with per-scene contact counts)
 };
 
-// optional per-phase SM cycle counters (thread 0 of every CTA; lcpb200_profile)
+// optional per-phase SM cycle counters (thread 0 of every CTA; lcpb200_profile). A compile-time switch: the
+// kernels are instantiated twice, and the production instantiation carries no profiling state (a pointer and a
+// timestamp live across every phase cost registers the LU and the solves need).
 enum { CPH_STRUCT = 0, CPH_WINV, CPH_ASSEMBLE, CPH_LU, CPH_SOLVE_RHS, CPH_SOLVE_TRI, CPH_SOLVE_POST, CPH_RESID,
        CPH_STEP, CPH_GRADS, CPH_COUNT };
+template <bool ON>
 struct Prof {
-  long long* p;               // nullptr or this CTA's CPH_COUNT counters
+  long long* p;               // this CTA's CPH_COUNT counters
   long long t;
-  __device__ __forceinline__ void start() { if (p && threadIdx.x == 0) t = clock64(); }
+  __device__ __forceinline__ explicit Prof(long long* p_) : p(p_), t(0) {}
+  __device__ __forceinline__ void start() { if (threadIdx.x == 0) t = clock64(); }
   __device__ __forceinline__ void lap(int ph) {
-    if (p && threadIdx.x == 0) {
+    if (threadIdx.x == 0) {
       const long long n = clock64();
       atomicAdd(reinterpret_cast<unsigned long long*>(p + ph), (unsigned long long)(n - t));   // no dependent load
       t = n;
     }
   }
+};
+template <>
+struct Prof<false> {
+  __device__ __forceinline__ explicit Prof(long long*) {}
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void lap(int) {}
 };
 
 // ------------------------------------------------------------------ structure detection
@@ -915,10 +925,14 @@ __device__ __noinline__ void solve_warp(int o_K, int o_rdiag, int o_bx) {
 
 // ------------------------------------------------------------------ solve_kkt (pdipm.py:325-354)
 // Inputs (nullptr == zero vector): rx[n], rs[m], rz[m], ry[e]; outputs dx[n], ds[m], dz[m], dy[e].
-template <typename T, int CS, int NS>
-__device__ __forceinline__ void solve_kkt(const CPlan& P, CSmem<T>& S, const Struct& st, Prof& pf, const T* rx,
-                                          const T* rs, const T* rz, const T* ry, T* dx, T* ds, T* dz, T* dy,
-                                          bool trans = false) {
+// solve_kkt, factor_kkt and the phases of forward_scene are __noinline__: each one recomputes its addresses from
+// the kernel parameters, so that nothing but a few loop scalars is live across the factorisation and the
+// substitution (whose register budget is the whole 128 of two CTAs per SM). Spilled values would live in local
+// memory, and with ~220 KB of shared memory per SM the L1 left for it is too small: a reload is an L2 round trip.
+template <typename T, int CS, int NS, typename PF>
+__device__ __noinline__ void solve_kkt(const CPlan& P, CSmem<T> S, Struct st, PF& pf, const T* rx,
+                                       const T* rs, const T* rz, const T* ry, T* dx, T* ds, T* dz, T* dy,
+                                       bool trans = false) {
   const int nc_ = st.ncomp;                       // positions are slot-major: pos(c, r) = r * ncomp + c
   const int n = P.n, e = P.e, N = P.N, NP = P.NP, tid = threadIdx.x, pcap = P.pcap;
   const int npos = st.ncomp * CS;
@@ -984,8 +998,8 @@ __device__ __forceinline__ void solve_kkt(const CPlan& P, CSmem<T>& S, const Str
 }
 
 // d is in S.d(): W, K, LU
-template <typename T, int NS, int CS>
-__device__ __forceinline__ void factor_kkt(const CPlan& P, CSmem<T>& S, const Struct& st, Prof& pf, bool trans = false) {
+template <typename T, int NS, int CS, typename PF>
+__device__ __noinline__ void factor_kkt(const CPlan& P, CSmem<T> S, Struct st, PF& pf, bool trans = false) {
   comp_inverse<T, CS>(P, S, st);
   __syncthreads();
   pf.lap(CPH_WINV);
@@ -1084,36 +1098,134 @@ __device__ __forceinline__ bool load_structure(const CPlan& P, Struct& st, const
 }
 
 // ------------------------------------------------------------------ forward (pdipm.py:49-179), one scene
-template <typename T, int NS, int CS>
-__device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S, const Struct& st, Prof& pf, int sc) {
+// Residuals of the current iterate (:82-96) into rx, rz, ry; returns s.z and the residual norm of :92-96.
+template <typename T>
+struct SzResid { T sz, resid; };
+
+template <typename T, int CS>
+__device__ __noinline__ SzResid<T> fwd_residuals(const CFwdArgs<T>& a, CSmem<T> S, Struct st, int sc) {
   const int nc_ = st.ncomp;                       // positions are slot-major: pos(c, r) = r * ncomp + c
   const CPlan& P = a.P;
   const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x, pcap = P.pcap;      // m: this scene's rows (<= P.m, the stride)
   const T* p = a.p + (size_t)sc * n;
   const T* h = a.h + (size_t)sc * P.m;
   const T* b = e > 0 ? a.b + (size_t)sc * e : nullptr;
-  T* o_x = a.zhat + (size_t)sc * n;
-  T* o_z = a.lam + (size_t)sc * P.m;
-  T* o_s = a.slack + (size_t)sc * P.m;
-  T* o_y = e > 0 ? a.nu + (size_t)sc * e : nullptr;
-  const T NANV = nan("");
-
-  // ---- initial point: d = 1, rhs (p, 0, -h, -b)                 :58-63
-  for (int i = tid; i < m; i += NT) { S.d()[i] = T(1); S.rs2()[i] = T(0); S.rz()[i] = -h[i]; }
-  for (int i = tid; i < n; i += NT) S.rx()[i] = p[i];
-  for (int i = tid; i < e; i += NT) S.ry()[i] = -b[i];
+  for (int c = tid; c < n; c += NT) {                            // rx = G^T z + Q x + p (+ A^T y)
+    T acc = 0;
+    const int cnt = S.clcnt()[c];
+    for (int l = 0; l < cnt; ++l) {
+      const int cp = S.clist()[l * n + c], cc = cp >> 3, pp = cp & 7;
+#pragma unroll
+      for (int r = 0; r < CS; ++r) {
+        const int i = S.rows()[r * nc_ + cc];
+        if (i != 0xFFFF) acc = fma(S.Gd()[(size_t)pp * pcap + r * nc_ + cc], S.z()[i], acc);
+      }
+    }
+    for (int k = 0; k < e; ++k) acc = fma(S.As()[k * n + c], S.y()[k], acc);
+    S.rx()[c] = acc + S.qd()[c] * S.x()[c] + p[c];
+  }
+  for (int tt = tid; tt < (CS << st.sh); tt += NT) {              // rz = G x + s - h - F z
+    const int r = tt >> st.sh, c = tt & ((1 << st.sh) - 1);
+    if (c >= nc_) continue;
+    const int pz = r * nc_ + c;
+    const int i = S.rows()[pz];
+    if (i == 0xFFFF) continue;
+    const int nc = S.ncols()[c];
+    T acc = 0;
+    for (int q = 0; q < nc; ++q) acc = fma(S.Gd()[(size_t)q * pcap + pz], S.x()[S.ccols()[q * pcap + c]], acc);
+    T fz = 0;
+#pragma unroll
+    for (int q = 0; q < CS; ++q) {
+      const int j = S.rows()[q * nc_ + c];
+      if (j != 0xFFFF) fz = fma(S.Fd()[(size_t)(r * CS + q) * nc_ + c], S.z()[j], fz);
+    }
+    S.rz()[i] = acc + S.s()[i] - h[i] - fz;
+  }
+  for (int k = tid; k < e; k += NT) {                            // ry = A x - b
+    T acc = 0;
+    for (int j = 0; j < n; ++j) acc = fma(S.As()[k * n + j], S.x()[j], acc);
+    S.ry()[k] = acc - b[k];
+  }
   __syncthreads();
+  T q4[4] = {0, 0, 0, 0};                                        // s.z, |rz|^2, |ry|^2, |rx|^2
+  for (int i = tid; i < m; i += NT) { q4[0] += S.s()[i] * S.z()[i]; q4[1] += S.rz()[i] * S.rz()[i]; }
+  for (int i = tid; i < e; i += NT) q4[2] += S.ry()[i] * S.ry()[i];
+  for (int i = tid; i < n; i += NT) q4[3] += S.rx()[i] * S.rx()[i];
+  block_reduce<T, 4>(q4, OpSum(), T(0), S.red());
+  const T sz = q4[0];
+  const T mu = fabs(sz / T(m));                                  // :91
+  return {sz, (e > 0 ? sqrt(q4[2]) : T(0)) + sqrt(q4[1]) + sqrt(q4[3]) + T(m) * mu};   // :92-96
+}
+
+// the best iterate so far becomes the output (:107-136)
+template <typename T>
+__device__ __noinline__ void fwd_store_best(const CFwdArgs<T>& a, CSmem<T> S, int m, int sc) {
+  const CPlan& P = a.P;
+  const int n = P.n, e = P.e, tid = threadIdx.x;
+  for (int i = tid; i < n; i += NT) a.zhat[(size_t)sc * n + i] = S.x()[i];
+  for (int i = tid; i < m; i += NT) { a.lam[(size_t)sc * P.m + i] = S.z()[i]; a.slack[(size_t)sc * P.m + i] = S.s()[i]; }
+  for (int i = tid; i < e; i += NT) a.nu[(size_t)sc * e + i] = S.y()[i];
+}
+
+// affine step length and centering (:140-158): rs2 = (-mu sigma + ds dz) / s, the corrector's rs
+template <typename T>
+__device__ __noinline__ void fwd_centering(CSmem<T> S, int m, T mu, T sz) {
+  const int tid = threadIdx.x;
+  T stz, sts;
+  get_steps(S.z(), S.dz(), S.s(), S.ds(), m, S.red(), stz, sts);
+  const T alpha_aff = nan_min(nan_min(stz, sts), T(1));          // :142-144
+  T t3[1] = {0};
+  for (int i = tid; i < m; i += NT) t3[0] += (S.s()[i] + alpha_aff * S.ds()[i]) * (S.z()[i] + alpha_aff * S.dz()[i]);
+  block_reduce<T, 1>(t3, OpSum(), T(0), S.red());
+  const T ratio = t3[0] / sz;                                    // :146-150
+  const T sig = ratio * ratio * ratio;
+  const T musig = -mu * sig;                                     // :152-158
+  for (int i = tid; i < m; i += NT) S.rs2()[i] = (musig + S.ds()[i] * S.dz()[i]) / S.s()[i];
+  __syncthreads();
+}
+
+// affine + corrector direction and the step along it (:160-174); the corrector is in rx, rz (ds), rs2 (dz), ry
+template <typename T>
+__device__ __noinline__ void fwd_step(const CPlan& P, CSmem<T> S, int m) {
+  const int n = P.n, e = P.e, tid = threadIdx.x;
+  for (int i = tid; i < n; i += NT) S.dx()[i] += S.rx()[i];          // :160-163
+  for (int i = tid; i < m; i += NT) { S.ds()[i] += S.rz()[i]; S.dz()[i] += S.rs2()[i]; }
+  for (int i = tid; i < e; i += NT) S.dy()[i] += S.ry()[i];
+  __syncthreads();
+  T stz, sts;
+  get_steps(S.z(), S.dz(), S.s(), S.ds(), m, S.red(), stz, sts);
+  const T alpha = nan_min(T(0.999) * nan_min(stz, sts), T(1));   // :164-166
+  for (int i = tid; i < n; i += NT) S.x()[i] += alpha * S.dx()[i];   // :171-174
+  for (int i = tid; i < m; i += NT) { S.s()[i] += alpha * S.ds()[i]; S.z()[i] += alpha * S.dz()[i]; }
+  for (int i = tid; i < e; i += NT) S.y()[i] += alpha * S.dy()[i];
+  __syncthreads();
+}
+
+template <typename T, int NS, int CS, typename PF>
+__device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc) {
+  const CPlan& P = a.P;
+  const int m = st.m;                                            // this scene's rows (<= P.m, the stride)
+  {
+    const int n = P.n, e = P.e, tid = threadIdx.x;
+    const T* h = a.h + (size_t)sc * P.m;
+    const T* b = e > 0 ? a.b + (size_t)sc * e : nullptr;
+    // ---- initial point: d = 1, rhs (p, 0, -h, -b)                 :58-63
+    for (int i = tid; i < m; i += NT) { S.d()[i] = T(1); S.rs2()[i] = T(0); S.rz()[i] = -h[i]; }
+    for (int i = tid; i < n; i += NT) S.rx()[i] = a.p[(size_t)sc * n + i];
+    for (int i = tid; i < e; i += NT) S.ry()[i] = -b[i];
+    __syncthreads();
+  }
   factor_kkt<T, NS, CS>(P, S, st, pf);
-  solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), S.rz(), e > 0 ? S.ry() : nullptr, S.x(), S.s(), S.z(), S.y());
+  solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), S.rz(), P.e > 0 ? S.ry() : nullptr, S.x(), S.s(), S.z(), S.y());
   if (m == 0) {
     // engine path, a scene without contacts: no complementarity, the equality-constrained solve above is the
     // answer (engines.py:35-49 solves [[M, -Je^T], [Je, 0]] x = [M v + dt f; 0] directly in that case)
-    for (int i = tid; i < n; i += NT) o_x[i] = S.x()[i];
-    for (int i = tid; i < e; i += NT) o_y[i] = S.y()[i];
-    if (tid == 0) { a.status[sc] = 2; a.iters[sc] = 0; if (a.resid) a.resid[sc] = T(0); }
+    fwd_store_best<T>(a, S, 0, sc);
+    if (threadIdx.x == 0) { a.status[sc] = 2; a.iters[sc] = 0; if (a.resid) a.resid[sc] = T(0); }
     return;
   }
   {   // shift s and z to >= 1 where the row minimum is <= 0       :65-75
+    const int tid = threadIdx.x;
     T mn[2] = {INFINITY, INFINITY};
     for (int i = tid; i < m; i += NT) { mn[0] = nan_min(mn[0], S.s()[i]); mn[1] = nan_min(mn[1], S.z()[i]); }
     block_reduce<T, 2>(mn, OpMin(), (T)INFINITY, S.red());
@@ -1124,120 +1236,53 @@ __device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S,
     __syncthreads();
   }
 
-  T best = NANV;
+  T best = nan("");
   bool have_best = false;
   int not_improved = 0, status = 0, it = 0;
-  const int npos = st.ncomp * CS;
   for (it = 0; it < a.max_iter; ++it) {
-    // ---- residuals                                              :82-96
-    for (int c = tid; c < n; c += NT) {                            // rx = G^T z + Q x + p (+ A^T y)
-      T acc = 0;
-      const int cnt = S.clcnt()[c];
-      for (int l = 0; l < cnt; ++l) {
-        const int cp = S.clist()[l * n + c], cc = cp >> 3, pp = cp & 7;
-#pragma unroll
-        for (int r = 0; r < CS; ++r) {
-          const int i = S.rows()[r * nc_ + cc];
-          if (i != 0xFFFF) acc = fma(S.Gd()[(size_t)pp * pcap + r * nc_ + cc], S.z()[i], acc);
-        }
-      }
-      for (int k = 0; k < e; ++k) acc = fma(S.As()[k * n + c], S.y()[k], acc);
-      S.rx()[c] = acc + S.qd()[c] * S.x()[c] + p[c];
-    }
-    for (int tt = tid; tt < (CS << st.sh); tt += NT) {              // rz = G x + s - h - F z
-      const int r = tt >> st.sh, c = tt & ((1 << st.sh) - 1);
-      if (c >= nc_) continue;
-      const int pz = r * nc_ + c;
-      const int i = S.rows()[pz];
-      if (i == 0xFFFF) continue;
-      const int nc = S.ncols()[c];
-      T acc = 0;
-      for (int q = 0; q < nc; ++q) acc = fma(S.Gd()[(size_t)q * pcap + pz], S.x()[S.ccols()[q * pcap + c]], acc);
-      T fz = 0;
-#pragma unroll
-      for (int q = 0; q < CS; ++q) {
-        const int j = S.rows()[q * nc_ + c];
-        if (j != 0xFFFF) fz = fma(S.Fd()[(size_t)(r * CS + q) * nc_ + c], S.z()[j], fz);
-      }
-      S.rz()[i] = acc + S.s()[i] - h[i] - fz;
-    }
-    for (int k = tid; k < e; k += NT) {                            // ry = A x - b
-      T acc = 0;
-      for (int j = 0; j < n; ++j) acc = fma(S.As()[k * n + j], S.x()[j], acc);
-      S.ry()[k] = acc - b[k];
-    }
-    __syncthreads();
-    T q4[4] = {0, 0, 0, 0};                                        // s.z, |rz|^2, |ry|^2, |rx|^2
-    for (int i = tid; i < m; i += NT) { q4[0] += S.s()[i] * S.z()[i]; q4[1] += S.rz()[i] * S.rz()[i]; }
-    for (int i = tid; i < e; i += NT) q4[2] += S.ry()[i] * S.ry()[i];
-    for (int i = tid; i < n; i += NT) q4[3] += S.rx()[i] * S.rx()[i];
-    block_reduce<T, 4>(q4, OpSum(), T(0), S.red());
+    const SzResid<T> r = fwd_residuals<T, CS>(a, S, st, sc);
     pf.lap(CPH_RESID);
-    const T sz = q4[0];
-    const T mu = fabs(sz / T(m));                                  // :91
-    const T resid = (e > 0 ? sqrt(q4[2]) : T(0)) + sqrt(q4[1]) + sqrt(q4[3]) + T(m) * mu;   // :92-96
+    const T mu = fabs(r.sz / T(m));                                // :91
 
     // ---- best iterate / termination (per scene)                 :107-136
     // (the reference refactors before this test, :98-102; the factors of a terminating iteration
     // are never used, so the test comes first here)
     bool improved;
     if (!have_best) { improved = true; have_best = true; not_improved = 0; }
-    else { improved = resid < best; not_improved = improved ? 0 : not_improved + 1; }
+    else { improved = r.resid < best; not_improved = improved ? 0 : not_improved + 1; }
     if (improved) {
-      best = resid;
-      for (int i = tid; i < n; i += NT) o_x[i] = S.x()[i];
-      for (int i = tid; i < m; i += NT) { o_z[i] = S.z()[i]; o_s[i] = S.s()[i]; }
-      for (int i = tid; i < e; i += NT) o_y[i] = S.y()[i];
+      best = r.resid;
+      fwd_store_best<T>(a, S, m, sc);
     }
     if (not_improved == a.not_improved_lim) { status = 1; ++it; break; }
     if (best < a.eps) { status = 2; ++it; break; }
     if (mu > T(1e100)) { status = 3; ++it; break; }
 
-    for (int i = tid; i < m; i += NT) S.d()[i] = S.z()[i] / S.s()[i];     // :98
+    for (int i = threadIdx.x; i < m; i += NT) S.d()[i] = S.z()[i] / S.s()[i];     // :98
     __syncthreads();
     factor_kkt<T, NS, CS>(P, S, st, pf);                               // :100
 
     // ---- affine direction                                       :138-139   (rs = z)
-    solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.z(), S.rz(), e > 0 ? S.ry() : nullptr, S.dx(), S.ds(), S.dz(), S.dy());
-    T stz, sts;
-    get_steps(S.z(), S.dz(), S.s(), S.ds(), m, S.red(), stz, sts);
-    const T alpha_aff = nan_min(nan_min(stz, sts), T(1));          // :142-144
-    T t3[1] = {0};
-    for (int i = tid; i < m; i += NT) t3[0] += (S.s()[i] + alpha_aff * S.ds()[i]) * (S.z()[i] + alpha_aff * S.dz()[i]);
-    block_reduce<T, 1>(t3, OpSum(), T(0), S.red());
-    const T ratio = t3[0] / sz;                                    // :146-150
-    const T sig = ratio * ratio * ratio;
-    const T musig = -mu * sig;                                     // :152-158
-    for (int i = tid; i < m; i += NT) S.rs2()[i] = (musig + S.ds()[i] * S.dz()[i]) / S.s()[i];
-    __syncthreads();
+    solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.z(), S.rz(), P.e > 0 ? S.ry() : nullptr, S.dx(), S.ds(), S.dz(), S.dy());
+    fwd_centering<T>(S, m, mu, r.sz);
     pf.lap(CPH_STEP);
     // corrector: outputs land in rx / rz / ry (dead until the next residual phase)
     solve_kkt<T, CS, NS>(P, S, st, pf, nullptr, S.rs2(), nullptr, nullptr, S.rx(), S.rz(), S.rs2(), S.ry());
     // NOTE: ds_c -> S.rz(), dz_c -> S.rs2() (solve_kkt reads rs before it writes dz/ds of the same row)
-    for (int i = tid; i < n; i += NT) S.dx()[i] += S.rx()[i];          // :160-163
-    for (int i = tid; i < m; i += NT) { S.ds()[i] += S.rz()[i]; S.dz()[i] += S.rs2()[i]; }
-    for (int i = tid; i < e; i += NT) S.dy()[i] += S.ry()[i];
-    __syncthreads();
-    get_steps(S.z(), S.dz(), S.s(), S.ds(), m, S.red(), stz, sts);
-    const T alpha = nan_min(T(0.999) * nan_min(stz, sts), T(1));   // :164-166
-    for (int i = tid; i < n; i += NT) S.x()[i] += alpha * S.dx()[i];   // :171-174
-    for (int i = tid; i < m; i += NT) { S.s()[i] += alpha * S.ds()[i]; S.z()[i] += alpha * S.dz()[i]; }
-    for (int i = tid; i < e; i += NT) S.y()[i] += alpha * S.dy()[i];
-    __syncthreads();
+    fwd_step<T>(P, S, m);
     pf.lap(CPH_STEP);
   }
-  if (tid == 0) { a.status[sc] = status; a.iters[sc] = it; if (a.resid) a.resid[sc] = best; }
+  if (threadIdx.x == 0) { a.status[sc] = status; a.iters[sc] = it; if (a.resid) a.resid[sc] = best; }
 }
 
-template <typename T, int NS>
+template <typename T, int NS, bool PROF>
 __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_forward_kernel(const __grid_constant__ CFwdArgs<T> a) {
   const CPlan& P = a.P;
   CSmem<T> S(P);
   const int n = P.n, m = P.m, e = P.e, tid = threadIdx.x;
   __shared__ int singular_s;
   const T NANV = nan("");
-  Prof pf;
-  pf.p = a.prof ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr;
+  Prof<PROF> pf(PROF ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr);
   for (int sc = blockIdx.x; sc < a.B; sc += gridDim.x) {
     if (tid == 0) singular_s = 0;
     __syncthreads();
@@ -1311,8 +1356,8 @@ __device__ __forceinline__ void write_outer(T* __restrict__ o, int rows, int col
 }
 
 // ------------------------------------------------------------------ backward (lcp.py:37-64), one scene
-template <typename T, int NS, int CS>
-__device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S, const Struct& st, Prof& pf, int sc) {
+template <typename T, int NS, int CS, typename PF>
+__device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc) {
   const CPlan& P = a.P;
   const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x;
   const T* zh = a.zhat + (size_t)sc * n;
@@ -1449,14 +1494,13 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
   pf.lap(CPH_GRADS);
 }
 
-template <typename T, int NS>
+template <typename T, int NS, bool PROF>
 __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(const __grid_constant__ CBwdArgs<T> a) {
   const CPlan& P = a.P;
   CSmem<T> S(P);
   const int n = P.n, m = P.m, e = P.e, tid = threadIdx.x;
   __shared__ int singular_s;
-  Prof pf;
-  pf.p = a.prof ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr;
+  Prof<PROF> pf(PROF ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr);
   for (int sc = blockIdx.x; sc < a.B; sc += gridDim.x) {
     if (a.only && !a.only[sc]) continue;
     if (tid == 0) singular_s = 0;
