@@ -216,7 +216,9 @@ int lcpb200_assemble_backward(int dtype, int B, int nb, int nc, double dt,
  * equality-constrained solve of engines.py:35-49; lam / slack rows of scene s are laid out for ITS count
  * (normal rows [0,c), friction [c,3c), gamma [3c,4c)), the arrays keep the stride m.
  * lcpb200_engine_backward: the chain rule through the assembly applied to the factored gradients of
- * lcp.py:52-63 (dG = dlam (x) zhat + lam (x) dx, ...): gradients w.r.t. the contact list, any may be NULL. */
+ * lcp.py:52-63 (dG = dlam (x) zhat + lam (x) dx, ...): gradients w.r.t. the contact list, any may be NULL.
+ * flags: LCPB200_BWD_BUG_COMPATIBLE (the reference's gradients) or LCPB200_BWD_EXACT_ADJOINT (the true
+ * adjoint: the transposed KKT system), on both the condensed and the large-scene kernels. */
 int lcpb200_engine_forward(lcpb200_handle_t h, int B, int nb, int nc, int mode, double dt,
                            const void* mass, const void* inertia, const void* v, const void* fext,
                            const void* normal, const void* p1, const void* p2,

@@ -128,6 +128,7 @@ struct BBwdArgs {
   double* wsd;
   int* wsi;
   long long* prof;
+  unsigned flags;                 // LCPB200_BWD_*: bit 0 = exact adjoint (transposed KKT system: K^T, W^T)
 };
 
 #ifdef LCP_BAND_DEVICE        // device code: compiled by lcp_band_kernels.cu only
@@ -413,7 +414,11 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
 }
 
 // ------------------------------------------------------------------ W_c = (F_c + diag(1/d))^-1, E_c = Gd^T W Gd
-__device__ __forceinline__ void contact_blocks(const Ctx& c, int mode, const double* mu) {
+// trans (exact-adjoint backward, mode 0): the transposed system, F_c^T in place of F_c. Its block is
+// (F_c^T + diag(1/d))^-1 = W_c^T, so c.W receives W_c^T and E_c = Gd^T W_c^T Gd; the border ([A, 0] / [A^T; 0])
+// is symmetric, so the band, the ordering and the LU are those of K^T unchanged. Mode 1 has F = 0 (W is a scalar):
+// trans changes nothing there.
+__device__ __forceinline__ void contact_blocks(const Ctx& c, int mode, const double* mu, bool trans) {
   const int ncap = c.ncap;
   for (int k = threadIdx.x; k < c.nc; k += NT) {
     const double* g = c.cg + 12 * (size_t)k;
@@ -475,9 +480,10 @@ __device__ __forceinline__ void contact_blocks(const Ctx& c, int mode, const dou
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
-      for (int q = 0; q < 4; ++q) Wo[r * 4 + q] = M[r][q];
-    // rows of Gd: gn, gf, -gf, 0
-    const double wnn = M[0][0], wnf = M[0][1] - M[0][2], wfn = M[1][0] - M[2][0];
+      for (int q = 0; q < 4; ++q) Wo[r * 4 + q] = trans ? M[q][r] : M[r][q];
+    // rows of Gd: gn, gf, -gf, 0 (W^T swaps the two off-diagonal couplings)
+    const double mnf = M[0][1] - M[0][2], mfn = M[1][0] - M[2][0];
+    const double wnn = M[0][0], wnf = trans ? mfn : mnf, wfn = trans ? mnf : mfn;
     const double wff = M[1][1] - M[1][2] - M[2][1] + M[2][2];
 #pragma unroll
     for (int a = 0; a < 6; ++a) {
@@ -1153,8 +1159,9 @@ __device__ __noinline__ void solve_kkt(const Ctx& c, BProf& pf, const double* rx
   pf.lap(BPH_POST);
 }
 
-__device__ __forceinline__ void factor_kkt(const Ctx& c, BProf& pf, int mode, const double* mu) {
-  contact_blocks(c, mode, mu);
+// trans: factor K^T (exact-adjoint backward); the forward passes a constant false
+__device__ __forceinline__ void factor_kkt(const Ctx& c, BProf& pf, int mode, const double* mu, bool trans) {
+  contact_blocks(c, mode, mu, trans);
   __syncthreads();
   pf.lap(BPH_WINV);
   assemble_band(c);
@@ -1206,7 +1213,7 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
   for (int i = tid; i < n; i += NT) c.rx[i] = c.ps[i];
   for (int i = tid; i < e; i += NT) c.ry[i] = -b[i];
   __syncthreads();
-  factor_kkt(c, pf, mode, mu);
+  factor_kkt(c, pf, mode, mu, false);
   solve_kkt(c, pf, c.rx, c.rs, c.rz, e > 0 ? c.ry : nullptr, c.x, c.s, c.z, c.y);
   if (m == 0) {                                                             // no contacts: engines.py:35-49
     for (int i = tid; i < n; i += NT) o_x[i] = c.x[i];
@@ -1305,7 +1312,7 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
     for (int r = 0; r < cs; ++r)
       for (int k = tid; k < nc; k += NT) { const int i = r * ncap + k; c.d[i] = c.z[i] / c.s[i]; }     // :98
     __syncthreads();
-    factor_kkt(c, pf, mode, mu);                                            // :100
+    factor_kkt(c, pf, mode, mu, false);                                     // :100
     // ---- affine direction                                       :138-139   (rs = z)
     solve_kkt(c, pf, c.rx, c.z, c.rz, e > 0 ? c.ry : nullptr, c.dx, c.ds, c.dz, c.dy);
     double stz, sts;
@@ -1392,7 +1399,8 @@ __global__ void __launch_bounds__(NT, 1) band_forward_kernel(const __grid_consta
 // One factorisation at d = lam / slack (clamped to [1e-10, 1e10] like the condensed fp64 backward, DESIGN.md
 // section 3.1), one solve with the right-hand side (dl/dzhat, 0, 0, 0), then the chain rule through the assembly
 // (world.py:144-234, engines.py:50-116) applied to the factored gradients of lcp.py:52-63 -- evaluated only at
-// the entries the assembly writes (same formulas as lcp_condensed.cuh's engine path; bug-compatible adjoint).
+// the entries the assembly writes (same formulas as lcp_condensed.cuh's engine path). flags bit 0 (exact adjoint)
+// factors and solves the transposed system K^T instead (DESIGN.md section 3.4); the chain rule is the same.
 __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf& pf, int sc) {
   const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, cs = c.cs, ncap = c.ncap, nb = c.nb;
   const cnd::EngineSoA<double>& E = a.soa;
@@ -1411,8 +1419,8 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
     }
   for (int i = tid; i < e; i += NT) c.y[i] = a.nu[(size_t)sc * e + i];
   __syncthreads();
-  factor_kkt(c, pf, mode, mu);                                              // :46
-  solve_kkt(c, pf, c.rx, c.rs, nullptr, nullptr, c.dx, c.ds, c.dz, c.dy);   // :47-50
+  factor_kkt(c, pf, mode, mu, (a.flags & 1u) != 0);                         // :46
+  solve_kkt(c, pf, c.rx, c.rs, nullptr, nullptr, c.dx, c.ds, c.dz, c.dy);   // :47-50 (c.W holds W^T when exact)
   const double* dx = c.dx;
   const double* dlam = c.dz;
   const double* lm = c.z;

@@ -865,7 +865,6 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   if (use_banded(h)) {
-    if (flags != LCPB200_BWD_BUG_COMPATIBLE) return fail("engine_backward: the large-scene kernel implements the bug-compatible adjoint only");
     if (int rc = ensure_bplan(h, B, nb, nc, mode)) return rc;
     bnd::BBwdArgs a;
     a.P = h->bplan;
@@ -884,6 +883,7 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
     a.drest = (double*)drestitution; a.dA = (double*)dA; a.db = (double*)db;
     a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
     a.prof = h->cprof;
+    a.flags = flags;
     CK(bnd::launch_band_backward(a, std::min(B, h->num_sms), st));
     return 0;
   }

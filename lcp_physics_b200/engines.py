@@ -173,13 +173,25 @@ def engine_solve(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2,
 class B200PdipmEngine(Engine):
     """Engine that solves the contact LCP with the CUDA PDIPM kernels (mirror of engines.py:17-116)."""
 
-    def __init__(self, max_iter=10, fused=True):
+    def __init__(self, max_iter=10, fused=True, exact_adjoint=False):
         # fused: contact list -> solution in one kernel (lcpb200_engine_forward); False (or an unsupported
-        # topology / size) assembles the dense LCP on the GPU and calls LCPFunction, like the reference
+        # topology / size) assembles the dense LCP on the GPU and calls LCPFunction, like the reference.
+        # exact_adjoint: gradients through the transposed KKT system (the true adjoint, DESIGN.md section 3.4)
+        # on both paths; False reproduces the reference's gradients, which are biased whenever friction is on.
         self.fused = fused
         self.lcp_solver = LCPFunction
         self.cached_inverse = None
         self.max_iter = max_iter
+        self.exact_adjoint = exact_adjoint
+
+    def _dense_solver(self, **kw):
+        """`self.lcp_solver(**kw)`, with exact_adjoint passed on; a replaced solver cannot honour it."""
+        if not self.exact_adjoint:
+            return self.lcp_solver(**kw)
+        if self.lcp_solver is not LCPFunction:
+            raise ValueError("B200PdipmEngine(exact_adjoint=True) needs lcp_solver = lcp_physics_b200.LCPFunction; "
+                             "%r would return the reference's gradients" % (self.lcp_solver,))
+        return self.lcp_solver(exact_adjoint=True, **kw)
 
     # ------------------------------------------------------------------ helpers
     @staticmethod
@@ -248,7 +260,7 @@ class B200PdipmEngine(Engine):
             A = b = None
         x, status = engine_solve(Mb[:, 1].unsqueeze(0).to(dev), Mb[:, 0].unsqueeze(0).to(dev), v.unsqueeze(0).to(dev),
                                  fext.unsqueeze(0).to(dev), normal, p1, p2, mu, rest, b1, b2, dt, A=A, b=b, mode=mode,
-                                 max_iter=max_iter)
+                                 max_iter=max_iter, exact_adjoint=self.exact_adjoint)
         st = int(status[0])
         if st == _lib.STATUS_SINGULAR_Q:
             from .lcp import SINGULAR_Q_MSG
@@ -292,7 +304,7 @@ class B200PdipmEngine(Engine):
         else:
             A = torch.tensor([], dtype=Q.dtype, device=dev)       # engines.py:59-60
             b = torch.tensor([], dtype=Q.dtype, device=dev)
-        x = -self.lcp_solver(max_iter=self.max_iter, verbose=-1)(Q, p, G, h, A, b, F)      # engines.py:76
+        x = -self._dense_solver(max_iter=self.max_iter, verbose=-1)(Q, p, G, h, A, b, F)   # engines.py:76
         new_v = x[:, :world.vec_len * len(world.bodies)].squeeze(0)
         return new_v.to(v0.device)
 
@@ -332,5 +344,5 @@ class B200PdipmEngine(Engine):
             A = torch.tensor([], dtype=Q.dtype, device=dev)
             b = torch.tensor([], dtype=Q.dtype, device=dev)
         Fz = Q.new_zeros(1, nc, nc)
-        x = self.lcp_solver()(Q, hvec, Jc.contiguous(), gc, A, b, Fz)      # engines.py:114 (default max_iter)
+        x = self._dense_solver()(Q, hvec, Jc.contiguous(), gc, A, b, Fz)   # engines.py:114 (default max_iter)
         return (-x).to(v.device)                                   # [1, n]; the caller squeezes (world.py:111)

@@ -36,11 +36,13 @@ from .engines import engine_solve
 class BatchedWorld:
     def __init__(self, pos, rad, vel=None, mass=1.0, restitution=0.5, fric_coeff=0.9, gravity=10.0,
                  static=(), gravity_mask=None, dt=1.0 / 30, eps=0.1, tol=1e-6, post_stab=False,
-                 strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None):
+                 strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False):
         """pos [B,nb,2], rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass / restitution /
         fric_coeff [B,nb] (or broadcastable), `static`: indices of bodies pinned by a TotalConstraint,
         `gravity`: g of the `Gravity` force (forces.py) applied to the bodies in gravity_mask
-        (default: every non-static body)."""
+        (default: every non-static body). `exact_adjoint`: backward() through every LCP solve uses the true
+        adjoint (the transposed KKT system, DESIGN.md section 3.4); the default False reproduces the reference's
+        gradients, which are biased for every step with friction. Forward results do not depend on it."""
         _lib.require_cuda()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         pos = torch.as_tensor(pos)
@@ -74,6 +76,7 @@ class BatchedWorld:
             self.A = None
         self.dt, self.eps, self.tol = float(dt), float(eps), float(tol)
         self.post_stab, self.strict_no_pen, self.max_iter = post_stab, strict_no_penetration, max_iter
+        self.exact_adjoint = bool(exact_adjoint)
         ii, jj = torch.triu_indices(nb, nb, 1)
         self.pi, self.pj = ii.to(self.device), jj.to(self.device)                   # pair (i, j), i < j, lexicographic
         self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), 3 * nb)
@@ -157,7 +160,8 @@ class BatchedWorld:
     def _lcp(self, mode, dt, b):
         z, status = engine_solve(self.mass, self.inertia, self.v, self.fext, self.c_normal, self.c_p1, self.c_p2,
                                  self.c_mu, self.c_rest, self.c_b1, self.c_b2, dt, A=self.A, b=b, mode=mode,
-                                 max_iter=self.max_iter if mode == 0 else 10, counts=self.counts)
+                                 max_iter=self.max_iter if mode == 0 else 10, exact_adjoint=self.exact_adjoint,
+                                 counts=self.counts)
         if bool((status == _lib.STATUS_SINGULAR_Q).any()):
             from .lcp import SINGULAR_Q_MSG
             raise RuntimeError(SINGULAR_Q_MSG)
