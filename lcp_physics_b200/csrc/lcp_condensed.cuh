@@ -47,6 +47,9 @@ constexpr int UC = 8;            // max distinct columns of G over the rows of o
 constexpr int CSMAX = 6;         // max rows per component of F
 constexpr int KS = 8;            // scan slots per row of F / G
 constexpr int LMAX = 16;         // max (component, slot) entries per column of G
+constexpr int LU_BW = 2;         // block band (16 x 16 blocks) of the band LU, factor_K_body<NS, LU_BW>
+constexpr int MISC_BAND_LU = 4;  // S.misc() slot set by mark_band_lu: 1 = factor this scene's K with the band LU
+constexpr int CFLAG_DENSE_LU = 4;          // CPlan::flags bit: dense LU for every scene (the reference the tests compare the band LU against)
 constexpr int STATUS_UNSUPPORTED = -100;   // internal: scene left to the dual-form kernel
 
 // ------------------------------------------------------------------ launch plan / shared layout
@@ -57,7 +60,8 @@ struct CPlan {
   int wcap;                   // capacity (elements) of W and Fd
   int smem_bytes;
   int ctas_per_sm;
-  int flags;                  // experiment switches (LCPB200_COND_FLAGS): 1 = 1/d in fp64, 2 = rz - rs/d in fp64
+  int flags;                  // experiment switches (LCPB200_COND_FLAGS): 1 = 1/d in fp64, 2 = rz - rs/d in fp64,
+                              // 4 = dense LU for every scene (CFLAG_DENSE_LU)
   int sbytes;                 // bytes of one scene's saved structure (save_structure / load_structure)
   // byte offsets into the dynamic shared memory (filled by carve_plan)
   int o_K, o_W, o_scr, o_bx, o_rdiag, o_Fd, o_Gd, o_As, o_x, o_rx, o_dx, o_qd, o_y, o_ry, o_dy,
@@ -530,6 +534,23 @@ __device__ __noinline__ bool build_structure_soa(const CPlan& P, CSmem<T>& S, St
   return true;
 }
 
+// Which LU factors this scene's K (factor_kkt). Block (i, j) of K = Q + G^T W G (16 x 16 blocks) is non-zero only
+// when one component of G has columns in both blocks, so the block band of K is the widest spread of a component's
+// sorted column list, and an LU without pivoting keeps it. Equality rows border K with A, which couples every
+// block: such scenes take the dense LU, as do all scenes under CFLAG_DENSE_LU. Called by the whole CTA once the
+// column lists are in shared memory; thread 0 writes the answer, the barrier before the scene's first
+// factorisation publishes it.
+template <typename T>
+__device__ __noinline__ void mark_band_lu(const CPlan& P, CSmem<T> S, Struct st) {
+  int wide = P.e > 0 || (P.flags & CFLAG_DENSE_LU);
+  for (int c = threadIdx.x; c < st.ncomp; c += NT) {
+    const int nc = S.ncols()[c];
+    if (nc > 0 && (S.ccols()[(nc - 1) * P.pcap + c] >> 4) - (S.ccols()[c] >> 4) > LU_BW) wide = 1;
+  }
+  wide = __syncthreads_or(wide);
+  if (threadIdx.x == 0) S.misc()[MISC_BAND_LU] = !wide;
+}
+
 __device__ __forceinline__ double rcp64_fast(double x) {
   // MUFU.RCP64H seed (>= 20 bits) + 2 Newton steps; exact division outside the seed's range
   double r;
@@ -688,16 +709,35 @@ __device__ __forceinline__ void assemble_K(const CPlan& P, CSmem<T>& S, const St
 // quasi-definite; zero pivots produce inf/nan exactly like the reference's LU would.
 // The loop is bound by the FP64 pipe (16 lanes / SMSP): masks are applied only in the diagonal
 // block's slots, and the two column passes keep the live registers under the 128 of 2 CTAs / SM.
-template <int NS, int B0>
-__device__ __forceinline__ void lu_phase(double (&a)[NS][NS], int o_buf, int o_rdiag, int& step, int ti, int tj) {
+//
+// Block band BW < NS - 1: the thread holds only the blocks with |r - c| <= BW, and phase B0 loads and
+// updates only blocks r, c in [B0, B0 + BW]. That is exact for a K whose non-zero blocks lie in the
+// band (mark_band_lu): without pivoting, the pivot rows and columns of phase B0 are zero beyond block
+// B0 + BW, so there the dense form adds products of a zero and a finite value, which leave every entry
+// as it was (K holds no -0). The entries that are computed see the same operations in the same order as
+// in the dense form: the factors are bitwise the same unless a pivot is zero or not finite.
+template <int NS, int BW>
+struct LuBand {
+  static constexpr bool DENSE = BW >= NS - 1;
+  static constexpr int W = DENSE ? NS : 2 * BW + 1;             // block columns held per block row
+  static __device__ __forceinline__ constexpr bool in(int r, int c) { return DENSE || (r - c <= BW && c - r <= BW); }
+  static __device__ __forceinline__ constexpr int col(int r, int c) { return DENSE ? c : c - r + BW; }   // slot of block (r, c)
+  static __host__ __device__ constexpr int end(int b0) { return DENSE || b0 + BW + 1 > NS ? NS : b0 + BW + 1; }   // phase b0: [b0, end)
+};
+
+template <int NS, int BW, int B0>
+__device__ __forceinline__ void lu_phase(double (&a)[NS][LuBand<NS, BW>::W], int o_buf, int o_rdiag, int& step, int ti,
+                                         int tj) {
   // Entries keep the value they had when their column became the pivot column: after the last
   // phase a[i][j] (i > j) = u_jj L[i][j] and a[i][j] (i <= j) = U[i][j]; factor_K scales by 1/u_jj.
   // With that convention a step is ONE masked rank-2 update, a -= m0 (x) w0 + m1 (x) w1, with
   //   m0_i = [i > k] a_ik / a_kk,             w0_j = [j > k] a_kj,
   //   m1_i = [i > k+1] (a_i,k+1 - m0_i a_k,k+1) / a'_k+1,k+1,   w1_j = [j > k+1] (a_k+1,j - l10 a_kj),
   // and the masks only matter inside the diagonal block (r == B0 / c == B0).
+  using Bd = LuBand<NS, BW>;
   constexpr int NP = 16 * NS;
-  constexpr int L = NS - B0;                          // live block rows / columns
+  constexpr int E = Bd::end(B0);
+  constexpr int L = E - B0;                           // live block rows / columns
   constexpr int CW = (L <= 4) ? L : 3;                // columns per pass (bounds the live registers)
   double* const rdiag = reinterpret_cast<double*>(cnd_smem + o_rdiag);
 #pragma unroll 1
@@ -711,12 +751,12 @@ __device__ __forceinline__ void lu_phase(double (&a)[NS][NS], int o_buf, int o_r
       if ((unsigned)sr < 2u) {                        // I hold part of pivot row k (sr = 0) or k+1 (sr = 1)
         double* dst = reinterpret_cast<double*>(U2) + sr;
 #pragma unroll
-        for (int c = B0; c < NS; ++c) dst[2 * (16 * c + tj)] = a[B0][c];
+        for (int c = B0; c < E; ++c) dst[2 * (16 * c + tj)] = a[B0][Bd::col(B0, c)];
       }
       if ((unsigned)sc < 2u) {                        // ... of pivot column k / k+1
         double* dst = reinterpret_cast<double*>(C2) + sc;
 #pragma unroll
-        for (int r = B0; r < NS; ++r) dst[2 * (16 * r + ti)] = a[r][B0];
+        for (int r = B0; r < E; ++r) dst[2 * (16 * r + ti)] = a[r][Bd::col(r, B0)];
       }
     }
     __syncthreads();
@@ -728,12 +768,12 @@ __device__ __forceinline__ void lu_phase(double (&a)[NS][NS], int o_buf, int o_r
     const double l10 = pk.y * r0;
     if ((ti | tj) == 0) { rdiag[k] = r0; rdiag[k + 1] = r1; }
 #pragma unroll
-    for (int cg = B0; cg < NS; cg += CW) {
+    for (int cg = B0; cg < E; cg += CW) {
       double w0[CW], w1[CW];                          // pivot rows restricted to this pass's columns
 #pragma unroll
       for (int q = 0; q < CW; ++q) {
         const int c = cg + q;
-        if (c < NS) {
+        if (c < E) {
           const double2 u = U2[16 * c + tj];
           const double x1 = fma(-l10, u.x, u.y);
           w0[q] = (c == B0 && !(tj > kk)) ? 0.0 : u.x;
@@ -741,7 +781,7 @@ __device__ __forceinline__ void lu_phase(double (&a)[NS][NS], int o_buf, int o_r
         }
       }
 #pragma unroll
-      for (int r = B0; r < NS; ++r) {
+      for (int r = B0; r < E; ++r) {
         const double2 cc = C2[16 * r + ti];
         double m0 = cc.x * r0;
         double m1 = fma(-m0, p01, cc.y) * r1;
@@ -752,23 +792,24 @@ __device__ __forceinline__ void lu_phase(double (&a)[NS][NS], int o_buf, int o_r
 #pragma unroll
         for (int q = 0; q < CW; ++q) {
           const int c = cg + q;
-          if (c < NS) a[r][c] = fma(-m1, w1[q], fma(-m0, w0[q], a[r][c]));
+          if (c < E) a[r][Bd::col(r, c)] = fma(-m1, w1[q], fma(-m0, w0[q], a[r][Bd::col(r, c)]));
         }
       }
     }
   }
 }
 
-template <int NS, int B0>
+template <int NS, int BW, int B0>
 struct LuPhases {
-  static __device__ __forceinline__ void run(double (&a)[NS][NS], int o_buf, int o_rdiag, int& step, int ti, int tj) {
-    lu_phase<NS, B0>(a, o_buf, o_rdiag, step, ti, tj);
-    LuPhases<NS, B0 + 1>::run(a, o_buf, o_rdiag, step, ti, tj);
+  static __device__ __forceinline__ void run(double (&a)[NS][LuBand<NS, BW>::W], int o_buf, int o_rdiag, int& step, int ti,
+                                             int tj) {
+    lu_phase<NS, BW, B0>(a, o_buf, o_rdiag, step, ti, tj);
+    LuPhases<NS, BW, B0 + 1>::run(a, o_buf, o_rdiag, step, ti, tj);
   }
 };
-template <int NS>
-struct LuPhases<NS, NS> {
-  static __device__ __forceinline__ void run(double (&)[NS][NS], int, int, int&, int, int) {}
+template <int NS, int BW>
+struct LuPhases<NS, BW, NS> {
+  static __device__ __forceinline__ void run(double (&)[NS][LuBand<NS, BW>::W], int, int, int&, int, int) {}
 };
 
 // Layout of the factors for the substitution warp (solve_warp): lane l owns rows QN*l + q', round
@@ -784,22 +825,25 @@ template <int NS> struct SolveLayout {
 };
 
 // K (shared, column major) -> registers -> LU -> factors back to the K region in the solve layout.
-template <int NS>
-__device__ __noinline__ void factor_K(int o_K, int o_rdiag, bool trans) {
+// BW = NS - 1: dense; BW < NS - 1: only the block band |r - c| <= BW of K is non-zero (LuBand).
+template <int NS, int BW>
+__device__ __forceinline__ void factor_K_body(int o_K, int o_rdiag, bool trans) {
+  using Bd = LuBand<NS, BW>;
   constexpr int NP = 16 * NS, QN = SolveLayout<NS>::QN;
   int tid_;                                          // read %tid.x once (opaque to the compiler: no re-reads in the loops)
   asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid_));
   const int ti = tid_ & 15, tj = tid_ >> 4;
   double* const K = reinterpret_cast<double*>(cnd_smem + o_K);
   double* const rdiag = reinterpret_cast<double*>(cnd_smem + o_rdiag);
-  double a[NS][NS];
+  double a[NS][Bd::W];
 #pragma unroll
   for (int c = 0; c < NS; ++c)
 #pragma unroll
-    for (int r = 0; r < NS; ++r) a[r][c] = K[(size_t)(16 * c + tj) * NP + 16 * r + ti];
+    for (int r = 0; r < NS; ++r)
+      if (Bd::in(r, c)) a[r][Bd::col(r, c)] = K[(size_t)(16 * c + tj) * NP + 16 * r + ti];
   __syncthreads();                                   // K region becomes the broadcast buffer
   int step = 0;
-  LuPhases<NS, 0>::run(a, o_K, o_rdiag, step, ti, tj);
+  LuPhases<NS, BW, 0>::run(a, o_K, o_rdiag, step, ti, tj);
   __syncthreads();                                   // rdiag complete, broadcast buffers dead
   // trans (exact-adjoint backward): K^T = U^T L^T = L' U' with L'[i][k] = U[k][i] / u_kk and
   // U'[i][k] / u'_kk = u_ii L[k][i] / u_kk, i.e. entry (i, k) of the solve layout receives a[k][i] / u_kk:
@@ -820,10 +864,26 @@ __device__ __noinline__ void factor_K(int o_K, int o_rdiag, bool trans) {
 #pragma unroll
     for (int r = 0; r < NS; ++r) {
       const int i = 16 * r + ti;
-      K[colpart + rowpart[r]] = (i != j) ? a[r][c] * (trans ? rrow[r] : rj) : a[r][c];
+      // out of the band the dense LU leaves +0 and scales it like any other entry: write the same product
+      // (the region still holds K there)
+      const double v = Bd::in(r, c) ? a[r][Bd::col(r, c)] : 0.0;
+      K[colpart + rowpart[r]] = (i != j) ? v * (trans ? rrow[r] : rj) : v;
     }
   }
   __syncthreads();
+}
+
+// One call target for both LU variants: with two, ptxas saved more of the callers' registers around the dense LU
+// (double, NS = 6 forward: 16 / 40 B of spills in the dense LU became 48 / 88 B).
+template <int NS>
+__device__ __noinline__ void factor_K(int o_K, int o_rdiag, bool trans, bool band) {
+  if constexpr (LU_BW < NS - 1) {
+    if (band) {
+      factor_K_body<NS, LU_BW>(o_K, o_rdiag, trans);
+      return;
+    }
+  }
+  factor_K_body<NS, NS - 1>(o_K, o_rdiag, trans);
 }
 
 // ------------------------------------------------------------------ triangular solves (ONE warp)
@@ -1005,7 +1065,8 @@ __device__ __noinline__ void factor_kkt(const CPlan& P, CSmem<T> S, Struct st, P
   pf.lap(CPH_WINV);
   assemble_K<T, NS, CS>(P, S, st);
   pf.lap(CPH_ASSEMBLE);
-  factor_K<NS>(P.o_K, P.o_rdiag, trans);
+  if constexpr (LU_BW < NS - 1) factor_K<NS>(P.o_K, P.o_rdiag, trans, S.misc()[MISC_BAND_LU] != 0);
+  else factor_K<NS>(P.o_K, P.o_rdiag, trans, false);
   pf.lap(CPH_LU);
 }
 
@@ -1307,6 +1368,7 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_forward_kernel(con
       __syncthreads();
       continue;
     }
+    if constexpr (LU_BW < NS - 1) mark_band_lu<T>(P, S, st);
     switch (st.cs) {
       case 1: forward_scene<T, NS, 1>(a, S, st, pf, sc); break;
       case 2: forward_scene<T, NS, 2>(a, S, st, pf, sc); break;
@@ -1520,6 +1582,7 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
       __syncthreads();
       continue;
     }
+    if constexpr (LU_BW < NS - 1) mark_band_lu<T>(P, S, st);   // also after load_structure: the saved column lists give the same answer
     switch (st.cs) {
       case 1: backward_scene<T, NS, 1>(a, S, st, pf, sc); break;
       case 2: backward_scene<T, NS, 2>(a, S, st, pf, sc); break;
