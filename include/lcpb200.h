@@ -166,6 +166,31 @@ int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const void* pos,
                              const int32_t* body2, const int32_t* counts, void* normal, void* p1, void* p2,
                              void* penetration, void* mu, void* restitution_c, void* stream);
 
+/* Contact detection and geometry for B scenes of nb circles and no static convex polygon obstacles (walls, floors,
+ * ramps: no degrees of freedom). The pairs of the body list [circles 0..nb-1, obstacles nb..nb+no-1] are visited in
+ * lexicographic order -- circle-circle pairs (i, j) and circle-obstacle pairs (i, nb + k) -- which is the contact
+ * order of a reference World whose bodies are [circles..., obstacles...]; obstacles never pair with each other.
+ * Circle-circle pairs use the rule of lcpb200_find_contacts / lcpb200_contact_geometry (this call with no == 0 is
+ * exactly those two). Circle-obstacle pairs use the circle-hull rule of physics/contacts.py:84-144 with the exact
+ * closest point: centre outside, contact iff |c - q| - r <= eps (q the closest point of the polygon), normal =
+ * (c - q) / |c - q|, p1 = q - c, p2 = q - oref, penetration = r - |c - q|; centre inside, the edge of largest
+ * separation sep (outward unit normal n): normal = n, p1 = -n sep, p2 = c + p1 - oref, penetration = r - sep.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb] fric[B,nb] rest[B,nb]   circles (fric / rest: only for the geometry)
+ *   verts[B,no,nv,2]                               world-frame vertices of every obstacle (convex, either orientation)
+ *   oref[B,no,2] ofric[B,no] orest[B,no]           obstacles' reference points (p2 is relative to it), friction and
+ *                                                  restitution (only for the geometry)
+ *   body1[B,cap] body2[B,cap] counts[B]            OUT: as lcpb200_find_contacts; body2 >= nb names obstacle
+ *                                                  body2 - nb, the one-body contacts of lcpb200_engine_forward
+ *   normal[B,cap,2] p1 p2 penetration[B,cap] mu restitution_c[B,cap]
+ *                                                  OUT, all NULL (detection only) or all non-NULL: geometry and
+ *                                                  material (means of the two bodies') of the selected pairs. */
+int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, double eps, const void* pos,
+                           const void* rad, const void* fric, const void* rest, const void* verts, const void* oref,
+                           const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
+                           void* normal, void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
+                           void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:
@@ -210,6 +235,11 @@ int lcpb200_assemble_backward(int dtype, int B, int nb, int nc, double dt,
  * cannot take (a contact of a body with itself, > 16 contacts on one body for the condensed kernels, a band or
  * border beyond the limits above) gets status -100 and no result: assemble it with lcpb200_assemble and call
  * lcpb200_forward.
+ * Static obstacles: body2[c] >= nb names a body without degrees of freedom (a wall, floor or ramp: the static
+ * polygons of lcpb200_world_contacts). Contact c is then a ONE-BODY contact: its rows of G touch body1's three
+ * columns only, exactly the reference's formulation with the obstacle pinned by a TotalConstraint, reduced by the
+ * pinned dofs. p2 is not used by such a contact and its dp2 gradient is zero. body1 must be < nb; body1 == body2, a
+ * negative index or a body1 >= nb gets status -100.
  * contact_count == NULL: every scene has the nc contacts body1[nc], body2[nc] (one topology for the batch).
  * contact_count[B] != NULL (batched worlds): scene s uses its first contact_count[s] <= nc contacts, body1 /
  * body2 are [B,nc] and all per-contact arrays are strided by nc; a scene with 0 contacts gets the

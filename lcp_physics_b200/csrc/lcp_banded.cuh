@@ -198,17 +198,23 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
     if (!(q != 0.0 && isfinite(q))) bad |= 2;
     c.ps[j] = E_.mode == 0 ? q * v[j] + E_.dt * E_.fext[(size_t)sc * n + j] : 0.0;   // engines.py:32 / :109
   }
-  for (int bq = tid; bq < nb; bq += NT) { c.deg[bq] = 0; mark[bq] = 0; }
+  // queue[] (idle until the BFS) counts each body's one-body contacts: contacts with a static obstacle (body2 >= nb,
+  // no dofs). They touch only body1's diagonal block, so they neither join the BFS graph nor send a body to the border.
+  int* const nobst = queue;
+  for (int bq = tid; bq < nb; bq += NT) { c.deg[bq] = 0; mark[bq] = 0; nobst[bq] = 0; }
   __syncthreads();
   for (int k = tid; k < nc; k += NT) {
     const int b1 = c.b1[k], b2 = c.b2[k];
-    if (b1 == b2 || b1 < 0 || b2 < 0 || b1 >= nb || b2 >= nb) { bad |= 1; continue; }
+    if (b1 == b2 || b1 < 0 || b2 < 0 || b1 >= nb) { bad |= 1; continue; }
+    const bool two = b2 < nb;
     const double nx = normal[2 * k], ny = normal[2 * k + 1];
     const double p1x = p1[2 * k], p1y = p1[2 * k + 1], p2x = p2[2 * k], p2y = p2[2 * k + 1];
     double r1[3], r2[3];
     cnd::contact_row<double>(p1x, p1y, p2x, p2y, nx, ny, r1, r2);           // Jc row (world.py:172-184)
+    if (!two) r2[0] = r2[1] = r2[2] = 0.0;
+    const double v20 = two ? v[3 * b2] : 0.0, v21 = two ? v[3 * b2 + 1] : 0.0, v22 = two ? v[3 * b2 + 2] : 0.0;
     const double jv = r1[0] * v[3 * b1] + r1[1] * v[3 * b1 + 1] + r1[2] * v[3 * b1 + 2] +
-                      r2[0] * v[3 * b2] + r2[1] * v[3 * b2 + 1] + r2[2] * v[3 * b2 + 2];
+                      r2[0] * v20 + r2[1] * v21 + r2[2] * v22;
     const double rc = E_.rest[(size_t)sc * ncs + k];
     double* g = c.cg + 12 * (size_t)k;
 #pragma unroll
@@ -216,6 +222,7 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
     if (E_.mode == 0) {
       c.h[k] = jv * rc;                                                     // engines.py:53,74
       cnd::contact_row<double>(p1x, p1y, p2x, p2y, ny, -nx, r1, r2);        // Jf rows: +- left_orthogonal(n)
+      if (!two) r2[0] = r2[1] = r2[2] = 0.0;
 #pragma unroll
       for (int q = 0; q < 3; ++q) { g[6 + q] = r1[q]; g[9 + q] = r2[q]; }
       c.h[c.ncap + k] = 0.0; c.h[2 * c.ncap + k] = 0.0; c.h[3 * c.ncap + k] = 0.0;
@@ -223,7 +230,8 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
       c.h[k] = jv + jv * -rc;                                               // engines.py:90
     }
     atomicAdd(&c.deg[b1], 1);
-    atomicAdd(&c.deg[b2], 1);
+    if (two) atomicAdd(&c.deg[b2], 1);
+    else atomicAdd(&nobst[b1], 1);
   }
   // bodies pinned by an equality row go to the border
   for (int t = tid; t < e * n; t += NT)
@@ -242,7 +250,7 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
       for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(FULL, incl, o); if (lane >= o) incl += u; }
       if (bq < nb) { c.start[bq] = run + incl - dg; startS[bq] = run + incl - dg; }
       run += __shfl_sync(FULL, incl, 31);
-      const bool isb = bq < nb && (mark[bq] != 0 || dg > DEGB);
+      const bool isb = bq < nb && (mark[bq] != 0 || dg - nobst[bq] > DEGB);
       const unsigned bl = __ballot_sync(FULL, isb);
       if (isb) c.rank[bq] = -1 - (nbb + __popc(bl & ((1u << lane) - 1)));
       else if (bq < nb) c.rank[bq] = 0x7fffffff;                            // not placed yet
@@ -258,7 +266,7 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
   for (int k = tid; k < nc; k += NT) {
     const int b1 = c.b1[k], b2 = c.b2[k];
     c.adj[c.start[b1] + atomicAdd(&c.deg[b1], 1)] = 2 * k;
-    c.adj[c.start[b2] + atomicAdd(&c.deg[b2], 1)] = 2 * k + 1;
+    if (b2 < nb) c.adj[c.start[b2] + atomicAdd(&c.deg[b2], 1)] = 2 * k + 1;
   }
   __syncthreads();
   // sort every list by contact index (deterministic gather order): short lists by one thread, long ones by rank
@@ -292,7 +300,10 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
   // neighbour lists (body ids) for the BFS
   for (int bq = tid; bq < nb; bq += NT) {
     const int s0 = c.start[bq], s1 = c.start[bq + 1];
-    for (int i = s0; i < s1; ++i) { const int a = c.adj[i], k = a >> 1; nbr[i] = (a & 1) ? c.b1[k] : c.b2[k]; }
+    for (int i = s0; i < s1; ++i) {
+      const int a = c.adj[i], k = a >> 1, o = (a & 1) ? c.b1[k] : c.b2[k];
+      nbr[i] = o < nb ? o : -1;                                             // -1: a static obstacle, not a graph node
+    }
     mark[bq] = c.rank[bq] < 0 ? -2 : -1;                                    // -2 border, -1 unvisited, >= 0 position
   }
   __syncthreads();
@@ -375,7 +386,7 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
   int bw3[3] = {0, 0, 0};
   for (int k = tid; k < nc; k += NT) {
     const int u1 = c.b1[k], u2 = c.b2[k];
-    if (mark[u1] >= 0 && mark[u2] >= 0) {
+    if (u2 < nb && mark[u1] >= 0 && mark[u2] >= 0) {
       bw3[0] = max(bw3[0], abs(mark[u1] - mark[u2]));
       bw3[1] = max(bw3[1], abs(rkx[u1] - rkx[u2]));
       bw3[2] = max(bw3[2], abs(rky[u1] - rky[u2]));
@@ -548,14 +559,15 @@ __device__ __noinline__ void assemble_band(const Ctx& c) {
     for (int it = s0; it < s1; ++it) {
       const int a = adj[it], k = a >> 1, side = a & 1;
       const int other = side ? c.b1[k] : c.b2[k];
-      const int ro = rank[other];
+      const bool two = other < c.nb;                                        // else a static obstacle: diagonal only
+      const int ro = two ? rank[other] : 0;
       const double* Eo = Eall + 36 * (size_t)k;
 #pragma unroll
       for (int q = 0; q < 3; ++q)
 #pragma unroll
         for (int q2 = 0; q2 < 3; ++q2) {
           dg[3 * q + q2] += Eo[(3 * side + q) * 6 + 3 * side + q2];
-          k_add(ks, rb, q, ro, q2, Eo[(3 * side + q) * 6 + 3 * (1 - side) + q2]);
+          if (two) k_add(ks, rb, q, ro, q2, Eo[(3 * side + q) * 6 + 3 * (1 - side) + q2]);
         }
     }
 #pragma unroll
@@ -575,7 +587,8 @@ __device__ __noinline__ void assemble_band(const Ctx& c) {
     for (int it = s0 + lane; it < s1; it += 32) {
       const int a = adj[it], k = a >> 1, side = a & 1;
       const int other = side ? c.b1[k] : c.b2[k];
-      const int ro = rank[other];
+      const bool two = other < c.nb;                                        // else a static obstacle: diagonal only
+      const int ro = two ? rank[other] : 0;
       const double* Eo = Eall + 36 * (size_t)k;
 #pragma unroll
       for (int q = 0; q < 3; ++q)
@@ -583,6 +596,7 @@ __device__ __noinline__ void assemble_band(const Ctx& c) {
         for (int q2 = 0; q2 < 3; ++q2) {
           dg[3 * q + q2] += Eo[(3 * side + q) * 6 + 3 * side + q2];
           const double val = Eo[(3 * side + q) * 6 + 3 * (1 - side) + q2];
+          if (!two) continue;
           if (ro >= 0) k_add(ks, rb, q, ro, q2, val);
           else atomicAdd(&c.Cn[(3 * bi + q) * BD + 3 * (-1 - ro) + q2], val);
         }
@@ -960,8 +974,9 @@ __device__ __forceinline__ void pass_backward(const SolveDims c, const double* b
     const bool ok = rel < na;
     const int rc = ok ? rel : 0;
     const double xv = ok ? c.sol[k0 + PV + rc] : 0.0;
+    // a select, not a product with xv = 0: in the last pass (na = 0) panel entry 0 is never written
 #pragma unroll
-    for (int p = 0; p < 8; ++p) acc[p] = fma(U[p * LP + rc], xv, acc[p]);
+    for (int p = 0; p < 8; ++p) acc[p] = ok ? fma(U[p * LP + rc], xv, acc[p]) : acc[p];
   }
   {
     const bool okb = lane < BD;
@@ -1130,7 +1145,7 @@ __device__ __noinline__ void solve_kkt(const Ctx& c, BProf& pf, const double* rx
     const int b1 = c.b1[k], b2 = c.b2[k];
     double x1[3], x2[3];
 #pragma unroll
-    for (int q = 0; q < 3; ++q) { x1[q] = c.sol[sol_index(c, b1, q)]; x2[q] = c.sol[sol_index(c, b2, q)]; }
+    for (int q = 0; q < 3; ++q) { x1[q] = c.sol[sol_index(c, b1, q)]; x2[q] = b2 < c.nb ? c.sol[sol_index(c, b2, q)] : 0.0; }
     double gn = 0.0, gf = 0.0;
 #pragma unroll
     for (int q = 0; q < 3; ++q) { gn = fma(g[q], x1[q], gn); gn = fma(g[3 + q], x2[q], gn); }
@@ -1264,12 +1279,14 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
     for (int k = tid; k < nc; k += NT) {                                    // rz = G x + s - h - F z
       const double* g = c.cg + 12 * (size_t)k;
       const int b1 = c.b1[k], b2 = c.b2[k];
+      const bool two = b2 < c.nb;                                          // else a static obstacle: g[3..5], g[9..11] = 0
+      const int j2 = two ? 3 * b2 : 3 * b1;
       double gn = 0.0, gf = 0.0;
 #pragma unroll
-      for (int q = 0; q < 3; ++q) { gn = fma(g[q], c.x[3 * b1 + q], gn); gn = fma(g[3 + q], c.x[3 * b2 + q], gn); }
+      for (int q = 0; q < 3; ++q) { gn = fma(g[q], c.x[3 * b1 + q], gn); gn = fma(g[3 + q], c.x[j2 + q], gn); }
       if (cs == 4) {
 #pragma unroll
-        for (int q = 0; q < 3; ++q) { gf = fma(g[6 + q], c.x[3 * b1 + q], gf); gf = fma(g[9 + q], c.x[3 * b2 + q], gf); }
+        for (int q = 0; q < 3; ++q) { gf = fma(g[6 + q], c.x[3 * b1 + q], gf); gf = fma(g[9 + q], c.x[j2 + q], gf); }
         const double zn = c.z[k], z1 = c.z[ncap + k], z2 = c.z[2 * ncap + k], zg = c.z[3 * ncap + k];
         c.rz[k] = gn + c.s[k] - c.h[k];                                      // F row 0 = 0
         c.rz[ncap + k] = gf + c.s[ncap + k] - c.h[ncap + k] - zg;            // F rows f1, f2: E gamma
@@ -1437,7 +1454,8 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
     }
     const double nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
     const double p1x = E.p1[ic * 2], p1y = E.p1[ic * 2 + 1], p2x = E.p2[ic * 2], p2y = E.p2[ic * 2 + 1];
-    const int j1 = 3 * c.b1[k], j2 = 3 * c.b2[k];
+    const bool two = c.b2[k] < nb;                                          // else body2 is a static obstacle: no dofs
+    const int j1 = 3 * c.b1[k], j2 = two ? 3 * c.b2[k] : j1;
     const double rc = E.rest[ic];
     const double dhc = -dlam[k];                                            // dh = -dlam  (:55)
     double gnx = 0, gny = 0, g1x = 0, g1y = 0, g2x = 0, g2y = 0, jcv = 0;
@@ -1449,15 +1467,15 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
 #pragma unroll
       for (int t = 0; t < 3; ++t) {
         g[t] = dl * zh[j1 + t] + lq * dx[j1 + t];                           // dG[i][j1 + t]  (:53)
-        g[3 + t] = dl * zh[j2 + t] + lq * dx[j2 + t];
+        g[3 + t] = two ? dl * zh[j2 + t] + lq * dx[j2 + t] : 0.0;
       }
       if (q == 0) {
         const double row[6] = {p1x * ddy_ - p1y * ddx_, ddx_, ddy_, -(p2x * ddy_ - p2y * ddx_), -ddx_, -ddy_};
 #pragma unroll
-        for (int t = 0; t < 3; ++t) jcv += row[t] * v[j1 + t] + row[3 + t] * v[j2 + t];
+        for (int t = 0; t < 3; ++t) jcv += row[t] * v[j1 + t] + row[3 + t] * (two ? v[j2 + t] : 0.0);
         const double hs_ = mode == 0 ? rc : (1.0 - rc);                     // h_c = (Jc v) rest  |  (Jc v)(1 - rest)
 #pragma unroll
-        for (int t = 0; t < 3; ++t) { g[t] += dhc * hs_ * v[j1 + t]; g[3 + t] += dhc * hs_ * v[j2 + t]; }
+        for (int t = 0; t < 3; ++t) { g[t] += dhc * hs_ * v[j1 + t]; g[3 + t] += dhc * hs_ * (two ? v[j2 + t] : 0.0); }
       }
       const double gdx = -p1y * g[0] + g[1] + p2y * g[3] - g[4];
       const double gdy = p1x * g[0] + g[2] - p2x * g[3] - g[5];

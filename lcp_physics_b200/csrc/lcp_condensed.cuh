@@ -7,7 +7,8 @@
 //   (1) F + diag(s/z) =: M is block diagonal after a row permutation -- the connected components
 //       of F's sparsity graph are the per-contact blocks {normal, friction dirs, gamma}
 //       (engines.py:66-72: E, mu, -E^T), size 2 + fd; for post-stabilisation F = 0 (size 1);
-//   (2) a component's rows of G touch two bodies only (world.py:172-211): <= 6 columns.
+//   (2) a component's rows of G touch two bodies only (world.py:172-211): <= 6 columns (3 for a one-body contact
+//       against a static obstacle, body2 >= nb).
 // Eliminating dz = M^-1 (G dx + rz - rs/d) instead gives the n x n (+ e equality rows) system
 //       [ Q + G^T M^-1 G   A^T ] [dx]   [ -rx - G^T M^-1 (rz - rs/d) ]
 //       [ A                0   ] [dy] = [ -ry                        ]
@@ -469,24 +470,27 @@ __device__ __noinline__ bool build_structure_soa(const CPlan& P, CSmem<T>& S, St
   __syncthreads();
   for (int c = tid; c < nc; c += NT) {
     const int b1 = tb1[c], b2 = tb2[c];
-    if (b1 == b2 || b1 < 0 || b2 < 0 || b1 >= nb || b2 >= nb) { bad |= 1; continue; }
-    const int lo = min(b1, b2), hi = max(b1, b2);
+    if (b1 == b2 || b1 < 0 || b2 < 0 || b1 >= nb) { bad |= 1; continue; }
+    // b2 >= nb: a static obstacle (no dofs). The contact's rows touch body1's three columns only.
+    const bool two = b2 < nb;
+    const int lo = two ? min(b1, b2) : b1, hi = max(b1, b2);
     const int o1 = b1 < b2 ? 0 : 3, o2 = 3 - o1;                   // slots of body1 / body2 in the sorted column list
 #pragma unroll
     for (int q = 0; q < 3; ++q) {
       S.ccols()[q * pcap + c] = (unsigned char)(3 * lo + q);
-      S.ccols()[(3 + q) * pcap + c] = (unsigned char)(3 * hi + q);
+      if (two) S.ccols()[(3 + q) * pcap + c] = (unsigned char)(3 * hi + q);
     }
-    S.ncols()[c] = 6;
+    S.ncols()[c] = two ? 6 : 3;
     const T nx = normal[2 * c], ny = normal[2 * c + 1];
     const T p1x = p1[2 * c], p1y = p1[2 * c + 1], p2x = p2[2 * c], p2y = p2[2 * c + 1];
     T r1[3], r2[3];
     contact_row<T>(p1x, p1y, p2x, p2y, nx, ny, r1, r2);            // Jc row
+    const T v20 = two ? v[3 * b2] : T(0), v21 = two ? v[3 * b2 + 1] : T(0), v22 = two ? v[3 * b2 + 2] : T(0);
     const T jv = r1[0] * v[3 * b1] + r1[1] * v[3 * b1 + 1] + r1[2] * v[3 * b1 + 2] +
-                 r2[0] * v[3 * b2] + r2[1] * v[3 * b2 + 1] + r2[2] * v[3 * b2 + 2];
+                 r2[0] * v20 + r2[1] * v21 + r2[2] * v22;
     const T rc = e_.rest[(size_t)sc * ncs + c];
 #pragma unroll
-    for (int q = 0; q < 3; ++q) { S.Gd()[(size_t)(o1 + q) * pcap + c] = r1[q]; S.Gd()[(size_t)(o2 + q) * pcap + c] = r2[q]; }
+    for (int q = 0; q < 3; ++q) { S.Gd()[(size_t)(o1 + q) * pcap + c] = r1[q]; if (two) S.Gd()[(size_t)(o2 + q) * pcap + c] = r2[q]; }
     S.rows()[c] = (unsigned short)c;
     S.posof()[c] = (unsigned short)c;
     if (e_.mode == 0) {
@@ -494,8 +498,9 @@ __device__ __noinline__ bool build_structure_soa(const CPlan& P, CSmem<T>& S, St
       contact_row<T>(p1x, p1y, p2x, p2y, ny, -nx, r1, r2);         // Jf rows: +- left_orthogonal(n)  (world.py:186-211)
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
-        S.Gd()[(size_t)(o1 + q) * pcap + nc + c] = r1[q];      S.Gd()[(size_t)(o2 + q) * pcap + nc + c] = r2[q];
-        S.Gd()[(size_t)(o1 + q) * pcap + 2 * nc + c] = -r1[q]; S.Gd()[(size_t)(o2 + q) * pcap + 2 * nc + c] = -r2[q];
+        S.Gd()[(size_t)(o1 + q) * pcap + nc + c] = r1[q];
+        S.Gd()[(size_t)(o1 + q) * pcap + 2 * nc + c] = -r1[q];
+        if (two) { S.Gd()[(size_t)(o2 + q) * pcap + nc + c] = r2[q]; S.Gd()[(size_t)(o2 + q) * pcap + 2 * nc + c] = -r2[q]; }
       }
       const int rw[4] = {c, nc + 2 * c, nc + 2 * c + 1, 3 * nc + c};
 #pragma unroll
@@ -511,7 +516,7 @@ __device__ __noinline__ bool build_structure_soa(const CPlan& P, CSmem<T>& S, St
       hs[c] = jv + jv * -rc;                                       // engines.py:90
     }
     // column lists: arrival order, ranked below
-    for (int q = 0; q < 6; ++q) {
+    for (int q = 0; q < (two ? 6 : 3); ++q) {
       const int a = q < 3 ? 3 * lo + q : 3 * hi + q - 3;
       const int slot = atomicAdd(&cl_cnt[a], 1);
       if (slot < LMAX) cl_tmp[slot * n + a] = (unsigned short)(c * 8 + q); else bad |= 1;
@@ -1465,7 +1470,8 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
       }
       const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
       const T p1x = E.p1[ic * 2], p1y = E.p1[ic * 2 + 1], p2x = E.p2[ic * 2], p2y = E.p2[ic * 2 + 1];
-      const int j1 = 3 * tb1[c], j2 = 3 * tb2[c];
+      const bool two = tb2[c] < nb;                               // else body2 is a static obstacle: no columns
+      const int j1 = 3 * tb1[c], j2 = two ? 3 * tb2[c] : j1;
       const T rc = E.rest[ic];
       const T dhc = -dlam[c] * (E.mode == 0 ? T(1) : T(1));      // dh = -dlam  (:55)
       T gnx = 0, gny = 0, g1x = 0, g1y = 0, g2x = 0, g2y = 0, jcv = 0;
@@ -1478,13 +1484,13 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
         T g[6];
         for (int t = 0; t < 3; ++t) {
           g[t] = dlam[i] * zh_[j1 + t] + lm[i] * dx[j1 + t];      // dG[i][j1+t]  (:53)
-          g[3 + t] = dlam[i] * zh_[j2 + t] + lm[i] * dx[j2 + t];
+          g[3 + t] = two ? dlam[i] * zh_[j2 + t] + lm[i] * dx[j2 + t] : T(0);
         }
         if (q == 0) {
           const T row[6] = {p1x * ddy_ - p1y * ddx_, ddx_, ddy_, -(p2x * ddy_ - p2y * ddx_), -ddx_, -ddy_};
-          for (int t = 0; t < 3; ++t) jcv += row[t] * v[j1 + t] + row[3 + t] * v[j2 + t];
+          for (int t = 0; t < 3; ++t) jcv += row[t] * v[j1 + t] + row[3 + t] * (two ? v[j2 + t] : T(0));
           const T hs_ = E.mode == 0 ? rc : (T(1) - rc);            // h_c = (Jc v) rest  |  (Jc v)(1 - rest)
-          for (int t = 0; t < 3; ++t) { g[t] += dhc * hs_ * v[j1 + t]; g[3 + t] += dhc * hs_ * v[j2 + t]; }
+          for (int t = 0; t < 3; ++t) { g[t] += dhc * hs_ * v[j1 + t]; g[3 + t] += dhc * hs_ * (two ? v[j2 + t] : T(0)); }
         }
         const T gdx = -p1y * g[0] + g[1] + p2y * g[3] - g[4];
         const T gdy = p1x * g[0] + g[2] - p2x * g[3] - g[5];

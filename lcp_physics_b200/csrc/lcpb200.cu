@@ -908,9 +908,11 @@ extern "C" int lcpb200_find_contacts(int dtype, int B, int nb, int cap, double e
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    cts::launch_find_contacts<float>(B, nb, cap, (float)eps, (const float*)pos, (const float*)rad, body1, body2, counts, sms, st);
+    cts::launch_find_contacts<float>(B, nb, 0, 0, cap, (float)eps, (const float*)pos, (const float*)rad, nullptr, body1,
+                                     body2, counts, sms, st);
   else
-    cts::launch_find_contacts<double>(B, nb, cap, eps, (const double*)pos, (const double*)rad, body1, body2, counts, sms, st);
+    cts::launch_find_contacts<double>(B, nb, 0, 0, cap, eps, (const double*)pos, (const double*)rad, nullptr, body1,
+                                      body2, counts, sms, st);
   CK(cudaGetLastError());
   return 0;
 }
@@ -929,13 +931,60 @@ extern "C" int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    cts::launch_contact_geometry<float>(B, nb, cap, (const float*)pos, (const float*)rad, (const float*)fric,
-                                        (const float*)rest, body1, body2, counts, (float*)normal, (float*)p1, (float*)p2,
-                                        (float*)pen, (float*)mu, (float*)rest_c, sms, st);
+    cts::launch_contact_geometry<float>(B, nb, 0, 0, cap, (const float*)pos, (const float*)rad, (const float*)fric,
+                                        (const float*)rest, nullptr, nullptr, nullptr, nullptr, body1, body2, counts,
+                                        (float*)normal, (float*)p1, (float*)p2, (float*)pen, (float*)mu, (float*)rest_c,
+                                        sms, st);
   else
-    cts::launch_contact_geometry<double>(B, nb, cap, (const double*)pos, (const double*)rad, (const double*)fric,
-                                         (const double*)rest, body1, body2, counts, (double*)normal, (double*)p1,
-                                         (double*)p2, (double*)pen, (double*)mu, (double*)rest_c, sms, st);
+    cts::launch_contact_geometry<double>(B, nb, 0, 0, cap, (const double*)pos, (const double*)rad, (const double*)fric,
+                                         (const double*)rest, nullptr, nullptr, nullptr, nullptr, body1, body2, counts,
+                                         (double*)normal, (double*)p1, (double*)p2, (double*)pen, (double*)mu,
+                                         (double*)rest_c, sms, st);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+template <typename T>
+static void world_contacts_t(int B, int nb, int no, int nv, int cap, double eps, const void* pos, const void* rad,
+                             const void* fric, const void* rest, const void* verts, const void* oref, const void* ofric,
+                             const void* orest, int32_t* body1, int32_t* body2, int32_t* counts, void* normal, void* p1,
+                             void* p2, void* pen, void* mu, void* rest_c, bool geometry, int sms, cudaStream_t st) {
+  cts::launch_find_contacts<T>(B, nb, no, nv, cap, (T)eps, (const T*)pos, (const T*)rad, (const T*)verts, body1, body2,
+                               counts, sms, st);
+  if (geometry)
+    cts::launch_contact_geometry<T>(B, nb, no, nv, cap, (const T*)pos, (const T*)rad, (const T*)fric, (const T*)rest,
+                                    (const T*)verts, (const T*)oref, (const T*)ofric, (const T*)orest, body1, body2,
+                                    counts, (T*)normal, (T*)p1, (T*)p2, (T*)pen, (T*)mu, (T*)rest_c, sms, st);
+}
+
+extern "C" int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, double eps, const void* pos,
+                                      const void* rad, const void* fric, const void* rest, const void* verts,
+                                      const void* oref, const void* ofric, const void* orest, int32_t* body1,
+                                      int32_t* body2, int32_t* counts, void* normal, void* p1, void* p2, void* pen,
+                                      void* mu, void* rest_c, void* stream) {
+  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
+  if (B < 0 || nb <= 0 || no < 0 || cap <= 0) return fail("world_contacts: need B >= 0, nb > 0, no >= 0, cap > 0");
+  if (no > 0 && nv < 3) return fail("world_contacts: obstacles need nv >= 3 vertices");
+  if ((long long)nb + no > 0x7fffffffLL) return fail("world_contacts: too many bodies");
+  if (!pos || !rad || !body1 || !body2 || !counts) return fail("world_contacts: NULL argument");
+  if (no > 0 && !verts) return fail("world_contacts: obstacles need verts");
+  const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
+                   (rest_c != nullptr);
+  if (ngeo != 0 && ngeo != 6) return fail("world_contacts: the geometry outputs are all NULL or all non-NULL");
+  const bool geometry = ngeo == 6;
+  if (geometry && (!fric || !rest || (no > 0 && (!oref || !ofric || !orest))))
+    return fail("world_contacts: the geometry needs fric, rest and, with obstacles, oref, ofric, orest");
+  if (B == 0) return 0;
+  int dev = 0, sms = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == LCPB200_F32)
+    world_contacts_t<float>(B, nb, no, nv, cap, eps, pos, rad, fric, rest, verts, oref, ofric, orest, body1, body2,
+                            counts, normal, p1, p2, pen, mu, rest_c, geometry, sms, st);
+  else
+    world_contacts_t<double>(B, nb, no, nv, cap, eps, pos, rad, fric, rest, verts, oref, ofric, orest, body1, body2,
+                             counts, normal, p1, p2, pen, mu, rest_c, geometry, sms, st);
   CK(cudaGetLastError());
   return 0;
 }

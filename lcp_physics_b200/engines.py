@@ -164,7 +164,10 @@ def engine_solve(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2,
     optional equality rows A [B,e,3nb], b [B,e]. Returns (zhat [B,3nb], status [B]); status == -100 marks a
     scene whose topology the fused kernel does not take (use assemble_contacts + LCPFunction for it).
     solve_dynamics: new_v = -zhat (engines.py:76); post_stabilization: dp = -zhat (engines.py:116).
-    counts [B] int32 (batched worlds): scene s uses its first counts[s] contacts; body1/body2 are then [B,nc]."""
+    counts [B] int32 (batched worlds): scene s uses its first counts[s] contacts; body1/body2 are then [B,nc].
+    body2 >= nb names a static obstacle (no dofs: a wall, floor or ramp): a one-body contact whose rows touch body1's
+    three columns only -- the reference's formulation with the obstacle pinned by a TotalConstraint, reduced by the
+    pinned dofs; its p2 is unused (zero gradient). body1 must be a body (< nb)."""
     _lib.require_cuda()
     return _EngineSolveFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode,
                                 max_iter, exact_adjoint, counts)

@@ -19,13 +19,18 @@ without contacts gets the equality-constrained solve of engines.py:35-49 inside 
 
 Scope (what the reference's demos use that this class mirrors): `Circle` bodies (bodies.py:114-140),
 `Gravity` (forces.py), `TotalConstraint` pins (constraints.py:176-192), restitution / friction as the
-mean of the two bodies (world.py:144-151, :213-224), `eps`, `tol`, `post_stab`, `strict_no_penetration`.
-Hulls (`Rect`, `Hull`), joints between bodies and the renderer are not mirrored (SURVEY.md section 8f).
+mean of the two bodies (world.py:144-151, :213-224), `eps`, `tol`, `post_stab`, `strict_no_penetration`,
+and STATIC convex polygon obstacles -- the reference's `Rect` / `Hull` floors, walls and ramps pinned by a
+`TotalConstraint` (`obstacles=`, `rect_vertices`): a pinned body has zero velocity, so its equality rows are
+eliminated exactly and a contact against it is a one-body contact (body2 >= nb, include/lcpb200.h) whose rows touch
+only the circle's three columns (DESIGN.md section 9). Dynamic hulls, hull-hull contacts, joints between bodies and
+the renderer are not mirrored (SURVEY.md section 8f).
 Everything is differentiable through torch autograd (the LCP through lcpb200_engine_backward). Scenes of up to
 42 bodies (3 nb + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes (BASELINE
 config 4: a 512-ball pile) the banded large-scene kernels (csrc/lcp_banded.cuh), float64.
 """
 import ctypes
+import math
 
 import torch
 
@@ -33,16 +38,81 @@ from . import _lib
 from .engines import engine_solve
 
 
+def rect_vertices(pos, dims, angle=0.0):
+    """World-frame vertices [4, 2] of the reference's `Rect(pos, dims)` rotated by `angle` (bodies.py:253-290: half
+    dims v0 = (w/2, h/2), v1 = (-w/2, h/2), vertices [v0, v1, -v0, -v1] about the centre, rotated by
+    [[cos, -sin], [sin, cos]]). Differentiable in every argument (tensors or numbers)."""
+    ref = next((t for t in (pos, dims, angle) if isinstance(t, torch.Tensor)), None)
+    dt_ = ref.dtype if ref is not None and ref.is_floating_point() else torch.float64
+    dev = ref.device if ref is not None else None
+    pos, dims, angle = [torch.as_tensor(t, dtype=dt_, device=dev) for t in (pos, dims, angle)]
+    h = dims / 2
+    v0, v1 = h, h * h.new_tensor([-1.0, 1.0])
+    local = torch.stack([v0, v1, -v0, -v1])
+    c, s = torch.cos(angle), torch.sin(angle)
+    rot = torch.stack([torch.stack([c, -s]), torch.stack([s, c])])
+    return pos + local @ rot.t()
+
+
+def polygon_centroid(verts):
+    """Area centroid [..., 2] of polygons [..., V, 2] (bodies.py:216-226: the reference point of a `Hull`)."""
+    a, b = verts, torch.roll(verts, -1, dims=-2)
+    cross = b[..., 0] * a[..., 1] - b[..., 1] * a[..., 0]
+    return (cross.unsqueeze(-1) * (a + b)).sum(-2) / (6 * (cross.sum(-1) / 2).unsqueeze(-1))
+
+
+def check_obstacles(verts, B):
+    """Validates obstacle vertices [no, V, 2] (shared by the batch) or [B, no, V, 2]; returns them as [B, no, V, 2].
+    Every polygon must have >= 3 vertices, a non-zero area and be convex (the contact rule of contacts.py:84-144 is
+    the one for convex hulls). All polygons share V: a polygon with fewer vertices may repeat one (its zero-length
+    edges are skipped by the contact rule)."""
+    v = torch.as_tensor(verts)
+    if v.dim() == 3:
+        v = v.unsqueeze(0).expand(B, -1, -1, -1)
+    if v.dim() != 4 or v.shape[0] != B or v.shape[3] != 2:
+        raise ValueError("obstacles: need vertices [no, V, 2] or [B, no, V, 2] (B = %d), got %s" % (B, tuple(v.shape)))
+    if v.shape[1] == 0:
+        raise ValueError("obstacles: no polygon given (pass obstacles=None)")
+    if v.shape[2] < 3:
+        raise ValueError("obstacles: every polygon needs at least 3 vertices")
+    w = v.detach().double()
+    if not bool(torch.isfinite(w).all()):
+        raise ValueError("obstacles: non-finite vertex")
+    e = torch.roll(w, -1, dims=2) - w
+    deg = ~(e.norm(dim=-1) > 0)                          # zero-length edges: a vertex repeated to pad to the common V
+    en, found = torch.roll(e, -1, dims=2), ~torch.roll(deg, -1, dims=2)
+    for s_ in range(2, v.shape[2]):                      # the next edge of non-zero length
+        ok = ~found & ~torch.roll(deg, -s_, dims=2)
+        en = torch.where(ok.unsqueeze(-1), torch.roll(e, -s_, dims=2), en)
+        found = found | ok
+    # cross product of consecutive edges; collinear vertices (|turn| at round-off level) are allowed
+    turn = (e[..., 0] * en[..., 1] - e[..., 1] * en[..., 0]) / (e.norm(dim=-1) * en.norm(dim=-1)).clamp_min(1e-300)
+    turn = torch.where(deg, torch.zeros_like(turn), turn)
+    area = (w[..., 0] * torch.roll(w, -1, dims=2)[..., 1] - w[..., 1] * torch.roll(w, -1, dims=2)[..., 0]).sum(-1)
+    if bool((area.abs() <= 0).any()):
+        raise ValueError("obstacles: a polygon has zero area")
+    tol = math.sqrt(torch.finfo(v.dtype).eps) if v.is_floating_point() else 1e-8    # coordinates rounded to v.dtype
+    if bool(((turn * area.sign().unsqueeze(-1)) < -tol).any()):
+        raise ValueError("obstacles: every polygon must be convex")
+    return v
+
+
 class BatchedWorld:
     def __init__(self, pos, rad, vel=None, mass=1.0, restitution=0.5, fric_coeff=0.9, gravity=10.0,
                  static=(), gravity_mask=None, dt=1.0 / 30, eps=0.1, tol=1e-6, post_stab=False,
-                 strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False):
+                 strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False,
+                 obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5):
         """pos [B,nb,2], rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass / restitution /
         fric_coeff [B,nb] (or broadcastable), `static`: indices of bodies pinned by a TotalConstraint,
         `gravity`: g of the `Gravity` force (forces.py) applied to the bodies in gravity_mask
         (default: every non-static body). `exact_adjoint`: backward() through every LCP solve uses the true
         adjoint (the transposed KKT system, DESIGN.md section 3.4); the default False reproduces the reference's
-        gradients, which are biased for every step with friction. Forward results do not depend on it."""
+        gradients, which are biased for every step with friction. Forward results do not depend on it.
+        `obstacles`: world-frame vertices of static convex polygons, [no, V, 2] (shared by the batch) or
+        [B, no, V, 2] (e.g. `rect_vertices`; a polygon with fewer than V vertices repeats one); they may require
+        grad. They act as the reference's pinned `Rect` / `Hull` bodies listed AFTER the circles: contact order,
+        rule and material are those of such a World.
+        `obstacle_fric` / `obstacle_rest`: their friction / restitution, [B,no] or broadcastable."""
         _lib.require_cuda()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         pos = torch.as_tensor(pos)
@@ -77,15 +147,27 @@ class BatchedWorld:
         self.dt, self.eps, self.tol = float(dt), float(eps), float(tol)
         self.post_stab, self.strict_no_pen, self.max_iter = post_stab, strict_no_penetration, max_iter
         self.exact_adjoint = bool(exact_adjoint)
-        ii, jj = torch.triu_indices(nb, nb, 1)
+        self.no, self.nv = 0, 0
+        if obstacles is not None:
+            ov = check_obstacles(obstacles, B)
+            self.ov = ov.to(device=self.device, dtype=self.dtype)                  # [B,no,V,2], keeps its graph
+            self.no, self.nv = int(ov.shape[1]), int(ov.shape[2])
+            bo = lambda t: to(t).expand(B, self.no).contiguous() if torch.as_tensor(t).dim() < 2 else to(t)
+            self.ofric, self.orest = bo(obstacle_fric), bo(obstacle_rest)
+            self.oref = polygon_centroid(self.ov)                                   # Hull.pos (bodies.py:166-173)
+        nt = nb + self.no
+        ii, jj = torch.triu_indices(nt, nt, 1)
+        if self.no:
+            keep = ii < nb                                                          # obstacles never pair up
+            ii, jj = ii[keep], jj[keep]
         self.pi, self.pj = ii.to(self.device), jj.to(self.device)                   # pair (i, j), i < j, lexicographic
-        self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), 3 * nb)
+        self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), (4 if self.no else 3) * nb)
         # 3 nb + 3 n_static <= 128 and <= 256 contacts: condensed-KKT kernels (fp32 / fp64, differentiable);
         # larger scenes: the banded large-scene kernels (fp64; lcp_banded.cuh)
         self.large = self.n + self.ne > 128 or 4 * self.cap > 1024
         if self.large and (self.dtype != torch.float64 or self.ne > 16):
             raise ValueError("BatchedWorld: scenes with 3 nb + 3 n_static > 128 (or > 256 contacts) need float64 "
-                             "and at most 5 pinned bodies")
+                             "and at most 5 pinned bodies (static obstacles do not count)")
         self.t = pos.new_zeros(B)
         self.find_contacts()
         if self.strict_no_pen and bool((self.max_penetration() > self.tol).any()):
@@ -96,6 +178,8 @@ class BatchedWorld:
         """Pair test + ordered compaction on the GPU (lcpb200_find_contacts: all nb (nb - 1) / 2 pairs of every
         scene, lexicographic order = the reference's contact order), then the contact geometry of the selected
         pairs with torch ops (differentiable w.r.t. the positions)."""
+        if self.no:
+            return self._find_contacts_obstacles()
         lib = _lib.load()
         B, cap, dev = self.B, self.cap, self.device
         pos = self.p[:, :, 1:]
@@ -141,11 +225,130 @@ class BatchedWorld:
         self.c_rest = 0.5 * (take(self.restitution, i1) + take(self.restitution, i2))          # world.py:144-151
         self.counts = counts
 
+    def _find_contacts_obstacles(self):
+        """find_contacts for worlds with static obstacles: lcpb200_world_contacts walks circle-circle and
+        circle-obstacle pairs in the order of a reference World with bodies [circles..., obstacles...]; the geometry
+        comes from the same call, or from torch ops (_geometry_torch) when something needs autograd."""
+        lib = _lib.load()
+        B, cap, dev = self.B, self.cap, self.device
+        pos_c = self.p[:, :, 1:].detach().contiguous()
+        b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        counts = torch.empty(B, dtype=torch.int32, device=dev)
+        needs_graph = torch.is_grad_enabled() and any(
+            t.requires_grad for t in (self.p, self.rad, self.fric_coeff, self.restitution, self.ov, self.ofric, self.orest))
+        d = lambda t: t.detach().contiguous()
+        geo = [None] * 6
+        if not needs_graph:
+            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+            geo = [new(2), new(2), new(2), new(), new(), new()]
+        with torch.cuda.device(dev):
+            _lib.check(lib.lcpb200_world_contacts(
+                _lib.dtype_code(self.dtype), B, self.nb, self.no, self.nv, cap, self.eps, _lib.ptr(pos_c),
+                *[_lib.ptr(d(t)) for t in (self.rad, self.fric_coeff, self.restitution, self.ov, self.oref, self.ofric,
+                                           self.orest)],
+                _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
+                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        if int(counts.max()) > cap:
+            raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
+        self.c_b1, self.c_b2, self.counts = b1, b2, counts
+        if not needs_graph:
+            self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest = geo
+            return
+        self.c_normal, self.c_p1, self.c_p2, pen, self.c_mu, self.c_rest = self._geometry_torch(b1, b2)
+        valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
+        self.c_pen = torch.where(valid, pen, pen.new_full((), -1e30))
+
+    def _circle_polygon_torch(self, c, k):
+        """Torch mirror of csrc/lcp_contacts.cuh circle_polygon for circle centres c [B,P,2] against obstacles
+        k [B,P] (long): (inside, closest point q, squared distance, separating-edge normal, separation)."""
+        B, P = k.shape
+        V = torch.gather(self.ov, 1, k.reshape(B, P, 1, 1).expand(B, P, self.nv, 2))       # [B,P,V,2]
+        Wv = torch.roll(V, -1, dims=2)
+        E = Wv - V
+        area = (V[..., 0] * Wv[..., 1] - V[..., 1] * Wv[..., 0]).sum(2)
+        orient = torch.where(area > 0, 1.0, -1.0).to(V.dtype).unsqueeze(2)
+        ln = E.norm(dim=3)
+        dg = ~(ln > 0)                                     # zero-length edges (repeated vertices): skipped, as the kernel
+        ln1 = torch.where(dg, torch.ones_like(ln), ln)     # keeps the skipped entries finite, gradients too
+        nrm = torch.stack([orient * E[..., 1] / ln1, -orient * E[..., 0] / ln1], 3)        # outward unit normals
+        rel = c.unsqueeze(2) - V
+        sp = torch.where(dg, torch.full_like(ln, -math.inf), (nrm * rel).sum(3))
+        inside = ~(sp > 0).any(2)
+        ee = (E * E).sum(3)
+        t = ((rel * E).sum(3) / torch.where(dg, torch.ones_like(ee), ee)).clamp(0.0, 1.0)
+        Q = V + t.unsqueeze(3) * E
+        d2 = torch.where(dg, torch.full_like(ln, math.inf), ((c.unsqueeze(2) - Q) ** 2).sum(3))
+        em = d2.argmin(2, keepdim=True)
+        q = torch.gather(Q, 2, em.unsqueeze(3).expand(-1, -1, 1, 2)).squeeze(2)
+        es = sp.argmax(2, keepdim=True)
+        n_in = torch.gather(nrm, 2, es.unsqueeze(3).expand(-1, -1, 1, 2)).squeeze(2)
+        sep = torch.gather(sp, 2, es).squeeze(2)
+        return inside, q, torch.gather(d2, 2, em).squeeze(2), n_in, sep
+
+    def _geometry_torch(self, b1, b2):
+        """Differentiable geometry and material of the selected pairs (circle-circle: contacts.py:69-77;
+        circle-obstacle: contacts.py:84-144, as lcpb200_world_contacts), gradients reaching positions, radii,
+        materials and the obstacle vertices."""
+        nb = self.nb
+        pos = self.p[:, :, 1:]
+        i1, i2 = b1.long(), b2.long()
+        cc = i2 < nb
+        j = torch.where(cc, i2, 0)
+        k = torch.where(cc, 0, i2 - nb)
+        take = lambda t, idx: torch.gather(t, 1, idx)
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+        c = take2(pos, i1)
+        r1 = take(self.rad, i1)
+        one = torch.zeros_like(c)
+        one[..., 0] = 1.0
+        # circle-circle (slots of obstacle pairs get a harmless unit offset: no 0 / 0 in either pass)
+        dcc = torch.where(cc.unsqueeze(2), c - take2(pos, j), one)
+        dist = dcc.norm(dim=2)
+        r2 = take(self.rad, j)
+        pen_cc = r1 + r2 - dist
+        n_cc = dcc / dist.unsqueeze(2)
+        p1_cc = -n_cc * (r1 - pen_cc / 2).unsqueeze(2)
+        p2_cc = n_cc * (r2 - pen_cc / 2).unsqueeze(2)
+        # circle-obstacle
+        inside, q, _, n_in, sep = self._circle_polygon_torch(c, k)
+        out = ~cc & ~inside
+        dq = torch.where(out.unsqueeze(2), c - q, one)
+        dq_n = dq.norm(dim=2)
+        n_co = torch.where(inside.unsqueeze(2), n_in, dq / dq_n.unsqueeze(2))
+        pen_co = torch.where(inside, r1 - sep, r1 - dq_n)
+        q_co = torch.where(inside.unsqueeze(2), c - n_in * sep.unsqueeze(2), q)   # best_pt2 = center - n (dist + rad)
+        p1_co = q_co - c
+        p2_co = q_co - take2(self.oref, k)
+        w = cc.unsqueeze(2)
+        normal = torch.where(w, n_cc, n_co)
+        p1 = torch.where(w, p1_cc, p1_co)
+        p2 = torch.where(w, p2_cc, p2_co)
+        pen = torch.where(cc, pen_cc, pen_co)
+        f1, e1 = take(self.fric_coeff, i1), take(self.restitution, i1)
+        mu = 0.5 * (f1 + torch.where(cc, take(self.fric_coeff, j), take(self.ofric, k)))          # world.py:213-224
+        rest = 0.5 * (e1 + torch.where(cc, take(self.restitution, j), take(self.orest, k)))       # world.py:144-151
+        return normal, p1, p2, pen, mu, rest
+
     def find_contacts_torch(self):
         """The same contact list with torch ops only (O(nb^2) tensors, a stable sort for the compaction): the
-        independent implementation tests/test_gpu_world.py checks lcpb200_find_contacts against. Returns
-        (counts, b1, b2)."""
+        independent implementation tests/test_gpu_world.py checks lcpb200_find_contacts against (and
+        tests/test_gpu_obstacles.py lcpb200_world_contacts). Returns (counts, b1, b2)."""
         pos = self.p[:, :, 1:]
+        if self.no:
+            nb = self.nb
+            cc = self.pj < nb
+            B = self.B
+            pj = torch.where(cc, self.pj, 0)
+            d = pos[:, self.pi] - pos[:, pj]
+            pen = self.rad[:, self.pi] + self.rad[:, pj] - d.norm(dim=2)
+            k = torch.where(cc, 0, self.pj - nb).unsqueeze(0).expand(B, -1)
+            inside, _, d2, _, _ = self._circle_polygon_torch(pos[:, self.pi], k)
+            hit_o = inside | ~(d2.sqrt() - self.rad[:, self.pi] > self.eps)              # contacts.py:110-112
+            active = torch.where(cc, pen >= -self.eps, hit_o)
+            counts = active.sum(1)
+            order = torch.sort((~active).to(torch.int8), dim=1, stable=True)[1][:, :self.cap]
+            return counts.to(torch.int32), self.pi[order].to(torch.int32), self.pj[order].to(torch.int32)
         d = pos[:, self.pi] - pos[:, self.pj]
         pen = self.rad[:, self.pi] + self.rad[:, self.pj] - d.norm(dim=2)
         active = pen >= -self.eps                                                  # `if penetration < -eps: return`
