@@ -191,6 +191,49 @@ int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, do
                            void* normal, void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
                            void* stream);
 
+/* Contact detection and geometry for B scenes of nb circles, np DYNAMIC convex polygons (the reference's Rect / Hull
+ * bodies) and no static obstacles. The pairs (i, j), i < j, of the body list [circles 0..nb-1, polygons nb..nb+np-1,
+ * obstacles nb+np..nb+np+no-1] (obstacles never pair with each other) are visited in lexicographic order, the contact
+ * order of a reference World built from [Circle..., Rect / Hull..., pinned Rect / Hull...]. A pair gives 0, 1 or 2
+ * contacts, stored in that order:
+ *   circle-circle                 as lcpb200_find_contacts;
+ *   circle-polygon / -obstacle    the circle-hull rule of lcpb200_world_contacts; p2 = q - centroid (two-body contact
+ *                                 for a polygon, one-body for an obstacle);
+ *   polygon-polygon / -obstacle   the hull-hull rule of physics/contacts.py:145-292: SAT both ways (edge normal
+ *                                 left_orthogonal(e) / |e|, support with >=, the last maximal vertex wins; separated iff
+ *                                 the largest edge separation is > eps; body2 holds the reference face iff its
+ *                                 separation is strictly larger), the incident edge at the support vertex whose
+ *                                 normal has the smallest dot product with the reference normal, and clipping of the
+ *                                 incident edge to the planes +-|e_ref| / 2 about the REFERENCE BODY's CENTROID (not
+ *                                 the edge's midpoint), twice, a point kept iff n . (v - v_ref) <= eps -- 0 to 2
+ *                                 contacts, in the order of the clipped points. SAT scans start at edge 0 (the reference
+ *                                 starts at the edge that won last time): the results differ only on an exact tie
+ *                                 between two edge separations.
+ * Zero-length edges (a vertex repeated to pad a polygon to nv) are skipped everywhere.
+ * Device pointers (NULL allowed for an empty group):
+ *   pos[B,nb,2] rad[B,nb] fric[B,nb] rest[B,nb]       circles (fric / rest: only for the geometry)
+ *   pverts[B,np,nv,2] pcen[B,np,2] pfric[B,np] prest[B,np]
+ *                                                     polygons: world-frame vertices (positive shoelace area),
+ *                                                     centroids, friction and restitution
+ *   overts[B,no,nv,2] oref[B,no,2] ofric[B,no] orest[B,no]
+ *                                                     obstacles, as lcpb200_world_contacts (either orientation)
+ *   body1[B,cap] body2[B,cap] counts[B]               OUT: as lcpb200_world_contacts; body2 >= nb + np names obstacle
+ *                                                     body2 - nb - np (a one-body contact)
+ *   feat[B,cap] int32                                 OUT: per hull-hull contact its discrete features (bits 0-1 the
+ *                                                     point: incident endpoint 0 / 1, cut by the first / second clip
+ *                                                     plane; bits 2-3 the first clip's outcome; bit 4 body2 holds the
+ *                                                     reference face; bits 5-12 reference edge; bits 13-20 incident
+ *                                                     edge), from which the geometry is rebuilt; -1 for other contacts
+ *   normal p1 p2 penetration mu restitution_c         OUT, all NULL or all non-NULL: as lcpb200_world_contacts
+ * 3 <= nv <= 256 when np + no > 0. With np == 0 the pairs, their order and the geometry are those of
+ * lcpb200_world_contacts. */
+int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
+                          const void* rad, const void* fric, const void* rest, const void* pverts, const void* pcen,
+                          const void* pfric, const void* prest, const void* overts, const void* oref,
+                          const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
+                          int32_t* feat, void* normal, void* p1, void* p2, void* penetration, void* mu,
+                          void* restitution_c, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

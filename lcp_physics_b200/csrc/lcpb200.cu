@@ -897,6 +897,19 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
 }
 
 // ------------------------------------------------------------------ assembly
+template <typename T>
+static cts::Bodies<T> bodies(int nb, int np, int no, int nv, const void* pos, const void* rad, const void* fric,
+                             const void* rest, const void* pverts, const void* pcen, const void* pfric,
+                             const void* prest, const void* overts, const void* oref, const void* ofric,
+                             const void* orest) {
+  cts::Bodies<T> bd;
+  bd.nb = nb; bd.np = np; bd.no = no; bd.nv = nv;
+  bd.pos = (const T*)pos; bd.rad = (const T*)rad; bd.fric = (const T*)fric; bd.rest = (const T*)rest;
+  bd.pverts = (const T*)pverts; bd.pcen = (const T*)pcen; bd.pfric = (const T*)pfric; bd.prest = (const T*)prest;
+  bd.overts = (const T*)overts; bd.oref = (const T*)oref; bd.ofric = (const T*)ofric; bd.orest = (const T*)orest;
+  return bd;
+}
+
 extern "C" int lcpb200_find_contacts(int dtype, int B, int nb, int cap, double eps, const void* pos, const void* rad,
                                      int32_t* body1, int32_t* body2, int32_t* counts, void* stream) {
   if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
@@ -908,11 +921,13 @@ extern "C" int lcpb200_find_contacts(int dtype, int B, int nb, int cap, double e
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    cts::launch_find_contacts<float>(B, nb, 0, 0, cap, (float)eps, (const float*)pos, (const float*)rad, nullptr, body1,
-                                     body2, counts, sms, st);
+    cts::launch_find_contacts<float, false>(
+        bodies<float>(nb, 0, 0, 0, pos, rad, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, (float)eps, body1, body2, nullptr,
+        counts, sms, st);
   else
-    cts::launch_find_contacts<double>(B, nb, 0, 0, cap, eps, (const double*)pos, (const double*)rad, nullptr, body1,
-                                      body2, counts, sms, st);
+    cts::launch_find_contacts<double, false>(
+        bodies<double>(nb, 0, 0, 0, pos, rad, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, eps, body1, body2, nullptr, counts,
+        sms, st);
   CK(cudaGetLastError());
   return 0;
 }
@@ -931,30 +946,25 @@ extern "C" int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    cts::launch_contact_geometry<float>(B, nb, 0, 0, cap, (const float*)pos, (const float*)rad, (const float*)fric,
-                                        (const float*)rest, nullptr, nullptr, nullptr, nullptr, body1, body2, counts,
-                                        (float*)normal, (float*)p1, (float*)p2, (float*)pen, (float*)mu, (float*)rest_c,
-                                        sms, st);
+    cts::launch_contact_geometry<float, false>(bodies<float>(nb, 0, 0, 0, pos, rad, fric, rest, 0, 0, 0, 0, 0, 0, 0, 0),
+                                               B, cap, body1, body2, nullptr, counts, (float*)normal, (float*)p1,
+                                               (float*)p2, (float*)pen, (float*)mu, (float*)rest_c, sms, st);
   else
-    cts::launch_contact_geometry<double>(B, nb, 0, 0, cap, (const double*)pos, (const double*)rad, (const double*)fric,
-                                         (const double*)rest, nullptr, nullptr, nullptr, nullptr, body1, body2, counts,
-                                         (double*)normal, (double*)p1, (double*)p2, (double*)pen, (double*)mu,
-                                         (double*)rest_c, sms, st);
+    cts::launch_contact_geometry<double, false>(
+        bodies<double>(nb, 0, 0, 0, pos, rad, fric, rest, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, body1, body2, nullptr,
+        counts, (double*)normal, (double*)p1, (double*)p2, (double*)pen, (double*)mu, (double*)rest_c, sms, st);
   CK(cudaGetLastError());
   return 0;
 }
 
-template <typename T>
-static void world_contacts_t(int B, int nb, int no, int nv, int cap, double eps, const void* pos, const void* rad,
-                             const void* fric, const void* rest, const void* verts, const void* oref, const void* ofric,
-                             const void* orest, int32_t* body1, int32_t* body2, int32_t* counts, void* normal, void* p1,
-                             void* p2, void* pen, void* mu, void* rest_c, bool geometry, int sms, cudaStream_t st) {
-  cts::launch_find_contacts<T>(B, nb, no, nv, cap, (T)eps, (const T*)pos, (const T*)rad, (const T*)verts, body1, body2,
-                               counts, sms, st);
+template <typename T, bool HULLS>
+static void body_contacts_t(const cts::Bodies<T>& bd, int B, int cap, double eps, int32_t* body1, int32_t* body2,
+                            int32_t* feat, int32_t* counts, void* normal, void* p1, void* p2, void* pen, void* mu,
+                            void* rest_c, bool geometry, int sms, cudaStream_t st) {
+  cts::launch_find_contacts<T, HULLS>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st);
   if (geometry)
-    cts::launch_contact_geometry<T>(B, nb, no, nv, cap, (const T*)pos, (const T*)rad, (const T*)fric, (const T*)rest,
-                                    (const T*)verts, (const T*)oref, (const T*)ofric, (const T*)orest, body1, body2,
-                                    counts, (T*)normal, (T*)p1, (T*)p2, (T*)pen, (T*)mu, (T*)rest_c, sms, st);
+    cts::launch_contact_geometry<T, HULLS>(bd, B, cap, body1, body2, feat, counts, (T*)normal, (T*)p1, (T*)p2, (T*)pen,
+                                           (T*)mu, (T*)rest_c, sms, st);
 }
 
 extern "C" int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, double eps, const void* pos,
@@ -980,11 +990,54 @@ extern "C" int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, 
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    world_contacts_t<float>(B, nb, no, nv, cap, eps, pos, rad, fric, rest, verts, oref, ofric, orest, body1, body2,
-                            counts, normal, p1, p2, pen, mu, rest_c, geometry, sms, st);
+    body_contacts_t<float, false>(bodies<float>(nb, 0, no, nv, pos, rad, fric, rest, 0, 0, 0, 0, verts, oref, ofric,
+                                                orest),
+                                  B, cap, eps, body1, body2, nullptr, counts, normal, p1, p2, pen, mu, rest_c, geometry,
+                                  sms, st);
   else
-    world_contacts_t<double>(B, nb, no, nv, cap, eps, pos, rad, fric, rest, verts, oref, ofric, orest, body1, body2,
-                             counts, normal, p1, p2, pen, mu, rest_c, geometry, sms, st);
+    body_contacts_t<double, false>(bodies<double>(nb, 0, no, nv, pos, rad, fric, rest, 0, 0, 0, 0, verts, oref, ofric,
+                                                  orest),
+                                   B, cap, eps, body1, body2, nullptr, counts, normal, p1, p2, pen, mu, rest_c,
+                                   geometry, sms, st);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                                     const void* pos, const void* rad, const void* fric, const void* rest,
+                                     const void* pverts, const void* pcen, const void* pfric, const void* prest,
+                                     const void* overts, const void* oref, const void* ofric, const void* orest,
+                                     int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
+                                     void* p1, void* p2, void* pen, void* mu, void* rest_c, void* stream) {
+  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
+  if (B < 0 || nb < 0 || np < 0 || no < 0 || cap <= 0 || nb + np <= 0)
+    return fail("body_contacts: need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
+  if (np + no > 0 && (nv < 3 || nv > cts::MAX_NV)) return fail("body_contacts: polygons need 3 <= nv <= 256 vertices");
+  if ((long long)nb + np + no > 0x7fffffffLL) return fail("body_contacts: too many bodies");
+  if ((nb > 0 && (!pos || !rad)) || (np > 0 && (!pverts || !pcen)) || (no > 0 && (!overts || !oref)) || !body1 ||
+      !body2 || !counts || !feat)
+    return fail("body_contacts: NULL argument");
+  const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
+                   (rest_c != nullptr);
+  if (ngeo != 0 && ngeo != 6) return fail("body_contacts: the geometry outputs are all NULL or all non-NULL");
+  const bool geometry = ngeo == 6;
+  if (geometry && ((nb > 0 && (!fric || !rest)) || (np > 0 && (!pfric || !prest)) || (no > 0 && (!ofric || !orest))))
+    return fail("body_contacts: the geometry needs the friction and restitution of every body group");
+  if (B == 0) return 0;
+  int dev = 0, sms = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == LCPB200_F32)
+    body_contacts_t<float, true>(bodies<float>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
+                                               overts, oref, ofric, orest),
+                                 B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c, geometry,
+                                 sms, st);
+  else
+    body_contacts_t<double, true>(bodies<double>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
+                                                 overts, oref, ofric, orest),
+                                  B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c, geometry,
+                                  sms, st);
   CK(cudaGetLastError());
   return 0;
 }

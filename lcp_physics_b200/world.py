@@ -23,11 +23,13 @@ mean of the two bodies (world.py:144-151, :213-224), `eps`, `tol`, `post_stab`, 
 and STATIC convex polygon obstacles -- the reference's `Rect` / `Hull` floors, walls and ramps pinned by a
 `TotalConstraint` (`obstacles=`, `rect_vertices`): a pinned body has zero velocity, so its equality rows are
 eliminated exactly and a contact against it is a one-body contact (body2 >= nb, include/lcpb200.h) whose rows touch
-only the circle's three columns (DESIGN.md section 9). Dynamic hulls, hull-hull contacts, joints between bodies and
-the renderer are not mirrored (SURVEY.md section 8f).
+only the circle's three columns (DESIGN.md section 9), and DYNAMIC convex polygons -- the reference's `Rect` / `Hull`
+bodies (`polygons=`), ordered after the circles and before the obstacles, with the hull-hull contact rule of
+contacts.py:145-292 (SAT + reference-face clipping, 0-2 contacts per pair) detected by lcpb200_body_contacts. Joints
+between bodies and the renderer are not mirrored (SURVEY.md section 8f).
 Everything is differentiable through torch autograd (the LCP through lcpb200_engine_backward). Scenes of up to
-42 bodies (3 nb + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes (BASELINE
-config 4: a 512-ball pile) the banded large-scene kernels (csrc/lcp_banded.cuh), float64.
+42 dynamic bodies (3 (nb + npoly) + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes
+(BASELINE config 4: a 512-ball pile) the banded large-scene kernels (csrc/lcp_banded.cuh), float64.
 """
 import ctypes
 import math
@@ -61,23 +63,25 @@ def polygon_centroid(verts):
     return (cross.unsqueeze(-1) * (a + b)).sum(-2) / (6 * (cross.sum(-1) / 2).unsqueeze(-1))
 
 
-def check_obstacles(verts, B):
+def check_obstacles(verts, B, name="obstacles"):
     """Validates obstacle vertices [no, V, 2] (shared by the batch) or [B, no, V, 2]; returns them as [B, no, V, 2].
     Every polygon must have >= 3 vertices, a non-zero area and be convex (the contact rule of contacts.py:84-144 is
     the one for convex hulls). All polygons share V: a polygon with fewer vertices may repeat one (its zero-length
-    edges are skipped by the contact rule)."""
+    edges are skipped by the contact rule). `name` labels the error messages."""
     v = torch.as_tensor(verts)
     if v.dim() == 3:
         v = v.unsqueeze(0).expand(B, -1, -1, -1)
     if v.dim() != 4 or v.shape[0] != B or v.shape[3] != 2:
-        raise ValueError("obstacles: need vertices [no, V, 2] or [B, no, V, 2] (B = %d), got %s" % (B, tuple(v.shape)))
+        raise ValueError("%s: need vertices [n, V, 2] or [B, n, V, 2] (B = %d), got %s" % (name, B, tuple(v.shape)))
     if v.shape[1] == 0:
-        raise ValueError("obstacles: no polygon given (pass obstacles=None)")
+        raise ValueError("%s: no polygon given (pass %s=None)" % (name, name))
     if v.shape[2] < 3:
-        raise ValueError("obstacles: every polygon needs at least 3 vertices")
+        raise ValueError("%s: every polygon needs at least 3 vertices" % name)
+    if v.shape[2] > 256:
+        raise ValueError("%s: at most 256 vertices per polygon" % name)
     w = v.detach().double()
     if not bool(torch.isfinite(w).all()):
-        raise ValueError("obstacles: non-finite vertex")
+        raise ValueError("%s: non-finite vertex" % name)
     e = torch.roll(w, -1, dims=2) - w
     deg = ~(e.norm(dim=-1) > 0)                          # zero-length edges: a vertex repeated to pad to the common V
     en, found = torch.roll(e, -1, dims=2), ~torch.roll(deg, -1, dims=2)
@@ -90,20 +94,58 @@ def check_obstacles(verts, B):
     turn = torch.where(deg, torch.zeros_like(turn), turn)
     area = (w[..., 0] * torch.roll(w, -1, dims=2)[..., 1] - w[..., 1] * torch.roll(w, -1, dims=2)[..., 0]).sum(-1)
     if bool((area.abs() <= 0).any()):
-        raise ValueError("obstacles: a polygon has zero area")
+        raise ValueError("%s: a polygon has zero area" % name)
     tol = math.sqrt(torch.finfo(v.dtype).eps) if v.is_floating_point() else 1e-8    # coordinates rounded to v.dtype
     if bool(((turn * area.sign().unsqueeze(-1)) < -tol).any()):
-        raise ValueError("obstacles: every polygon must be convex")
+        raise ValueError("%s: every polygon must be convex" % name)
     return v
+
+
+def check_polygons(verts, B):
+    """Validates the vertices of dynamic polygons as check_obstacles does, and their orientation: a `Hull` asserts a
+    positive shoelace area (bodies.py:169, :228-235, `_is_clockwise` in screen coordinates), which makes
+    left_orthogonal(edge) the outward normal the hull-hull rule uses. Returns [B, npoly, V, 2]."""
+    v = check_obstacles(verts, B, name="polygons")
+    w = v.detach().double()
+    area = (w[..., 0] * torch.roll(w, -1, dims=2)[..., 1] - w[..., 1] * torch.roll(w, -1, dims=2)[..., 0]).sum(-1)
+    if bool((area < 0).any()):
+        raise ValueError("polygons: vertices must be in the orientation of positive shoelace area (as Hull asserts); "
+                         "reverse their order")
+    return v
+
+
+def polygon_inertia(rel, mass):
+    """Hull's angular inertia (bodies.py:179-189) of polygons with vertices rel [..., V, 2] about their centroid:
+    m / 6 * sum |v2 x v1| (v1.v1 + v1.v2 + v2.v2) / sum |v2 x v1|; for a rectangle it equals Rect's m (w^2 + h^2) / 12."""
+    a, b = rel, torch.roll(rel, -1, dims=-2)
+    nc = (b[..., 0] * a[..., 1] - b[..., 1] * a[..., 0]).abs()
+    num = (nc * ((a * a).sum(-1) + (a * b).sum(-1) + (b * b).sum(-1))).sum(-1)
+    return mass * num / nc.sum(-1) / 6
+
+
+def _pad_vertices(v, V):
+    """[B, n, V0, 2] -> [B, n, V, 2] (V >= V0) by repeating the last vertex: a zero-length edge, skipped by every rule."""
+    if v.shape[2] == V:
+        return v
+    return torch.cat([v, v[:, :, -1:].expand(-1, -1, V - v.shape[2], -1)], 2)
 
 
 class BatchedWorld:
     def __init__(self, pos, rad, vel=None, mass=1.0, restitution=0.5, fric_coeff=0.9, gravity=10.0,
                  static=(), gravity_mask=None, dt=1.0 / 30, eps=0.1, tol=1e-6, post_stab=False,
                  strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False,
-                 obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5):
-        """pos [B,nb,2], rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass / restitution /
-        fric_coeff [B,nb] (or broadcastable), `static`: indices of bodies pinned by a TotalConstraint,
+                 obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5, polygons=None, poly_rot=0.0, poly_vel=None,
+                 poly_mass=1.0, poly_fric=0.9, poly_rest=0.5):
+        """pos [B,nb,2] (nb may be 0), rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass /
+        restitution / fric_coeff [B,nb] (or broadcastable).
+        `polygons`: dynamic convex polygons, the reference's `Rect` / `Hull` bodies (bodies.py:154-301): world-frame
+        vertices at the initial pose, [npoly, V, 2] (shared by the batch) or [B, npoly, V, 2], in the orientation of
+        positive shoelace area (e.g. `rect_vertices`); `poly_rot`: their initial rotation p[0] ([B, npoly] or
+        broadcastable), `poly_vel` [B, npoly, 3] or None, `poly_mass` / `poly_fric` / `poly_rest` [B, npoly] or
+        broadcastable; all may require grad. A polygon's position is its area centroid and its inertia Hull's.
+        Bodies are ordered [circles (nb), polygons (npoly), obstacles]: p, v, get_p(), get_v(), mass, inertia, fext
+        and the `static` / `gravity_mask` indices cover the nb + npoly dynamic bodies in that order.
+        `static`: indices of bodies pinned by a TotalConstraint,
         `gravity`: g of the `Gravity` force (forces.py) applied to the bodies in gravity_mask
         (default: every non-static body). `exact_adjoint`: backward() through every LCP solve uses the true
         adjoint (the transposed KKT system, DESIGN.md section 3.4); the default False reproduces the reference's
@@ -120,15 +162,37 @@ class BatchedWorld:
         to = lambda t: torch.as_tensor(t, dtype=self.dtype).to(self.device)
         pos = to(pos)
         B, nb, _ = pos.shape
-        self.B, self.nb, self.n = B, nb, 3 * nb
+        self.np = 0
+        if polygons is not None:
+            pv = check_polygons(polygons, B).to(device=self.device, dtype=self.dtype)  # [B,np,V,2], keeps its graph
+            self.np = int(pv.shape[1])
+        nd = nb + self.np                                                           # dynamic bodies
+        if nd == 0:
+            raise ValueError("BatchedWorld: no circle and no polygon given")
+        self.B, self.nb, self.nd, self.n = B, nb, nd, 3 * nd
         bc = lambda t: to(t).expand(B, nb).contiguous() if torch.as_tensor(t).dim() < 2 else to(t)
         self.rad, self.mass = bc(rad), bc(mass)
         self.restitution, self.fric_coeff = bc(restitution), bc(fric_coeff)
         self.inertia = self.mass * self.rad * self.rad / 2                          # bodies.py:126
         self.p = torch.cat([pos.new_zeros(B, nb, 1), pos], 2)                       # (rot, x, y)  bodies.py:27-33
-        self.v = to(vel).reshape(B, self.n).clone() if vel is not None else pos.new_zeros(B, self.n)
+        v0 = to(vel).reshape(B, 3 * nb).clone() if vel is not None else pos.new_zeros(B, 3 * nb)
+        if self.np:
+            bp = lambda t: to(t).expand(B, self.np).contiguous() if torch.as_tensor(t).dim() < 2 else to(t)
+            pmass, rot = bp(poly_mass), bp(poly_rot)
+            self.pfric, self.prest = bp(poly_fric), bp(poly_rest)
+            cen = polygon_centroid(pv)                                              # Hull.pos (bodies.py:170-173)
+            rel = pv - cen.unsqueeze(2)
+            c, s = torch.cos(rot).unsqueeze(2), torch.sin(rot).unsqueeze(2)
+            # Hull.verts at rotation 0: R(-rot) (verts - centroid); every step rotates them by p[0] (bodies.py:202-214)
+            self.plocal = torch.stack([c * rel[..., 0] + s * rel[..., 1], -s * rel[..., 0] + c * rel[..., 1]], 3)
+            self.mass = torch.cat([self.mass, pmass], 1)
+            self.inertia = torch.cat([self.inertia, polygon_inertia(rel, pmass)], 1)
+            self.p = torch.cat([self.p, torch.cat([rot.unsqueeze(2), cen], 2)], 1)
+            pvel = to(poly_vel).reshape(B, 3 * self.np) if poly_vel is not None else pos.new_zeros(B, 3 * self.np)
+            v0 = torch.cat([v0, pvel], 1)
+        self.v = v0
         self.static = [int(k) for k in static]
-        gm = torch.ones(nb, dtype=torch.bool)
+        gm = torch.ones(nd, dtype=torch.bool)
         gm[self.static] = False
         if gravity_mask is not None:
             gm = torch.as_tensor(gravity_mask, dtype=torch.bool)
@@ -155,19 +219,29 @@ class BatchedWorld:
             bo = lambda t: to(t).expand(B, self.no).contiguous() if torch.as_tensor(t).dim() < 2 else to(t)
             self.ofric, self.orest = bo(obstacle_fric), bo(obstacle_rest)
             self.oref = polygon_centroid(self.ov)                                   # Hull.pos (bodies.py:166-173)
-        nt = nb + self.no
+        if self.np:
+            self.nv = max(self.nv, int(pv.shape[2]))                                # one common V for both groups
+            self.plocal = _pad_vertices(self.plocal, self.nv)
+            if self.no:
+                self.ov = _pad_vertices(self.ov, self.nv)
+        nt = nd + self.no
         ii, jj = torch.triu_indices(nt, nt, 1)
         if self.no:
-            keep = ii < nb                                                          # obstacles never pair up
+            keep = ii < nd                                                          # obstacles never pair up
             ii, jj = ii[keep], jj[keep]
         self.pi, self.pj = ii.to(self.device), jj.to(self.device)                   # pair (i, j), i < j, lexicographic
-        self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), (4 if self.no else 3) * nb)
-        # 3 nb + 3 n_static <= 128 and <= 256 contacts: condensed-KKT kernels (fp32 / fp64, differentiable);
-        # larger scenes: the banded large-scene kernels (fp64; lcp_banded.cuh)
+        if self.np:
+            # a polygon-polygon or polygon-obstacle pair may give 2 contacts
+            most = int(self.pi.numel()) + int((self.pi >= nb).sum())
+            self.cap = int(contact_capacity) if contact_capacity else max(1, min(most, (4 if self.no else 3) * nb + 8 * self.np))
+        else:
+            self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), (4 if self.no else 3) * nb)
+        # 3 (nb + npoly) + 3 n_static <= 128 and <= 256 contacts: condensed-KKT kernels (fp32 / fp64,
+        # differentiable); larger scenes: the banded large-scene kernels (fp64; lcp_banded.cuh)
         self.large = self.n + self.ne > 128 or 4 * self.cap > 1024
         if self.large and (self.dtype != torch.float64 or self.ne > 16):
-            raise ValueError("BatchedWorld: scenes with 3 nb + 3 n_static > 128 (or > 256 contacts) need float64 "
-                             "and at most 5 pinned bodies (static obstacles do not count)")
+            raise ValueError("BatchedWorld: scenes with 3 (nb + npoly) + 3 n_static > 128 (or > 256 contacts) need "
+                             "float64 and at most 5 pinned bodies (static obstacles do not count)")
         self.t = pos.new_zeros(B)
         self.find_contacts()
         if self.strict_no_pen and bool((self.max_penetration() > self.tol).any()):
@@ -178,6 +252,8 @@ class BatchedWorld:
         """Pair test + ordered compaction on the GPU (lcpb200_find_contacts: all nb (nb - 1) / 2 pairs of every
         scene, lexicographic order = the reference's contact order), then the contact geometry of the selected
         pairs with torch ops (differentiable w.r.t. the positions)."""
+        if self.np:
+            return self._find_contacts_bodies()
         if self.no:
             return self._find_contacts_obstacles()
         lib = _lib.load()
@@ -259,11 +335,106 @@ class BatchedWorld:
         valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
         self.c_pen = torch.where(valid, pen, pen.new_full((), -1e30))
 
-    def _circle_polygon_torch(self, c, k):
-        """Torch mirror of csrc/lcp_contacts.cuh circle_polygon for circle centres c [B,P,2] against obstacles
-        k [B,P] (long): (inside, closest point q, squared distance, separating-edge normal, separation)."""
+    def polygon_vertices(self):
+        """World-frame vertices [B, npoly, V, 2] of the dynamic polygons at the current p: centroid + R(rot) local
+        (Hull.set_p / rotate_verts, bodies.py:202-214), differentiable in p and the polygons' initial vertices."""
+        q = self.p[:, self.nb:]
+        c, s = torch.cos(q[:, :, 0:1]), torch.sin(q[:, :, 0:1])
+        lx, ly = self.plocal[..., 0], self.plocal[..., 1]
+        return torch.stack([q[:, :, 1:2] + (c * lx - s * ly), q[:, :, 2:3] + (s * lx + c * ly)], 3)
+
+    def _find_contacts_bodies(self):
+        """find_contacts for worlds with dynamic polygons: lcpb200_body_contacts walks the pairs of the body list
+        [circles..., polygons..., obstacles...] (circle-circle, circle-polygon and hull-hull rules; 0-2 contacts per
+        pair) and returns each hull-hull contact's features; the geometry comes from the same call, or from torch ops
+        that rebuild it from those features (_geometry_torch) when something needs autograd."""
+        lib = _lib.load()
+        B, cap, dev, nb = self.B, self.cap, self.device, self.nb
+        pverts = self.polygon_vertices()
+        pcen = self.p[:, nb:, 1:]
+        b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        feat = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        counts = torch.empty(B, dtype=torch.int32, device=dev)
+        obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
+        needs_graph = torch.is_grad_enabled() and any(
+            t is not None and t.requires_grad
+            for t in (self.p, self.rad, self.fric_coeff, self.restitution, self.plocal, self.pfric, self.prest) + obst)
+        d = lambda t: t.detach().contiguous() if t is not None else None
+        geo = [None] * 6
+        if not needs_graph:
+            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+            geo = [new(2), new(2), new(2), new(), new(), new()]
+        # contiguous copies held until the call returns (a temporary's memory could be reused before the kernel runs)
+        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen, self.pfric,
+                              self.prest) + obst]
+        with torch.cuda.device(dev):
+            _lib.check(lib.lcpb200_body_contacts(
+                _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps, *[_lib.ptr(t) for t in ins],
+                _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat), *[_lib.ptr(t) for t in geo],
+                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        if int(counts.max()) > cap:
+            raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
+        self.c_b1, self.c_b2, self.c_feat, self.counts = b1, b2, feat, counts
+        if not needs_graph:
+            self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest = geo
+            return
+        self.c_normal, self.c_p1, self.c_p2, pen, self.c_mu, self.c_rest = self._geometry_torch(b1, b2, feat, pverts)
+        valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
+        self.c_pen = torch.where(valid, pen, pen.new_full((), -1e30))
+
+    def _hull_torch(self, i1, i2, feat, verts, ref):
+        """Torch mirror of the hull-hull geometry of csrc/lcp_contacts.cuh (contacts.py:156-201, clip_segment_to_line
+        :270-292) for the pairs (i1, i2) [B,C] of polygon bodies, REBUILT FROM THE KERNEL'S FEATURES feat [B,C] (which
+        body holds the reference face, reference and incident edges, the first clip's outcome, which clipped point),
+        so the graph path and the kernel path cannot select different features. verts [B,P,V,2] / ref [B,P,2]: the
+        polygons [dynamic..., obstacles...] and their centroids. Returns normal, p1, p2, penetration."""
+        nb, V = self.nb, self.nv
+        P = verts.shape[1]
+        f = feat.long().clamp_min(0)
+        kind, clip1, ref2 = f & 3, (f >> 2) & 3, ((f >> 4) & 1).bool()
+        re, ie = (f >> 5) & 255, (f >> 13) & 255
+        k1, k2 = (i1 - nb).clamp(0, P - 1), (i2 - nb).clamp(0, P - 1)
+        kr, ki = torch.where(ref2, k2, k1), torch.where(ref2, k1, k2)
+        poly = lambda k: torch.gather(verts, 1, k.unsqueeze(2).unsqueeze(3).expand(-1, -1, V, 2))   # [B,C,V,2]
+        Vr, Vi = poly(kr), poly(ki)
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+        cr, ci = take2(ref, kr), take2(ref, ki)
+        vtx = lambda Vx, e: torch.gather(Vx, 2, e.unsqueeze(2).unsqueeze(3).expand(-1, -1, 1, 2)).squeeze(2)
+        Wr = torch.roll(Vr, -1, dims=2)
+        area = (Vr[..., 0] * Wr[..., 1] - Vr[..., 1] * Wr[..., 0]).sum(2)
+        orient = torch.where(area > 0, 1.0, -1.0).to(verts.dtype)
+        E = vtx(Vr, (re + 1) % V) - vtx(Vr, re)
+        ln = E.norm(dim=2)
+        ln1 = torch.where(ln > 0, ln, torch.ones_like(ln))
+        n = torch.stack([orient * E[..., 1] / ln1, -orient * E[..., 0] / ln1], 2)   # outward normal of the reference edge
+        r = vtx(Vr, re) - cr
+        h = (ln / 2).unsqueeze(2)
+        v0, v1 = vtx(Vi, ie) - cr, vtx(Vi, (ie + 1) % V) - cr                        # incident edge, reference frame
+        cp = torch.stack([n[..., 1], -n[..., 0]], 2)                                # clip plane left_orthogonal(n)
+        dot = lambda a, b: (a * b).sum(2, keepdim=True)
+        safe = lambda x: torch.where(x != 0, x, torch.ones_like(x))
+        d0, d1 = dot(cp, v0) + h, dot(cp, v1) + h
+        c1 = v0 + d0 / safe(d0 - d1) * (v1 - v0)
+        a = torch.where((clip1 == 2).unsqueeze(2), v1, v0)
+        b = torch.where((clip1 == 0).unsqueeze(2), v1, c1)
+        e0, e1 = dot(-cp, a) + h, dot(-cp, b) + h
+        c2 = a + e0 / safe(e0 - e1) * (b - a)
+        k_ = kind.unsqueeze(2)
+        v = torch.where(k_ == 0, v0, torch.where(k_ == 1, v1, torch.where(k_ == 2, c1, c2)))
+        dist = dot(n, v - r)
+        q = v + n * -dist                                                           # on the reference edge's line
+        s = q + cr - ci
+        w = ref2.unsqueeze(2)
+        return torch.where(w, n, -n), torch.where(w, s, q), torch.where(w, q, s), -dist.squeeze(2)
+
+    def _circle_polygon_torch(self, c, k, verts=None):
+        """Torch mirror of csrc/lcp_contacts.cuh circle_polygon for circle centres c [B,P,2] against polygons
+        k [B,P] (long) of verts (default: the obstacles): (inside, closest point q, squared distance, separating-edge
+        normal, separation)."""
         B, P = k.shape
-        V = torch.gather(self.ov, 1, k.reshape(B, P, 1, 1).expand(B, P, self.nv, 2))       # [B,P,V,2]
+        verts = self.ov if verts is None else verts
+        V = torch.gather(verts, 1, k.reshape(B, P, 1, 1).expand(B, P, self.nv, 2))          # [B,P,V,2]
         Wv = torch.roll(V, -1, dims=2)
         E = Wv - V
         area = (V[..., 0] * Wv[..., 1] - V[..., 1] * Wv[..., 0]).sum(2)
@@ -286,18 +457,34 @@ class BatchedWorld:
         sep = torch.gather(sp, 2, es).squeeze(2)
         return inside, q, torch.gather(d2, 2, em).squeeze(2), n_in, sep
 
-    def _geometry_torch(self, b1, b2):
+    def _geometry_torch(self, b1, b2, feat=None, pverts=None):
         """Differentiable geometry and material of the selected pairs (circle-circle: contacts.py:69-77;
-        circle-obstacle: contacts.py:84-144, as lcpb200_world_contacts), gradients reaching positions, radii,
-        materials and the obstacle vertices."""
+        circle-polygon: contacts.py:84-144, as lcpb200_world_contacts; hull-hull: _hull_torch, from the kernel's
+        features feat), gradients reaching positions, radii, materials and the polygon / obstacle vertices.
+        pverts: the dynamic polygons' world-frame vertices (worlds with polygons)."""
         nb = self.nb
         pos = self.p[:, :, 1:]
         i1, i2 = b1.long(), b2.long()
+        take = lambda t, idx: torch.gather(t, 1, idx)
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+        if self.np:                                  # polygon k of body nb + k: [dynamic polygons..., obstacles...]
+            cat = lambda a, b: torch.cat([a, b], 1) if self.no else a
+            polys, pref = cat(pverts, self.ov if self.no else None), cat(pos[:, nb:], self.oref if self.no else None)
+            pfr = cat(self.pfric, self.ofric if self.no else None)
+            prs = cat(self.prest, self.orest if self.no else None)
+            hh = i1 >= nb
+            n_h, p1_h, p2_h, pen_h = self._hull_torch(i1, i2, feat, polys, pref)
+            kh1 = (i1 - nb).clamp_min(0)
+            mu_h = 0.5 * (take(pfr, kh1) + take(pfr, (i2 - nb).clamp_min(0)))
+            rest_h = 0.5 * (take(prs, kh1) + take(prs, (i2 - nb).clamp_min(0)))
+            if nb == 0:
+                return n_h, p1_h, p2_h, pen_h, mu_h, rest_h
+            i1 = torch.where(hh, 0, i1)
+        else:
+            polys, pref, pfr, prs = self.ov, self.oref, self.ofric, self.orest
         cc = i2 < nb
         j = torch.where(cc, i2, 0)
         k = torch.where(cc, 0, i2 - nb)
-        take = lambda t, idx: torch.gather(t, 1, idx)
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         c = take2(pos, i1)
         r1 = take(self.rad, i1)
         one = torch.zeros_like(c)
@@ -310,8 +497,8 @@ class BatchedWorld:
         n_cc = dcc / dist.unsqueeze(2)
         p1_cc = -n_cc * (r1 - pen_cc / 2).unsqueeze(2)
         p2_cc = n_cc * (r2 - pen_cc / 2).unsqueeze(2)
-        # circle-obstacle
-        inside, q, _, n_in, sep = self._circle_polygon_torch(c, k)
+        # circle-obstacle / circle-polygon
+        inside, q, _, n_in, sep = self._circle_polygon_torch(c, k, polys)
         out = ~cc & ~inside
         dq = torch.where(out.unsqueeze(2), c - q, one)
         dq_n = dq.norm(dim=2)
@@ -319,21 +506,28 @@ class BatchedWorld:
         pen_co = torch.where(inside, r1 - sep, r1 - dq_n)
         q_co = torch.where(inside.unsqueeze(2), c - n_in * sep.unsqueeze(2), q)   # best_pt2 = center - n (dist + rad)
         p1_co = q_co - c
-        p2_co = q_co - take2(self.oref, k)
+        p2_co = q_co - take2(pref, k)
         w = cc.unsqueeze(2)
         normal = torch.where(w, n_cc, n_co)
         p1 = torch.where(w, p1_cc, p1_co)
         p2 = torch.where(w, p2_cc, p2_co)
         pen = torch.where(cc, pen_cc, pen_co)
         f1, e1 = take(self.fric_coeff, i1), take(self.restitution, i1)
-        mu = 0.5 * (f1 + torch.where(cc, take(self.fric_coeff, j), take(self.ofric, k)))          # world.py:213-224
-        rest = 0.5 * (e1 + torch.where(cc, take(self.restitution, j), take(self.orest, k)))       # world.py:144-151
+        mu = 0.5 * (f1 + torch.where(cc, take(self.fric_coeff, j), take(pfr, k)))          # world.py:213-224
+        rest = 0.5 * (e1 + torch.where(cc, take(self.restitution, j), take(prs, k)))       # world.py:144-151
+        if self.np:
+            h = hh.unsqueeze(2)
+            return (torch.where(h, n_h, normal), torch.where(h, p1_h, p1), torch.where(h, p2_h, p2),
+                    torch.where(hh, pen_h, pen), torch.where(hh, mu_h, mu), torch.where(hh, rest_h, rest))
         return normal, p1, p2, pen, mu, rest
 
     def find_contacts_torch(self):
         """The same contact list with torch ops only (O(nb^2) tensors, a stable sort for the compaction): the
         independent implementation tests/test_gpu_world.py checks lcpb200_find_contacts against (and
-        tests/test_gpu_obstacles.py lcpb200_world_contacts). Returns (counts, b1, b2)."""
+        tests/test_gpu_obstacles.py lcpb200_world_contacts). Returns (counts, b1, b2). Not available for worlds with
+        dynamic polygons: their hull-hull rule is checked against the CPU oracle (oracle/polygon_oracle.py)."""
+        if self.np:
+            raise NotImplementedError("find_contacts_torch: worlds with dynamic polygons (see oracle/polygon_oracle.py)")
         pos = self.p[:, :, 1:]
         if self.no:
             nb = self.nb
@@ -392,7 +586,7 @@ class BatchedWorld:
         dts = self.v.new_full((self.B,), float(dt))
         done = torch.zeros(self.B, dtype=torch.bool, device=self.device)
         while True:
-            moved = start_p + self.v.reshape(self.B, self.nb, 3) * dts.reshape(self.B, 1, 1)      # body.move(dt)
+            moved = start_p + self.v.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)      # body.move(dt)
             self.p = torch.where(done.reshape(self.B, 1, 1), self.p, moved)
             self.find_contacts()
             ok = self.max_penetration() <= self.tol
@@ -405,7 +599,7 @@ class BatchedWorld:
         if self.post_stab:
             tmp_v = self.v
             dp = self.post_stabilization() / 2                                     # world.py:111-112
-            self.p = self.p + dp.reshape(self.B, self.nb, 3) * dts.reshape(self.B, 1, 1)
+            self.p = self.p + dp.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)
             self.v = tmp_v
             self.find_contacts()
         self.t = self.t + dts
