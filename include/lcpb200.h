@@ -234,6 +234,22 @@ int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int 
                           int32_t* feat, void* normal, void* p1, void* p2, void* penetration, void* mu,
                           void* restitution_c, void* stream);
 
+/* lcpb200_body_contacts with pairs excluded from contact (the reference's Body.add_no_contact: contacts.py:60 returns
+ * before any rule when `geom1 in geom2.no_contact`). The arguments are those of lcpb200_body_contacts, plus
+ *   no_contact   const uint32_t[ceil(nt * nt / 32)], shared by the batch (device): bit i * nt + j (bit k is bit
+ *                k % 32 of word k / 32), i < j, nt = nb + np + no, set iff the pair (i, j) of the body list never
+ *                makes contact. Only bits with i < j are read; a pair of two obstacles is never visited anyway.
+ * An excluded pair gives no contact and no rule is evaluated for it: the contacts, their order, feat and the geometry
+ * are those of lcpb200_body_contacts with the excluded pairs' contacts removed. Covers every world kind (np == 0 and /
+ * or no == 0 included). */
+int lcpb200_body_contacts_masked(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                                 const void* pos, const void* rad, const void* fric, const void* rest,
+                                 const void* pverts, const void* pcen, const void* pfric, const void* prest,
+                                 const void* overts, const void* oref, const void* ofric, const void* orest,
+                                 int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
+                                 void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
+                                 const uint32_t* no_contact, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

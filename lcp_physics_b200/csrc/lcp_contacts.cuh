@@ -20,7 +20,9 @@
 //     reference-face clipping): 0, 1 or 2 contacts per pair, stored in the order of the clipped points;
 //   * obstacles never pair with each other.
 // The walk is templated on HULLS: HULLS == false is the walk of lcpb200_find_contacts (no == 0) and
-// lcpb200_world_contacts (circles and obstacles, np == 0), one contact per pair at most.
+// lcpb200_world_contacts (circles and obstacles, np == 0), one contact per pair at most. MASK == true
+// (lcpb200_body_contacts_masked) reads a pair-exclusion bitmask shared by the batch and skips an excluded pair before
+// any rule is evaluated, as the reference's `if geom1 in geom2.no_contact: return` (contacts.py:60, add_no_contact).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -275,10 +277,13 @@ __host__ __device__ int hull_hull(const T* __restrict__ P1, const T* __restrict_
 // One CTA per scene walks the pairs (i, j), i < j, i < nb + np (a dynamic body), j < nb + np + no, in lexicographic
 // order; obstacles never pair with each other. Each pair yields 0, 1 or 2 contacts (HULLS == false: 0 or 1).
 // feat [B, cap] (HULLS only, may be nullptr): the hull-hull features, -1 for every other contact.
-template <typename T, bool HULLS>
+// no_contact (MASK only): bit i * nt + j (i < j, nt = nb + np + no) set iff the pair (i, j) never makes contact; an
+// excluded pair sets no hit bit, so the compaction keeps the order of the remaining pairs.
+template <typename T, bool HULLS, bool MASK = false>
 __global__ void __launch_bounds__(NT) find_contacts_kernel(Bodies<T> bd, int B, int cap, T eps,
                                                            int32_t* __restrict__ body1, int32_t* __restrict__ body2,
-                                                           int32_t* __restrict__ feat, int32_t* __restrict__ counts) {
+                                                           int32_t* __restrict__ feat, int32_t* __restrict__ counts,
+                                                           const uint32_t* __restrict__ no_contact = nullptr) {
   __shared__ int warp_tot[NT / 32];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nb = bd.nb, nv = bd.nv;
@@ -312,7 +317,14 @@ __global__ void __launch_bounds__(NT) find_contacts_kernel(Bodies<T> bd, int B, 
       for (int u = 0; u < ITEMS; ++u) {
         pi[u] = i; pj[u] = j;
         if (q + u < npairs) {
-          if (j < nb) {
+          bool skip = false;
+          if constexpr (MASK) {
+            const long long bit = (long long)i * nt + j;
+            skip = (__ldg(no_contact + (bit >> 5)) >> (bit & 31)) & 1u;
+          }
+          if (skip) {
+            if constexpr (HULLS) f[2 * u] = -1;
+          } else if (j < nb) {
             const T dx = P[2 * i] - P[2 * j], dy = P[2 * i + 1] - P[2 * j + 1];
             const T dist = sqrt(dx * dx + dy * dy);
             const T pen = R[i] + R[j] - dist;                    // contacts.py:70-73
@@ -464,11 +476,12 @@ static void launch_contact_geometry(const Bodies<T>& bd, int B, int cap, const i
                                                                pen, mu, rest_c);
 }
 
-template <typename T, bool HULLS>
+template <typename T, bool HULLS, bool MASK = false>
 static void launch_find_contacts(const Bodies<T>& bd, int B, int cap, T eps, int32_t* body1, int32_t* body2,
-                                 int32_t* feat, int32_t* counts, int num_sms, cudaStream_t st) {
+                                 int32_t* feat, int32_t* counts, int num_sms, cudaStream_t st,
+                                 const uint32_t* no_contact = nullptr) {
   const int grid = B < 8 * num_sms ? B : 8 * num_sms;
-  find_contacts_kernel<T, HULLS><<<grid, NT, 0, st>>>(bd, B, cap, eps, body1, body2, feat, counts);
+  find_contacts_kernel<T, HULLS, MASK><<<grid, NT, 0, st>>>(bd, B, cap, eps, body1, body2, feat, counts, no_contact);
 }
 
 }  // namespace cts

@@ -957,11 +957,12 @@ extern "C" int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const
   return 0;
 }
 
-template <typename T, bool HULLS>
+template <typename T, bool HULLS, bool MASK = false>
 static void body_contacts_t(const cts::Bodies<T>& bd, int B, int cap, double eps, int32_t* body1, int32_t* body2,
                             int32_t* feat, int32_t* counts, void* normal, void* p1, void* p2, void* pen, void* mu,
-                            void* rest_c, bool geometry, int sms, cudaStream_t st) {
-  cts::launch_find_contacts<T, HULLS>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st);
+                            void* rest_c, bool geometry, int sms, cudaStream_t st,
+                            const uint32_t* no_contact = nullptr) {
+  cts::launch_find_contacts<T, HULLS, MASK>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st, no_contact);
   if (geometry)
     cts::launch_contact_geometry<T, HULLS>(bd, B, cap, body1, body2, feat, counts, (T*)normal, (T*)p1, (T*)p2, (T*)pen,
                                            (T*)mu, (T*)rest_c, sms, st);
@@ -1003,43 +1004,69 @@ extern "C" int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, 
   return 0;
 }
 
-extern "C" int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
-                                     const void* pos, const void* rad, const void* fric, const void* rest,
-                                     const void* pverts, const void* pcen, const void* pfric, const void* prest,
-                                     const void* overts, const void* oref, const void* ofric, const void* orest,
-                                     int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
-                                     void* p1, void* p2, void* pen, void* mu, void* rest_c, void* stream) {
+// lcpb200_body_contacts and lcpb200_body_contacts_masked: one argument check, the walk with or without the mask
+template <bool MASK>
+static int body_contacts_impl(const char* name, int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                              const void* pos, const void* rad, const void* fric, const void* rest, const void* pverts,
+                              const void* pcen, const void* pfric, const void* prest, const void* overts,
+                              const void* oref, const void* ofric, const void* orest, int32_t* body1, int32_t* body2,
+                              int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2, void* pen, void* mu,
+                              void* rest_c, const uint32_t* no_contact, void* stream) {
+  const std::string nm(name);
   if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
   if (B < 0 || nb < 0 || np < 0 || no < 0 || cap <= 0 || nb + np <= 0)
-    return fail("body_contacts: need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
-  if (np + no > 0 && (nv < 3 || nv > cts::MAX_NV)) return fail("body_contacts: polygons need 3 <= nv <= 256 vertices");
-  if ((long long)nb + np + no > 0x7fffffffLL) return fail("body_contacts: too many bodies");
+    return fail(nm + ": need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
+  if (np + no > 0 && (nv < 3 || nv > cts::MAX_NV)) return fail(nm + ": polygons need 3 <= nv <= 256 vertices");
+  if ((long long)nb + np + no > 0x7fffffffLL) return fail(nm + ": too many bodies");
   if ((nb > 0 && (!pos || !rad)) || (np > 0 && (!pverts || !pcen)) || (no > 0 && (!overts || !oref)) || !body1 ||
-      !body2 || !counts || !feat)
-    return fail("body_contacts: NULL argument");
+      !body2 || !counts || !feat || (MASK && !no_contact))
+    return fail(nm + ": NULL argument");
   const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
                    (rest_c != nullptr);
-  if (ngeo != 0 && ngeo != 6) return fail("body_contacts: the geometry outputs are all NULL or all non-NULL");
+  if (ngeo != 0 && ngeo != 6) return fail(nm + ": the geometry outputs are all NULL or all non-NULL");
   const bool geometry = ngeo == 6;
   if (geometry && ((nb > 0 && (!fric || !rest)) || (np > 0 && (!pfric || !prest)) || (no > 0 && (!ofric || !orest))))
-    return fail("body_contacts: the geometry needs the friction and restitution of every body group");
+    return fail(nm + ": the geometry needs the friction and restitution of every body group");
   if (B == 0) return 0;
   int dev = 0, sms = 0;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == LCPB200_F32)
-    body_contacts_t<float, true>(bodies<float>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
-                                               overts, oref, ofric, orest),
-                                 B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c, geometry,
-                                 sms, st);
+    body_contacts_t<float, true, MASK>(bodies<float>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
+                                                     overts, oref, ofric, orest),
+                                       B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c,
+                                       geometry, sms, st, no_contact);
   else
-    body_contacts_t<double, true>(bodies<double>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
-                                                 overts, oref, ofric, orest),
-                                  B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c, geometry,
-                                  sms, st);
+    body_contacts_t<double, true, MASK>(bodies<double>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric,
+                                                       prest, overts, oref, ofric, orest),
+                                        B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c,
+                                        geometry, sms, st, no_contact);
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                                     const void* pos, const void* rad, const void* fric, const void* rest,
+                                     const void* pverts, const void* pcen, const void* pfric, const void* prest,
+                                     const void* overts, const void* oref, const void* ofric, const void* orest,
+                                     int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
+                                     void* p1, void* p2, void* pen, void* mu, void* rest_c, void* stream) {
+  return body_contacts_impl<false>("body_contacts", dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts,
+                                   pcen, pfric, prest, overts, oref, ofric, orest, body1, body2, counts, feat, normal,
+                                   p1, p2, pen, mu, rest_c, nullptr, stream);
+}
+
+extern "C" int lcpb200_body_contacts_masked(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                                            const void* pos, const void* rad, const void* fric, const void* rest,
+                                            const void* pverts, const void* pcen, const void* pfric, const void* prest,
+                                            const void* overts, const void* oref, const void* ofric, const void* orest,
+                                            int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat,
+                                            void* normal, void* p1, void* p2, void* pen, void* mu, void* rest_c,
+                                            const uint32_t* no_contact, void* stream) {
+  return body_contacts_impl<true>("body_contacts_masked", dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest,
+                                  pverts, pcen, pfric, prest, overts, oref, ofric, orest, body1, body2, counts, feat,
+                                  normal, p1, p2, pen, mu, rest_c, no_contact, stream);
 }
 
 extern "C" int lcpb200_assemble(int dtype, int B, int nb, int nc, double dt, const void* mass, const void* inertia,

@@ -25,8 +25,11 @@ and STATIC convex polygon obstacles -- the reference's `Rect` / `Hull` floors, w
 eliminated exactly and a contact against it is a one-body contact (body2 >= nb, include/lcpb200.h) whose rows touch
 only the circle's three columns (DESIGN.md section 9), and DYNAMIC convex polygons -- the reference's `Rect` / `Hull`
 bodies (`polygons=`), ordered after the circles and before the obstacles, with the hull-hull contact rule of
-contacts.py:145-292 (SAT + reference-face clipping, 0-2 contacts per pair) detected by lcpb200_body_contacts. Joints
-between bodies and the renderer are not mirrored (SURVEY.md section 8f).
+contacts.py:145-292 (SAT + reference-face clipping, 0-2 contacts per pair) detected by lcpb200_body_contacts, and
+CONSTRAINTS between bodies (`constraints=`: `Joint`, `FixedJoint`, `XConstraint`, `YConstraint`, `RotConstraint`,
+constraints.py:13-173) as equality rows of the engine's LCP, rebuilt with torch ops at every engine call, pairs excluded
+from contact (`no_contact=`, Body.add_no_contact: skipped in the GPU pair walk, lcpb200_body_contacts_masked) and
+time-dependent external forces (`external_force=`, forces.py ExternalForce). The renderer is not mirrored.
 Everything is differentiable through torch autograd (the LCP through lcpb200_engine_backward). Scenes of up to
 42 dynamic bodies (3 (nb + npoly) + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes
 (BASELINE config 4: a 512-ball pile) the banded large-scene kernels (csrc/lcp_banded.cuh), float64.
@@ -123,6 +126,68 @@ def polygon_inertia(rel, mass):
     return mass * num / nc.sum(-1) / 6
 
 
+# ------------------------------------------------------------------ constraints.py:13-173, by body index
+class Joint:
+    """Revolute joint (constraints.py:13-53) between bodies i and j (j None: a joint to the world point `anchor`) at
+    `anchor`, [2] (shared by the batch) or [B, 2], which may require grad. 2 equality rows."""
+    num_constraints = 2
+
+    def __init__(self, i, j, anchor):
+        self.i, self.j, self.anchor = i, j, anchor
+
+    def bodies(self):
+        return (self.i,) if self.j is None else (self.i, self.j)
+
+
+class FixedJoint:
+    """Fixed joint (constraints.py:56-92): welds body j to body i. 3 equality rows."""
+    num_constraints = 3
+
+    def __init__(self, i, j):
+        self.i, self.j = i, j
+
+    def bodies(self):
+        return (self.i, self.j)
+
+
+class _AxisConstraint:
+    num_constraints = 1
+    dof = None                                    # the constrained coordinate of (rot, x, y)
+
+    def __init__(self, i):
+        self.i, self.j = i, None
+
+    def bodies(self):
+        return (self.i,)
+
+
+class XConstraint(_AxisConstraint):
+    """Prevents motion along x (constraints.py:122-146): the row [0, 1, 0] on body i."""
+    dof = 1
+
+
+class YConstraint(_AxisConstraint):
+    """Prevents motion along y (constraints.py:95-119): the row [0, 0, 1] on body i."""
+    dof = 2
+
+
+class RotConstraint(_AxisConstraint):
+    """Prevents rotation (constraints.py:149-173): the row [1, 0, 0] on body i."""
+    dof = 0
+
+
+def _cart_to_polar(v):
+    """utils.py:75-82 (positive=True) per scene: r, theta of v [B, 2], theta in [0, 2 pi)."""
+    r = v.norm(dim=1)
+    th = torch.atan2(v[:, 1], v[:, 0])
+    return r, torch.where(th < 0, th + 2 * math.pi, th)
+
+
+def _polar_to_cart(r, th):
+    """utils.py:85-90 per scene: [B, 2]."""
+    return torch.stack([torch.cos(th) * r, torch.sin(th) * r], 1)
+
+
 def _pad_vertices(v, V):
     """[B, n, V0, 2] -> [B, n, V, 2] (V >= V0) by repeating the last vertex: a zero-length edge, skipped by every rule."""
     if v.shape[2] == V:
@@ -135,7 +200,8 @@ class BatchedWorld:
                  static=(), gravity_mask=None, dt=1.0 / 30, eps=0.1, tol=1e-6, post_stab=False,
                  strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False,
                  obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5, polygons=None, poly_rot=0.0, poly_vel=None,
-                 poly_mass=1.0, poly_fric=0.9, poly_rest=0.5):
+                 poly_mass=1.0, poly_fric=0.9, poly_rest=0.5, constraints=None, no_contact=None,
+                 external_force=None):
         """pos [B,nb,2] (nb may be 0), rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass /
         restitution / fric_coeff [B,nb] (or broadcastable).
         `polygons`: dynamic convex polygons, the reference's `Rect` / `Hull` bodies (bodies.py:154-301): world-frame
@@ -154,7 +220,13 @@ class BatchedWorld:
         [B, no, V, 2] (e.g. `rect_vertices`; a polygon with fewer than V vertices repeats one); they may require
         grad. They act as the reference's pinned `Rect` / `Hull` bodies listed AFTER the circles: contact order,
         rule and material are those of such a World.
-        `obstacle_fric` / `obstacle_rest`: their friction / restitution, [B,no] or broadcastable."""
+        `obstacle_fric` / `obstacle_rest`: their friction / restitution, [B,no] or broadcastable.
+        `constraints`: `Joint` / `FixedJoint` / `XConstraint` / `YConstraint` / `RotConstraint` specs naming dynamic
+        bodies by index (topology shared by the batch); their equality rows follow the `static` pins' rows, in list
+        order. `no_contact`: pairs (a, b) of indices in [circles, polygons, obstacles] that never make contact
+        (Body.add_no_contact), shared by the batch; joints do not imply it. `external_force`: f(t) -> [B, nd, 3]
+        (rot, x, y) given the per-scene time t [B], evaluated once per step at its start and added to gravity
+        (ExternalForce); gradients reach whatever f closes over."""
         _lib.require_cuda()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         pos = torch.as_tensor(pos)
@@ -200,6 +272,8 @@ class BatchedWorld:
         if gravity is not None:
             self.fext[:, 2::3] = self.mass * float(gravity) * gm.to(self.device).to(self.dtype)   # Gravity: DOWN * m * g
         self.ne = 3 * len(self.static)
+        self.cons = list(constraints) if constraints is not None else []
+        self.external_force = external_force
         if self.ne:
             A = pos.new_zeros(self.ne, self.n)
             for r, k in enumerate(self.static):
@@ -230,6 +304,10 @@ class BatchedWorld:
             keep = ii < nd                                                          # obstacles never pair up
             ii, jj = ii[keep], jj[keep]
         self.pi, self.pj = ii.to(self.device), jj.to(self.device)                   # pair (i, j), i < j, lexicographic
+        self._init_constraints(to)
+        self.nc_mask = None
+        if no_contact is not None:
+            self._init_no_contact(no_contact, nt)
         if self.np:
             # a polygon-polygon or polygon-obstacle pair may give 2 contacts
             most = int(self.pi.numel()) + int((self.pi >= nb).sum())
@@ -239,6 +317,14 @@ class BatchedWorld:
         # 3 (nb + npoly) + 3 n_static <= 128 and <= 256 contacts: condensed-KKT kernels (fp32 / fp64,
         # differentiable); larger scenes: the banded large-scene kernels (fp64; lcp_banded.cuh)
         self.large = self.n + self.ne > 128 or 4 * self.cap > 1024
+        if self.large and self.cons:
+            # the banded kernel holds the equality rows and every body they touch in a border of <= 16 rows
+            touched = set(self.static) | {k for c in self.cons for k in c.bodies()}
+            border = 3 * len(touched) + self.ne
+            if border > 16:
+                raise ValueError("BatchedWorld: a large scene (3 (nb + npoly) + e > 128 or > 256 contacts) holds its "
+                                 "equality rows and the bodies they touch in the banded kernel's border of at most 16 "
+                                 "rows; here 3 x %d bodies + %d rows = %d" % (len(touched), self.ne, border))
         if self.large and (self.dtype != torch.float64 or self.ne > 16):
             raise ValueError("BatchedWorld: scenes with 3 (nb + npoly) + 3 n_static > 128 (or > 256 contacts) need "
                              "float64 and at most 5 pinned bodies (static obstacles do not count)")
@@ -247,12 +333,108 @@ class BatchedWorld:
         if self.strict_no_pen and bool((self.max_penetration() > self.tol).any()):
             raise AssertionError("Interpenetration at start")                      # world.py:66-68
 
+    # ------------------------------------------------------------------ constraints.py:13-173, world.py:156-170
+    def _init_constraints(self, to):
+        """Validates the constraint specs and sets up each Joint's state as Joint.__init__ does (constraints.py:16-27):
+        pos = anchor, pos1 = anchor - pos(body1), (r1, rot1) = cart_to_polar(pos1). Adds their rows to self.ne."""
+        nd, B = self.nd, self.B
+        self._jstate = []                         # per constraint: [r1, rot1, pos1, pos] (Joint) or None
+        for c in self.cons:
+            if not isinstance(c, (Joint, FixedJoint, _AxisConstraint)):
+                raise ValueError("constraints: expected Joint, FixedJoint, XConstraint, YConstraint or RotConstraint, "
+                                 "got %r" % (c,))
+            if isinstance(c, FixedJoint) and c.j is None:
+                raise ValueError("constraints: FixedJoint needs two bodies")
+            for k in (c.i,) + (() if c.j is None else (c.j,)):
+                if not isinstance(k, int) or k < 0 or k >= nd + self.no:
+                    raise ValueError("constraints: body index %r out of range (%d dynamic bodies)" % (k, nd))
+                if k >= nd:
+                    raise ValueError("constraints: body %d is an obstacle, which has no degrees of freedom (use "
+                                     "j=None for a joint to a world point)" % k)
+            if c.j is not None and c.i == c.j:
+                raise ValueError("constraints: a constraint joins body %d to itself" % c.i)
+            st = None
+            if isinstance(c, Joint):
+                a = to(c.anchor)
+                if a.dim() == 1:
+                    a = a.unsqueeze(0).expand(B, 2)
+                if a.shape != (B, 2):
+                    raise ValueError("constraints: Joint anchor must be [2] or [B, 2], got %s" % (tuple(a.shape),))
+                if not bool(torch.isfinite(a.detach()).all()):
+                    raise ValueError("constraints: non-finite Joint anchor")
+                pos1 = a - self.p[:, c.i, 1:]
+                r1, rot1 = _cart_to_polar(pos1)
+                st = [r1, rot1, pos1, a]
+            self._jstate.append(st)
+            self.ne += c.num_constraints
+        if self.cons:
+            self.A = self._equality_rows()
+
+    def _equality_rows(self):
+        """World.Je() (world.py:156-170) for every scene, [B, ne, n]: the `static` pins' identity rows, then each
+        constraint's J() (constraints.py:29-36, :70-77, :106-108, :133-135, :160-162) at the current state, as
+        differentiable torch ops."""
+        B, n = self.B, self.n
+        A = self.p.new_zeros(B, self.ne, n)
+        for r, k in enumerate(self.static):
+            for q in range(3):
+                A[:, 3 * r + q, 3 * k + q] = 1.0
+        r = 3 * len(self.static)
+        for c, st in zip(self.cons, self._jstate):
+            i, j = 3 * c.i, None if c.j is None else 3 * c.j
+            if isinstance(c, _AxisConstraint):
+                A[:, r, i + c.dof] = 1.0
+            elif isinstance(c, Joint):
+                pos1, pos = st[2], st[3]
+                A[:, r, i], A[:, r, i + 1] = -pos1[:, 1], 1.0
+                A[:, r + 1, i], A[:, r + 1, i + 2] = pos1[:, 0], 1.0
+                if j is not None:
+                    pos2 = pos - self.p[:, c.j, 1:]                       # update_pos: pos2 = pos - body2.pos
+                    A[:, r, j], A[:, r, j + 1] = pos2[:, 1], -1.0
+                    A[:, r + 1, j], A[:, r + 1, j + 2] = -pos2[:, 0], -1.0
+            else:                                                          # FixedJoint: pos1 = 0, pos = body1.pos
+                pos2 = self.p[:, c.i, 1:] - self.p[:, c.j, 1:]
+                A[:, r, i + 1], A[:, r + 1, i + 2], A[:, r + 2, i] = 1.0, 1.0, 1.0
+                A[:, r, j], A[:, r, j + 1] = pos2[:, 1], -1.0
+                A[:, r + 1, j], A[:, r + 1, j + 2] = -pos2[:, 0], -1.0
+                A[:, r + 2, j] = -1.0
+            r += c.num_constraints
+        return A
+
+    def _move_joints(self, rot_start, vel, dts):
+        """Joint.move(dt) after the bodies moved (constraints.py:38-49): rot1 = rot_start + v_rot(body1) dt,
+        pos1 = polar_to_cart(r1, rot1), pos = pos(body1) + pos1. FixedJoint and the axis constraints keep no state."""
+        for c, st, r0 in zip(self.cons, self._jstate, rot_start):
+            if st is None:
+                continue
+            rot1 = r0 + vel[:, 3 * c.i] * dts
+            pos1 = _polar_to_cart(st[0], rot1)
+            st[1:] = [rot1, pos1, self.p[:, c.i, 1:] + pos1]
+
+    def _init_no_contact(self, pairs, nt):
+        """Pair-exclusion bitmask of lcpb200_body_contacts_masked: bit i * nt + j (i < j) per excluded pair."""
+        words = [0] * ((nt * nt + 31) // 32)
+        ex = torch.zeros(nt, nt, dtype=torch.bool)
+        for pr in pairs:
+            a, b = (int(x) for x in pr)
+            if not (0 <= a < nt and 0 <= b < nt):
+                raise ValueError("no_contact: body index out of range in %r (%d bodies)" % (tuple(pr), nt))
+            if a == b:
+                raise ValueError("no_contact: the pair (%d, %d) names one body twice" % (a, b))
+            a, b = min(a, b), max(a, b)
+            bit = a * nt + b
+            words[bit >> 5] |= 1 << (bit & 31)
+            ex[a, b] = True
+        words = [w - (1 << 32) if w >= 1 << 31 else w for w in words]            # the same 32 bits as int32
+        self.nc_mask = torch.tensor(words, dtype=torch.int32, device=self.device)
+        self.nc_pair_excluded = ex.to(self.device)[self.pi, self.pj]              # per pair of self.pi / self.pj
+
     # ------------------------------------------------------------------ contacts.py:68-80, batched
     def find_contacts(self):
         """Pair test + ordered compaction on the GPU (lcpb200_find_contacts: all nb (nb - 1) / 2 pairs of every
         scene, lexicographic order = the reference's contact order), then the contact geometry of the selected
         pairs with torch ops (differentiable w.r.t. the positions)."""
-        if self.np:
+        if self.np or self.nc_mask is not None:
             return self._find_contacts_bodies()
         if self.no:
             return self._find_contacts_obstacles()
@@ -350,8 +532,9 @@ class BatchedWorld:
         that rebuild it from those features (_geometry_torch) when something needs autograd."""
         lib = _lib.load()
         B, cap, dev, nb = self.B, self.cap, self.device, self.nb
-        pverts = self.polygon_vertices()
-        pcen = self.p[:, nb:, 1:]
+        pverts = self.polygon_vertices() if self.np else None
+        pcen = self.p[:, nb:, 1:] if self.np else None
+        poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
         b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
         b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
         feat = torch.empty(B, cap, dtype=torch.int32, device=dev)
@@ -359,19 +542,23 @@ class BatchedWorld:
         obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
         needs_graph = torch.is_grad_enabled() and any(
             t is not None and t.requires_grad
-            for t in (self.p, self.rad, self.fric_coeff, self.restitution, self.plocal, self.pfric, self.prest) + obst)
+            for t in (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
         d = lambda t: t.detach().contiguous() if t is not None else None
         geo = [None] * 6
         if not needs_graph:
             new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
             geo = [new(2), new(2), new(2), new(), new(), new()]
         # contiguous copies held until the call returns (a temporary's memory could be reused before the kernel runs)
-        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen, self.pfric,
-                              self.prest) + obst]
+        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
+               + obst]
+        # worlds with no_contact pairs: the same walk reading the pair-exclusion mask (every world kind)
+        masked = self.nc_mask is not None
+        fn = lib.lcpb200_body_contacts_masked if masked else lib.lcpb200_body_contacts
         with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_body_contacts(
+            _lib.check(fn(
                 _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps, *[_lib.ptr(t) for t in ins],
                 _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat), *[_lib.ptr(t) for t in geo],
+                *((_lib.ptr(self.nc_mask),) if masked else ()),
                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         if int(counts.max()) > cap:
             raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
@@ -480,8 +667,10 @@ class BatchedWorld:
             if nb == 0:
                 return n_h, p1_h, p2_h, pen_h, mu_h, rest_h
             i1 = torch.where(hh, 0, i1)
-        else:
+        elif self.no:
             polys, pref, pfr, prs = self.ov, self.oref, self.ofric, self.orest
+        else:                                        # circles only (worlds with no_contact pairs)
+            polys = None
         cc = i2 < nb
         j = torch.where(cc, i2, 0)
         k = torch.where(cc, 0, i2 - nb)
@@ -497,6 +686,9 @@ class BatchedWorld:
         n_cc = dcc / dist.unsqueeze(2)
         p1_cc = -n_cc * (r1 - pen_cc / 2).unsqueeze(2)
         p2_cc = n_cc * (r2 - pen_cc / 2).unsqueeze(2)
+        if polys is None:
+            return (n_cc, p1_cc, p2_cc, pen_cc, 0.5 * (take(self.fric_coeff, i1) + take(self.fric_coeff, j)),
+                    0.5 * (take(self.restitution, i1) + take(self.restitution, j)))
         # circle-obstacle / circle-polygon
         inside, q, _, n_in, sep = self._circle_polygon_torch(c, k, polys)
         out = ~cc & ~inside
@@ -540,12 +732,16 @@ class BatchedWorld:
             inside, _, d2, _, _ = self._circle_polygon_torch(pos[:, self.pi], k)
             hit_o = inside | ~(d2.sqrt() - self.rad[:, self.pi] > self.eps)              # contacts.py:110-112
             active = torch.where(cc, pen >= -self.eps, hit_o)
+            if self.nc_mask is not None:
+                active = active & ~self.nc_pair_excluded                                  # contacts.py:60
             counts = active.sum(1)
             order = torch.sort((~active).to(torch.int8), dim=1, stable=True)[1][:, :self.cap]
             return counts.to(torch.int32), self.pi[order].to(torch.int32), self.pj[order].to(torch.int32)
         d = pos[:, self.pi] - pos[:, self.pj]
         pen = self.rad[:, self.pi] + self.rad[:, self.pj] - d.norm(dim=2)
         active = pen >= -self.eps                                                  # `if penetration < -eps: return`
+        if self.nc_mask is not None:
+            active = active & ~self.nc_pair_excluded                                      # contacts.py:60
         counts = active.sum(1)
         order = torch.sort((~active).to(torch.int8), dim=1, stable=True)[1][:, :self.cap]   # active pairs first, in pair order
         return counts.to(torch.int32), self.pi[order].to(torch.int32), self.pj[order].to(torch.int32)
@@ -554,9 +750,10 @@ class BatchedWorld:
         return self.c_pen.max(dim=1)[0]
 
     # ------------------------------------------------------------------ engine calls
-    def _lcp(self, mode, dt, b):
-        z, status = engine_solve(self.mass, self.inertia, self.v, self.fext, self.c_normal, self.c_p1, self.c_p2,
-                                 self.c_mu, self.c_rest, self.c_b1, self.c_b2, dt, A=self.A, b=b, mode=mode,
+    def _lcp(self, mode, dt, b, fext=None):
+        z, status = engine_solve(self.mass, self.inertia, self.v, self.fext if fext is None else fext, self.c_normal,
+                                 self.c_p1, self.c_p2, self.c_mu, self.c_rest, self.c_b1, self.c_b2, dt, A=self.A, b=b,
+                                 mode=mode,
                                  max_iter=self.max_iter if mode == 0 else 10, exact_adjoint=self.exact_adjoint,
                                  counts=self.counts)
         if bool((status == _lib.STATUS_SINGULAR_Q).any()):
@@ -567,12 +764,24 @@ class BatchedWorld:
         return z
 
     def solve_dynamics(self, dt):
-        """engines.py:26-78 for every scene: new_v = -zhat."""
+        """engines.py:26-78 for every scene: new_v = -zhat. The constraints' rows are rebuilt at the current state and
+        the external force is evaluated at the step's start time (apply_forces(world.t), engines.py:27-32)."""
+        if self.cons:
+            self.A = self._equality_rows()
         b = self.v.new_zeros(self.B, self.ne) if self.ne else None
-        return -self._lcp(0, dt, b)
+        fext = None
+        if self.external_force is not None:
+            f = self.external_force(self.t)
+            if tuple(f.shape) != (self.B, self.nd, 3):
+                raise ValueError("external_force: f(t) must return [B, nd, 3] = %s, got %s"
+                                 % ((self.B, self.nd, 3), tuple(f.shape)))
+            fext = self.fext + f.reshape(self.B, self.n)
+        return -self._lcp(0, dt, b, fext)
 
     def post_stabilization(self):
-        """engines.py:80-116 for every scene: -zhat with b = Je v."""
+        """engines.py:80-116 for every scene: -zhat with b = Je v, the constraints' rows at the current pose."""
+        if self.cons:
+            self.A = self._equality_rows()
         b = torch.bmm(self.A, self.v.unsqueeze(2)).squeeze(2) if self.ne else None
         return -self._lcp(1, 0.0, b)
 
@@ -582,6 +791,7 @@ class BatchedWorld:
 
     def step_dt(self, dt):
         start_p = self.p.clone()
+        start_rot = [st[1] if st is not None else None for st in self._jstate]      # world.py:85
         self.v = self.solve_dynamics(dt)
         dts = self.v.new_full((self.B,), float(dt))
         done = torch.zeros(self.B, dtype=torch.bool, device=self.device)
@@ -596,10 +806,15 @@ class BatchedWorld:
             if bool(done.all()):
                 break
             dts = torch.where(done, dts, dts / 2)                                  # world.py:101 (positions reset: start_p)
+        if self.cons:
+            # joints moved with the bodies by the step's final dt, from the start value (world.py:92-93, :104-107)
+            self._move_joints(start_rot, self.v, dts)
         if self.post_stab:
             tmp_v = self.v
             dp = self.post_stabilization() / 2                                     # world.py:111-112
             self.p = self.p + dp.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)
+            if self.cons:
+                self._move_joints([st[1] if st is not None else None for st in self._jstate], dp, dts)   # :117-118
             self.v = tmp_v
             self.find_contacts()
         self.t = self.t + dts
