@@ -289,8 +289,10 @@ int lcpb200_assemble_backward(int dtype, int B, int nb, int nc, double dt,
  * e.g. World.Je()); nothing dense is written to or read from HBM. The handle must have been created with
  * n = 3 nb, m = 4 nc (mode 0) or nc (mode 1). n + e <= 128: the condensed-KKT kernels (fp32 / fp64); larger
  * scenes (fp64 only, e.g. BASELINE config 4: 512 bodies): the banded large-scene kernels (lcp_banded.cuh), which
- * order the bodies so that the condensed matrix is an arrow matrix (half bandwidth <= 128 after the ordering, <= 16
- * border rows: pinned bodies, bodies with > 12 contacts, equality rows). A scene whose contact topology the kernel
+ * order the bodies so that the condensed matrix is an arrow matrix (<= 16 border rows: pinned bodies, bodies with
+ * > 12 two-body contacts, equality rows) whose half bandwidth bw, rounded up to a multiple of 8, is at most the
+ * plan's limit. That limit comes from shared memory: on an H100 it is 128 rows up to 773 bodies, 120 up to 1492,
+ * 112 up to 2173 and 104 beyond (a half bandwidth of 42, 39, 36, 34 bodies). A scene whose contact topology the kernel
  * cannot take (a contact of a body with itself, > 16 contacts on one body for the condensed kernels, a band or
  * border beyond the limits above) gets status -100 and no result: assemble it with lcpb200_assemble and call
  * lcpb200_forward.

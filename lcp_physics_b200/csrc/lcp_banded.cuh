@@ -153,7 +153,7 @@ struct Ctx {
   const int32_t *b1, *b2;
   const double* A;
   int nb, n, e, cs, ncap, nc, m;
-  int nband, Nb, Nbp, nbb, nbd, bw, bwa, Wc, LDW, LP, fbs, npass, ldk, win_doubles;
+  int nband, Nb, Nbp, nbb, nbd, bw, bwa, Wc, LDW, LP, fbs, npass, ldk, win_doubles, bwa_max;
   int o_win, o_sol, o_lp, o_up, o_cf;      // byte offsets of the shared-memory arrays (see smem_d)
 };
 
@@ -420,6 +420,10 @@ __device__ __noinline__ int build_structure(Ctx& c, const cnd::EngineSoA<double>
   c.fbs = 72 + 2 * PV * c.LP;
   c.npass = c.Nbp / PV;
   c.ldk = c.bw + 1;
+  // The plan sized the band rows (Kb / KbT: ldk <= bwa_max + 1), the panels, the factor blocks and the
+  // substitution's rows (32 SUBR) for bwa <= bwa_max. The window check alone is not enough: the leftover shared
+  // memory of a plan can hold the window of the next width up while the L2 workspace cannot hold its band.
+  if (c.bwa > c.bwa_max) return 1;
   if ((long long)c.LDW * c.LDW > c.win_doubles) return 1;                    // band too wide for the window
   return 0;
 }
@@ -1375,6 +1379,7 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const BPlan& P, double* wsd, in
   c.up = reinterpret_cast<double*>(bnd_smem + P.o_up);
   c.win = reinterpret_cast<double*>(bnd_smem + P.o_win);
   c.win_doubles = P.win_bytes / 8;
+  c.bwa_max = P.bwa_max;
   c.o_win = P.o_win; c.o_sol = P.o_sol; c.o_lp = P.o_lp; c.o_up = P.o_up; c.o_cf = P.o_cf;
   double* g = wsd + (size_t)blockIdx.x * P.g_doubles;
   c.qd = g + P.g_qd; c.ps = g + P.g_ps; c.x = g + P.g_x; c.dx = g + P.g_dx; c.rx = g + P.g_rx;

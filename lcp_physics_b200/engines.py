@@ -123,7 +123,7 @@ class _EngineSolveFn(torch.autograd.Function):
                 *[_lib.ptr(t) for t in (zhat, nu, lam, slack, status, iters, resid)], _stream_ptr(dev)))
         ctx.save_for_backward(*ins, mu_c, rest_c, A_c, body1, body2, zhat, nu, lam, slack, counts)
         ctx.meta = (float(dt), int(mode), bool(exact), B, nb, nc, e)
-        _last_info.update(iters=iters, resid=resid, status=status, lam=lam, slack=slack)
+        _last_info.update(iters=iters, resid=resid, status=status, lam=lam, slack=slack, nu=nu)
         ctx.mark_non_differentiable(status)
         return zhat, status
 
@@ -153,7 +153,8 @@ _last_info = {}
 
 def last_solve_info():
     """Diagnostics of the most recent engine_solve call (device tensors): PDIPM iteration counts, best residuals,
-    status, multipliers and slacks per scene (the reference prints them with verbose >= 1, pdipm.py:97-105)."""
+    status, multipliers, slacks and equality multipliers (nu, None without equality rows) per scene (the reference
+    prints them with verbose >= 1, pdipm.py:97-105)."""
     return _last_info
 
 
