@@ -626,15 +626,25 @@ __device__ __forceinline__ void comp_inverse(const CPlan& P, CSmem<T>& S, const 
   }
 }
 
+// Positions per thread comp_apply needs for rows of CS slots: the grid it covers is t < CS << sh, sh = ceil(log2(ncomp)).
+// build_structure admits ncomp * CS <= pcap <= 4 NT (pcap is m rounded up to 8, m <= 4 NT), so ncomp <= 4 NT / CS:
+// 4 for CS = 1, 2, 4; 5 for CS = 5 (ncomp <= 204: 5 << 8 = 1280); 6 for CS = 3 (ncomp <= 341: 3 << 9) and 6 (ncomp <= 170).
+template <int CS>
+struct ApplySpan {
+  static constexpr int ceil_log2(int x) { return x <= 1 ? 0 : 1 + ceil_log2((x + 1) / 2); }
+  static constexpr int U = ((CS << ceil_log2(4 * NT / CS)) + NT - 1) / NT;
+};
+
 // out_c = W_c * in_c for every component, in place in S.scr (one thread per (component, row))
 template <typename T, int CS>
 __device__ __forceinline__ void comp_apply(CSmem<T>& S, const Struct& st, bool trans = false) {
+  constexpr int U = ApplySpan<CS>::U;
   const int nc_ = st.ncomp;                       // positions are slot-major: pos(c, r) = r * ncomp + c
   const int npos = nc_ * CS;
   const int sh = st.sh, cmask = (1 << sh) - 1, tot = CS << sh;
-  double val[4];
+  double val[U];
 #pragma unroll
-  for (int u = 0; u < 4; ++u) {
+  for (int u = 0; u < U; ++u) {
     const int t = threadIdx.x + u * NT, r = t >> sh, c = t & cmask;
     val[u] = 0.0;
     if (t < tot && c < nc_) {
@@ -646,7 +656,7 @@ __device__ __forceinline__ void comp_apply(CSmem<T>& S, const Struct& st, bool t
   }
   __syncthreads();
 #pragma unroll
-  for (int u = 0; u < 4; ++u) {
+  for (int u = 0; u < U; ++u) {
     const int t = threadIdx.x + u * NT, r = t >> sh, c = t & cmask;
     if (t < tot && c < nc_) S.scr()[r * nc_ + c] = val[u];
   }
@@ -1368,7 +1378,8 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_forward_kernel(con
         for (int i = tid; i < e; i += NT) a.nu[(size_t)sc * e + i] = NANV;
         if (tid == 0) { a.status[sc] = -1; a.iters[sc] = 0; if (a.resid) a.resid[sc] = NANV; }
       } else if (tid == 0) {
-        a.status[sc] = STATUS_UNSUPPORTED;
+        a.status[sc] = STATUS_UNSUPPORTED;     // the dual form (dense API) overwrites both; the engine path returns them
+        a.iters[sc] = 0;
       }
       __syncthreads();
       continue;

@@ -1,9 +1,36 @@
-"""Shared test helpers: golden fixture loading and error metrics."""
+"""Shared test helpers: golden fixture loading, error metrics, the fp32 accuracy gate and the dual-form switch."""
+import contextlib
 import glob
 import os
 
 import numpy as np
 import torch
+
+
+@contextlib.contextmanager
+def dual_only():
+    """Plan new handles without the condensed-KKT kernels (the dense / dual-form path)."""
+    from lcp_physics_b200 import _lib
+    os.environ["LCPB200_NO_CONDENSED"] = "1"
+    _lib.clear_handles()
+    try:
+        yield
+    finally:
+        del os.environ["LCPB200_NO_CONDENSED"]
+        _lib.clear_handles()
+
+
+def fp32_gate(zhat, ref32, ref64, what):
+    """Distributional fp32 accuracy gate (tests/test_gpu_parity.py's module docstring): zhat against the fp32 and
+    the fp64 reference of the same scenes."""
+    err = rel_err(zhat, ref32)
+    own = rel_err(ref32, ref64)
+    mine = rel_err(zhat, ref64)
+    assert float((err <= 1e-3 + 1.5 * own).float().mean()) >= 0.95, (what, err, own)
+    assert float((err < 1e-3).float().mean()) >= 0.85, (what, err)
+    assert float(err.max()) <= 2e-2, (what, err)
+    assert float(mine.median()) <= 1.2 * float(own.median()) + 1e-6, (what, mine.median(), own.median())
+    assert float(mine.quantile(0.9)) <= 1.2 * float(own.quantile(0.9)) + 1e-4, (what, mine.quantile(0.9), own.quantile(0.9))
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 

@@ -82,12 +82,13 @@ def _gz(B, n, dtype, seed=3):
     return torch.randn(B, n, generator=torch.Generator().manual_seed(seed), dtype=torch.float64).to(dtype)
 
 
+@pytest.mark.parametrize("nb,nc", [(NB, NC), (20, 40), (40, 80)])       # NS = 6, 4 and 8 blocks of K
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
-def test_band_lu_dense_api_bitwise(dtype):
+def test_band_lu_dense_api_bitwise(dtype, nb, nc):
     from lcp_physics_b200.scenes import make_scenes
-    B = 96
-    inp = make_scenes(B, NB, NC, fd=2, e=0, dtype=dtype, seed=11)
-    g = _gz(B, 3 * NB, dtype)
+    B = 96 if nb == NB else 32
+    inp = make_scenes(B, nb, nc, fd=2, e=0, dtype=dtype, seed=11)
+    g = _gz(B, 3 * nb, dtype)
     got, ref = both(lambda: dense_solve(inp, g))
     assert (got[4] >= 0).all()
     assert_same(got, ref, str(dtype))
@@ -138,18 +139,19 @@ def test_equality_rows_take_the_dense_lu(dtype):
     assert_same(got, ref, str(dtype))
 
 
+@pytest.mark.parametrize("nb,nc", [(NB, NC), (20, 40), (40, 80)])       # NS = 6, 4 and 8 blocks of K
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
 @pytest.mark.parametrize("mode", [0, 1])
-def test_band_lu_engine_path_bitwise(mode, dtype):
+def test_band_lu_engine_path_bitwise(mode, dtype, nb, nc):
     from lcp_physics_b200.engines import engine_solve
     from lcp_physics_b200.scenes import make_contact_soa
-    B = 64
-    soa = dict(make_contact_soa(B, NB, NC, seed=14))
-    fext = torch.zeros(B, 3 * NB, dtype=torch.float64)
+    B = 64 if nb == NB else 24
+    soa = dict(make_contact_soa(B, nb, nc, seed=14))
+    fext = torch.zeros(B, 3 * nb, dtype=torch.float64)
     fext[:, 2::3] = 10.0 * soa["mass"]
     soa["fext"] = fext
     b1, b2 = soa["body1"].cuda(), soa["body2"].cuda()
-    gz = _gz(B, 3 * NB, dtype).cuda()
+    gz = _gz(B, 3 * nb, dtype).cuda()
 
     def run():
         res = []

@@ -25,12 +25,12 @@ the gates are, on 48 scenes per shape against outputs of the unmodified referenc
 (The kernel's median error against fp64 is in fact 100x smaller than the reference's.)
 """
 import contextlib
-import os
 
 import pytest
 import torch
 
-from tests.helpers import golden_names, load_golden, load_seeded_golden, rel_err, seeded_names
+from tests.helpers import dual_only, fp32_gate as _fp32_gate, golden_names, load_golden, load_seeded_golden, rel_err, \
+    seeded_names
 
 pytestmark = pytest.mark.gpu
 
@@ -39,19 +39,6 @@ GRADS = "dQ dp dG dh dA db dF".split()
 
 def _cuda(ts):
     return tuple(t.cuda() if t is not None else None for t in ts)
-
-
-@contextlib.contextmanager
-def dual_only():
-    """Plan new handles without the condensed-KKT kernels (the dense / dual-form path)."""
-    from lcp_physics_b200 import _lib
-    os.environ["LCPB200_NO_CONDENSED"] = "1"
-    _lib.clear_handles()
-    try:
-        yield
-    finally:
-        del os.environ["LCPB200_NO_CONDENSED"]
-        _lib.clear_handles()
 
 
 PATHS = ["default", "dual"]
@@ -115,17 +102,6 @@ def test_backward_matches_reference_golden_fp64(name):
 
 
 # ------------------------------------------------------------------ reference goldens, fp32
-def _fp32_gate(zhat, ref32, ref64, what):
-    err = rel_err(zhat, ref32)
-    own = rel_err(ref32, ref64)
-    mine = rel_err(zhat, ref64)
-    assert float((err <= 1e-3 + 1.5 * own).float().mean()) >= 0.95, (what, err, own)
-    assert float((err < 1e-3).float().mean()) >= 0.85, (what, err)
-    assert float(err.max()) <= 2e-2, (what, err)
-    assert float(mine.median()) <= 1.2 * float(own.median()) + 1e-6, (what, mine.median(), own.median())
-    assert float(mine.quantile(0.9)) <= 1.2 * float(own.quantile(0.9)) + 1e-4, (what, mine.quantile(0.9), own.quantile(0.9))
-
-
 @pytest.mark.parametrize("path", PATHS)
 @pytest.mark.parametrize("name", golden_names())
 def test_forward_fp32_golden(name, path):
