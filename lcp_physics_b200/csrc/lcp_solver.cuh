@@ -429,7 +429,9 @@ __device__ __noinline__ bool prefactor(SceneCtx<T, MODE>& c, int* flag) {
   if (singular) return false;
   constexpr int VC_ = VecOf<T>::VC;
   if (c.Rsaved) {
-    // R was saved by the forward pass (backward only): nothing to form
+    // R was saved by the forward pass (backward only): nothing to form. The G copies are still the ones the
+    // staged branch below builds, so that the gradients do not depend on whether R was saved.
+    if (!offdiag && n % VC_ == 0 && MODE != 2 && c.stage_ld > 0) build_g_ell(c, c.Gsrc, n);
   } else if (!offdiag && n % VC_ == 0) {
     // R = G diag(1/q) G^T + F with G staged in the (still unused) shared-memory region of T
     T* qd = v.scratch;                                           // n <= scratch
