@@ -328,6 +328,25 @@ int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode,
                             void* dmass, void* dinertia, void* dv, void* dfext,
                             void* dnormal, void* dp1, void* dp2, void* dmu, void* drestitution,
                             void* dA, void* db, unsigned flags, void* stream);
+/* lcpb200_engine_backward_batched: R >= 1 cotangents of the same saved solves in one call -- the rows of a
+ * vector-Jacobian product, e.g. R = n one-hot cotangents for the whole Jacobian of zhat. Same inputs as
+ * lcpb200_engine_backward (one set for the batch: mass[B,nb], ..., zhat[B,n], lam / slack[B,m], nu[B,e]), but
+ * dl_dzhat is [R,B,n] and every output is [R,B,...] (dmass[R,B,nb], dv[R,B,n], dnormal[R,B,nc,2], dA[R,B,e,n],
+ * ...): slot r holds exactly what lcpb200_engine_backward returns for the cotangent dl_dzhat[r]. Each scene's
+ * KKT matrix is factored once per chunk of cotangents, not once per cotangent; the cotangents of a scene are split
+ * into chunks only to fill the GPU when B is small, and the results do not depend on that split. The same NULL
+ * rules and flags as lcpb200_engine_backward; a scene with status -100 gets zero gradients in every slot.
+ * lcpb200_engine_backward is this call with R = 1. */
+int lcpb200_engine_backward_batched(lcpb200_handle_t h, int R, int B, int nb, int nc, int mode, double dt,
+                                    const void* mass, const void* inertia, const void* v, const void* fext,
+                                    const void* normal, const void* p1, const void* p2,
+                                    const int32_t* body1, const int32_t* body2, const int32_t* contact_count,
+                                    const void* mu, const void* restitution, const void* A,
+                                    const void* zhat, const void* nu, const void* lam, const void* slack,
+                                    const void* dl_dzhat,
+                                    void* dmass, void* dinertia, void* dv, void* dfext,
+                                    void* dnormal, void* dp1, void* dp2, void* dmu, void* drestitution,
+                                    void* dA, void* db, unsigned flags, void* stream);
 
 #ifdef __cplusplus
 }

@@ -121,6 +121,7 @@ struct BArgs {
 struct BBwdArgs {
   BPlan P;
   int B;
+  int R, chunks;                  // R cotangents, [R][B][...] slots, (scene, chunk) work items: as cnd::CBwdArgs
   cnd::EngineSoA<double> soa;
   const double* A;
   const double *zhat, *nu, *lam, *slack, *g;
@@ -1423,38 +1424,25 @@ __global__ void __launch_bounds__(NT, 1) band_forward_kernel(const __grid_consta
 // (world.py:144-234, engines.py:50-116) applied to the factored gradients of lcp.py:52-63 -- evaluated only at
 // the entries the assembly writes (same formulas as lcp_condensed.cuh's engine path). flags bit 0 (exact adjoint)
 // factors and solves the transposed system K^T instead (DESIGN.md section 3.4); the chain rule is the same.
-__device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf& pf, int sc) {
-  const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, cs = c.cs, ncap = c.ncap, nb = c.nb;
+//
+// The gradients of one cotangent from the solve's dx, dlam, dnu in c: inputs of scene sc, outputs at row so.
+__device__ __forceinline__ void backward_grads(const BBwdArgs& a, Ctx& c, BProf& pf, int sc, int so) {
+  const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, ncap = c.ncap, nb = c.nb;
   const cnd::EngineSoA<double>& E = a.soa;
   const int ncs = E.nc, mode = E.mode;
-  const double* mu = E.mu ? E.mu + (size_t)sc * ncs : nullptr;
   const double* zh = a.zhat + (size_t)sc * n;
-  const double* lamv = a.lam + (size_t)sc * a.P.m;
-  const double* slk = a.slack + (size_t)sc * a.P.m;
-  for (int i = tid; i < n; i += NT) { c.x[i] = zh[i]; c.rx[i] = a.g[(size_t)sc * n + i]; }
-  for (int r = 0; r < cs; ++r)
-    for (int k = tid; k < nc; k += NT) {
-      const int i = r * ncap + k, o = out_row(r, k, nc);
-      double d = lamv[o] / slk[o];                                          // :44
-      d = d > 1e10 ? 1e10 : (d < 1e-10 ? 1e-10 : d);
-      c.z[i] = lamv[o]; c.s[i] = slk[o]; c.d[i] = d; c.rs[i] = 0.0;
-    }
-  for (int i = tid; i < e; i += NT) c.y[i] = a.nu[(size_t)sc * e + i];
-  __syncthreads();
-  factor_kkt(c, pf, mode, mu, (a.flags & 1u) != 0);                         // :46
-  solve_kkt(c, pf, c.rx, c.rs, nullptr, nullptr, c.dx, c.ds, c.dz, c.dy);   // :47-50 (c.W holds W^T when exact)
   const double* dx = c.dx;
   const double* dlam = c.dz;
   const double* lm = c.z;
   const double* v = E.v + (size_t)sc * n;
   for (int k = tid; k < ncs; k += NT) {
-    const size_t ic = (size_t)sc * ncs + k;
+    const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
     if (k >= nc) {                                                          // unused slots of a scene with fewer contacts
-      if (a.dnormal) { a.dnormal[ic * 2] = 0; a.dnormal[ic * 2 + 1] = 0; }
-      if (a.dp1) { a.dp1[ic * 2] = 0; a.dp1[ic * 2 + 1] = 0; }
-      if (a.dp2) { a.dp2[ic * 2] = 0; a.dp2[ic * 2 + 1] = 0; }
-      if (a.drest) a.drest[ic] = 0;
-      if (a.dmu) a.dmu[ic] = 0;
+      if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
+      if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
+      if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
+      if (a.drest) a.drest[oc] = 0;
+      if (a.dmu) a.dmu[oc] = 0;
       continue;
     }
     const double nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
@@ -1490,11 +1478,11 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
       else if (q == 1) { gny += gdx; gnx += -gdy; }                         // dir1 = (ny, -nx)
       else { gny += -gdx; gnx += gdy; }                                     // dir2 = (-ny, nx)
     }
-    if (a.dnormal) { a.dnormal[ic * 2] = gnx; a.dnormal[ic * 2 + 1] = gny; }
-    if (a.dp1) { a.dp1[ic * 2] = g1x; a.dp1[ic * 2 + 1] = g1y; }
-    if (a.dp2) { a.dp2[ic * 2] = g2x; a.dp2[ic * 2 + 1] = g2y; }
-    if (a.drest) a.drest[ic] = mode == 0 ? dhc * jcv : -dhc * jcv;
-    if (a.dmu) a.dmu[ic] = mode == 0 ? -(dlam[3 * ncap + k] * lm[k]) : 0.0;   // dF[gamma_c][c]  (:54)
+    if (a.dnormal) { a.dnormal[oc * 2] = gnx; a.dnormal[oc * 2 + 1] = gny; }
+    if (a.dp1) { a.dp1[oc * 2] = g1x; a.dp1[oc * 2 + 1] = g1y; }
+    if (a.dp2) { a.dp2[oc * 2] = g2x; a.dp2[oc * 2 + 1] = g2y; }
+    if (a.drest) a.drest[oc] = mode == 0 ? dhc * jcv : -dhc * jcv;
+    if (a.dmu) a.dmu[oc] = mode == 0 ? -(dlam[3 * ncap + k] * lm[k]) : 0.0;   // dF[gamma_c][c]  (:54)
   }
   for (int body = tid; body < nb; body += NT) {
     double dm = 0.0;
@@ -1504,7 +1492,7 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
       const int j = 3 * body + comp;
       const double md = comp == 0 ? E.inertia[(size_t)sc * nb + body] : E.mass[(size_t)sc * nb + body];
       const double dpj = mode == 0 ? dx[j] : 0.0;                           // dp = dx (:52); post-stabilisation has p = 0
-      if (a.dfext) a.dfext[(size_t)sc * n + j] = E.dt * dpj;
+      if (a.dfext) a.dfext[(size_t)so * n + j] = E.dt * dpj;
       if (a.dv) {
         double acc = md * dpj;
         for (int it = s0; it < s1; ++it) {                                  // the contacts that touch this body
@@ -1512,22 +1500,52 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
           const double hs_ = mode == 0 ? E.rest[(size_t)sc * ncs + k] : (1.0 - E.rest[(size_t)sc * ncs + k]);
           acc += -dlam[k] * hs_ * c.cg[12 * (size_t)k + 3 * side + comp];  // dh_c d(h_c)/dv_j
         }
-        a.dv[(size_t)sc * n + j] = acc;
+        a.dv[(size_t)so * n + j] = acc;
       }
       const double dq = dx[j] * zh[j] + dpj * v[j];                         // dQ_jj = 1/2 (dx_j z_j + z_j dx_j)  (:61), dp_j d(p_j)/dM_jj
-      if (comp == 0) { if (a.dinertia) a.dinertia[(size_t)sc * nb + body] = dq; }
+      if (comp == 0) { if (a.dinertia) a.dinertia[(size_t)so * nb + body] = dq; }
       else dm += dq;
     }
-    if (a.dmass) a.dmass[(size_t)sc * nb + body] = dm;
+    if (a.dmass) a.dmass[(size_t)so * nb + body] = dm;
   }
-  if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)sc * e + i] = -c.dy[i];
+  if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)so * e + i] = -c.dy[i];
   if (a.dA && e > 0) {
-    double* o = a.dA + (size_t)sc * e * n;
+    double* o = a.dA + (size_t)so * e * n;
     for (int i = 0; i < e; ++i)
       for (int j = tid; j < n; j += NT) o[(size_t)i * n + j] = c.dy[i] * zh[j] + c.y[i] * dx[j];
   }
   __syncthreads();
   pf.lap(BPH_GRADS);
+}
+
+// One factorisation at the saved solution, then one solve and chain rule per cotangent r in [r0, r1); each
+// round streams the factor blocks back from the L2 workspace.
+__device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf& pf, int sc, int r0, int r1) {
+  const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, cs = c.cs, ncap = c.ncap;
+  const cnd::EngineSoA<double>& E = a.soa;
+  const int ncs = E.nc, mode = E.mode;
+  const double* mu = E.mu ? E.mu + (size_t)sc * ncs : nullptr;
+  const double* zh = a.zhat + (size_t)sc * n;
+  const double* lamv = a.lam + (size_t)sc * a.P.m;
+  const double* slk = a.slack + (size_t)sc * a.P.m;
+  for (int i = tid; i < n; i += NT) c.x[i] = zh[i];
+  for (int r = 0; r < cs; ++r)
+    for (int k = tid; k < nc; k += NT) {
+      const int i = r * ncap + k, o = out_row(r, k, nc);
+      double d = lamv[o] / slk[o];                                          // :44
+      d = d > 1e10 ? 1e10 : (d < 1e-10 ? 1e-10 : d);
+      c.z[i] = lamv[o]; c.s[i] = slk[o]; c.d[i] = d; c.rs[i] = 0.0;
+    }
+  for (int i = tid; i < e; i += NT) c.y[i] = a.nu[(size_t)sc * e + i];
+  __syncthreads();
+  factor_kkt(c, pf, mode, mu, (a.flags & 1u) != 0);                         // :46
+  for (int r = r0; r < r1; ++r) {
+    const int so = r * a.B + sc;
+    for (int i = tid; i < n; i += NT) c.rx[i] = a.g[(size_t)so * n + i];
+    __syncthreads();
+    solve_kkt(c, pf, c.rx, c.rs, nullptr, nullptr, c.dx, c.ds, c.dz, c.dy);   // :47-50 (c.W holds W^T when exact)
+    backward_grads(a, c, pf, sc, so);
+  }
 }
 
 __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_constant__ BBwdArgs a) {
@@ -1536,7 +1554,9 @@ __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_const
   init_ctx(c, P, a.wsd, a.wsi);
   BProf pf;
   pf.start(a.prof ? a.prof + (size_t)blockIdx.x * BPH_COUNT : nullptr);
-  for (int sc = blockIdx.x; sc < a.B; sc += gridDim.x) {
+  for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
+    const int sc = w / a.chunks, ch = w - sc * a.chunks;
+    const int r0 = (int)((long long)a.R * ch / a.chunks), r1 = (int)((long long)a.R * (ch + 1) / a.chunks);
     const int ncs = a.soa.nc, n = P.n, nb = P.nb, e = P.e;
     c.nc = a.soa.nc_s ? a.soa.nc_s[sc] : ncs;
     c.b1 = a.soa.b1 + (a.soa.nc_s ? (size_t)sc * ncs : 0);
@@ -1547,20 +1567,23 @@ __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_const
     pf.lap(BPH_STRUCT);
     if (rc != 0) {                                                          // the forward reported it: zero gradients
       const int tid = threadIdx.x;
-      for (int i = tid; i < n; i += NT) { if (a.dv) a.dv[(size_t)sc * n + i] = 0; if (a.dfext) a.dfext[(size_t)sc * n + i] = 0; }
-      for (int i = tid; i < nb; i += NT) { if (a.dmass) a.dmass[(size_t)sc * nb + i] = 0; if (a.dinertia) a.dinertia[(size_t)sc * nb + i] = 0; }
-      for (int i = tid; i < ncs; i += NT) {
-        const size_t ic = (size_t)sc * ncs + i;
-        if (a.dnormal) { a.dnormal[ic * 2] = 0; a.dnormal[ic * 2 + 1] = 0; }
-        if (a.dp1) { a.dp1[ic * 2] = 0; a.dp1[ic * 2 + 1] = 0; }
-        if (a.dp2) { a.dp2[ic * 2] = 0; a.dp2[ic * 2 + 1] = 0; }
-        if (a.drest) a.drest[ic] = 0;
-        if (a.dmu) a.dmu[ic] = 0;
+      for (int r = r0; r < r1; ++r) {
+        const size_t so = (size_t)r * a.B + sc;
+        for (int i = tid; i < n; i += NT) { if (a.dv) a.dv[so * n + i] = 0; if (a.dfext) a.dfext[so * n + i] = 0; }
+        for (int i = tid; i < nb; i += NT) { if (a.dmass) a.dmass[so * nb + i] = 0; if (a.dinertia) a.dinertia[so * nb + i] = 0; }
+        for (int i = tid; i < ncs; i += NT) {
+          const size_t oc = so * ncs + i;
+          if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
+          if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
+          if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
+          if (a.drest) a.drest[oc] = 0;
+          if (a.dmu) a.dmu[oc] = 0;
+        }
+        for (int i = tid; i < e; i += NT) if (a.db) a.db[so * e + i] = 0;
+        if (a.dA) for (int i = tid; i < e * n; i += NT) a.dA[so * e * n + i] = 0;
       }
-      for (int i = tid; i < e; i += NT) if (a.db) a.db[(size_t)sc * e + i] = 0;
-      if (a.dA) for (int i = tid; i < e * n; i += NT) a.dA[(size_t)sc * e * n + i] = 0;
     } else {
-      backward_scene(a, c, pf, sc);
+      backward_scene(a, c, pf, sc, r0, r1);
     }
     __syncthreads();
   }

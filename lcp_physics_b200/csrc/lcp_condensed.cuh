@@ -1130,6 +1130,10 @@ template <typename T>
 struct CBwdArgs {
   CPlan P;
   int B;
+  // R cotangents per scene: g and every gradient output are [R][B][...], slot r of scene sc at row r B + sc.
+  // A work item is (scene, chunk): chunk k of `chunks` factors the scene's KKT matrix once and solves for the
+  // cotangents [R k / chunks, R (k + 1) / chunks).
+  int R, chunks;
   const T *Q, *G, *A, *F;
   const T *zhat, *nu, *lam, *slack, *g;
   T *dQ, *dp, *dG, *dh, *dA, *db, *dF;
@@ -1434,30 +1438,11 @@ __device__ __forceinline__ void write_outer(T* __restrict__ o, int rows, int col
 }
 
 // ------------------------------------------------------------------ backward (lcp.py:37-64), one scene
-template <typename T, int NS, int CS, typename PF>
-__device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc) {
+// The gradients of one cotangent from the solve's dx, dlam, dnu: inputs of scene sc, outputs at row so.
+template <typename T, int CS, typename PF>
+__device__ __forceinline__ void backward_grads(const CBwdArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc, int so) {
   const CPlan& P = a.P;
   const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x;
-  const T* zh = a.zhat + (size_t)sc * n;
-  const T* lam = a.lam + (size_t)sc * P.m;
-  const T* slk = a.slack + (size_t)sc * P.m;
-  const T* nu = e > 0 ? a.nu + (size_t)sc * e : nullptr;
-  for (int i = tid; i < n; i += NT) { S.x()[i] = zh[i]; S.rx()[i] = a.g[(size_t)sc * n + i]; }
-  for (int i = tid; i < m; i += NT) {
-    T d = lam[i] / slk[i];                                                              // :44
-    // fp64 only: at the round-off floor (lambda, s ~ 1e-16) d spans 1e+-16 and the condensed matrix
-    // K = Q + G^T (F + 1/d)^-1 G, which inherits the large entries, can no longer be factored (kappa u >= 1,
-    // exact zero pivots). Clamping d to [1e-10, 1e10] moves the KKT diagonal of rows that are converged
-    // to 1e-16 by < 1e-10 -- far below the 1e-4 at which the reference's own gradients are reproducible
-    // there (tests/test_oracle.py) -- and keeps kappa(K) u <= 1e-6.
-    if (sizeof(T) == 8) d = d > T(1e10) ? T(1e10) : (d < T(1e-10) ? T(1e-10) : d);
-    S.z()[i] = lam[i]; S.s()[i] = slk[i]; S.d()[i] = d; S.rs2()[i] = T(0);
-  }
-  for (int i = tid; i < e; i += NT) S.y()[i] = nu[i];
-  __syncthreads();
-  const bool exact = (a.flags & 1u) != 0;
-  factor_kkt<T, NS, CS>(P, S, st, pf, exact);                                               // :46  (m == 0: K = [[Q, A^T], [A, 0]])
-  solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), nullptr, nullptr, S.dx(), S.ds(), S.dz(), S.dy(), exact);   // :47-50
   const T* dx = S.dx(); const T* dlam = S.dz(); const T* dnu = S.dy();
   if (a.soa.mass) {
     // Engine path: the chain rule through the assembly (world.py:144-234, engines.py:50-116) applied to the
@@ -1470,13 +1455,13 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
     const T* v = E.v + (size_t)sc * n;
     const T* zh_ = S.x(); const T* lm = S.z();
     for (int c = tid; c < ncs; c += NT) {
-      const size_t ic = (size_t)sc * ncs + c;
+      const size_t ic = (size_t)sc * ncs + c, oc = (size_t)so * ncs + c;
       if (c >= nc) {                                              // unused slots of a scene with fewer contacts
-        if (a.dnormal) { a.dnormal[ic * 2] = 0; a.dnormal[ic * 2 + 1] = 0; }
-        if (a.dp1) { a.dp1[ic * 2] = 0; a.dp1[ic * 2 + 1] = 0; }
-        if (a.dp2) { a.dp2[ic * 2] = 0; a.dp2[ic * 2 + 1] = 0; }
-        if (a.drest) a.drest[ic] = 0;
-        if (a.dmu) a.dmu[ic] = 0;
+        if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
+        if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
+        if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
+        if (a.drest) a.drest[oc] = 0;
+        if (a.dmu) a.dmu[oc] = 0;
         continue;
       }
       const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
@@ -1511,17 +1496,17 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
         else if (q == 1) { gny += gdx; gnx += -gdy; }               // dir1 = (ny, -nx)
         else { gny += -gdx; gnx += gdy; }                           // dir2 = (-ny, nx)
       }
-      if (a.dnormal) { a.dnormal[ic * 2] = gnx; a.dnormal[ic * 2 + 1] = gny; }
-      if (a.dp1) { a.dp1[ic * 2] = g1x; a.dp1[ic * 2 + 1] = g1y; }
-      if (a.dp2) { a.dp2[ic * 2] = g2x; a.dp2[ic * 2 + 1] = g2y; }
-      if (a.drest) a.drest[ic] = E.mode == 0 ? dhc * jcv : -dhc * jcv;
-      if (a.dmu) a.dmu[ic] = E.mode == 0 ? -(dlam[3 * nc + c] * lm[c]) : T(0);     // dF[gamma_c][c]  (:54)
+      if (a.dnormal) { a.dnormal[oc * 2] = gnx; a.dnormal[oc * 2 + 1] = gny; }
+      if (a.dp1) { a.dp1[oc * 2] = g1x; a.dp1[oc * 2 + 1] = g1y; }
+      if (a.dp2) { a.dp2[oc * 2] = g2x; a.dp2[oc * 2 + 1] = g2y; }
+      if (a.drest) a.drest[oc] = E.mode == 0 ? dhc * jcv : -dhc * jcv;
+      if (a.dmu) a.dmu[oc] = E.mode == 0 ? -(dlam[3 * nc + c] * lm[c]) : T(0);     // dF[gamma_c][c]  (:54)
     }
     for (int j = tid; j < n; j += NT) {
       const int body = j / 3, comp = j - 3 * body;
       const T md = comp == 0 ? E.inertia[(size_t)sc * nb + body] : E.mass[(size_t)sc * nb + body];
       const T dpj = E.mode == 0 ? dx[j] : T(0);                     // dp = dx (:52); post-stabilisation has p = 0
-      if (a.dfext) a.dfext[(size_t)sc * n + j] = E.dt * dpj;
+      if (a.dfext) a.dfext[(size_t)so * n + j] = E.dt * dpj;
       if (a.dv) {
         T acc = md * dpj;
         const int cnt = S.clcnt()[j];
@@ -1530,10 +1515,10 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
           const T hs_ = E.mode == 0 ? E.rest[(size_t)sc * ncs + c] : (T(1) - E.rest[(size_t)sc * ncs + c]);
           acc += -dlam[c] * hs_ * S.Gd()[(size_t)pslot * P.pcap + c];      // dh_c d(h_c)/dv_j, Jc row = slot-0 rows of Gd
         }
-        a.dv[(size_t)sc * n + j] = acc;
+        a.dv[(size_t)so * n + j] = acc;
       }
       const T dqjj = dx[j] * zh_[j];                                // dQ_jj = 1/2 (dx_j z_j + z_j dx_j)  (:61)
-      if (comp == 0 && a.dinertia) a.dinertia[(size_t)sc * nb + body] = dqjj + dpj * v[j];
+      if (comp == 0 && a.dinertia) a.dinertia[(size_t)so * nb + body] = dqjj + dpj * v[j];
     }
     __syncthreads();
     for (int body = tid; body < nb; body += NT) {
@@ -1543,11 +1528,11 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
         const int j = 3 * body + comp;
         acc += dx[j] * zh_[j] + (E.mode == 0 ? dx[j] : T(0)) * v[j];
       }
-      a.dmass[(size_t)sc * nb + body] = acc;
+      a.dmass[(size_t)so * nb + body] = acc;
     }
-    if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)sc * e + i] = -dnu[i];
+    if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)so * e + i] = -dnu[i];
     if (a.dA && e > 0) {
-      T* o = a.dA + (size_t)sc * e * n;
+      T* o = a.dA + (size_t)so * e * n;
       for (int i = 0; i < e; ++i)
         for (int j = tid; j < n; j += NT) o[(size_t)i * n + j] = dnu[i] * S.x()[j] + S.y()[i] * dx[j];
     }
@@ -1556,21 +1541,57 @@ __device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S
     pf.lap(CPH_GRADS);
     return;
   }
-  if (a.dp) for (int i = tid; i < n; i += NT) a.dp[(size_t)sc * n + i] = dx[i];                       // :52
-  if (a.dh) for (int i = tid; i < m; i += NT) a.dh[(size_t)sc * m + i] = -dlam[i];                    // :55
-  if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)sc * e + i] = -dnu[i];            // :58
+  if (a.dp) for (int i = tid; i < n; i += NT) a.dp[(size_t)so * n + i] = dx[i];                       // :52
+  if (a.dh) for (int i = tid; i < m; i += NT) a.dh[(size_t)so * m + i] = -dlam[i];                    // :55
+  if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)so * e + i] = -dnu[i];            // :58
   // the four dense outer products (0.4 MB per scene at cfg 3): 16-byte stores, V elements of one row per thread
   if (a.dG)                                                      // :53  dlam (x) zhat + lam (x) dx
-    write_outer<T>(a.dG + (size_t)sc * m * n, m, n, [&](int i, int j) { return dlam[i] * S.x()[j] + S.z()[i] * dx[j]; });
+    write_outer<T>(a.dG + (size_t)so * m * n, m, n, [&](int i, int j) { return dlam[i] * S.x()[j] + S.z()[i] * dx[j]; });
   if (a.dF)                                                      // :54  -dlam (x) lam
-    write_outer<T>(a.dF + (size_t)sc * m * m, m, m, [&](int i, int j) { return -(dlam[i] * S.z()[j]); });
+    write_outer<T>(a.dF + (size_t)so * m * m, m, m, [&](int i, int j) { return -(dlam[i] * S.z()[j]); });
   if (a.dA && e > 0)                                             // :57
-    write_outer<T>(a.dA + (size_t)sc * e * n, e, n, [&](int i, int j) { return dnu[i] * S.x()[j] + S.y()[i] * dx[j]; });
+    write_outer<T>(a.dA + (size_t)so * e * n, e, n, [&](int i, int j) { return dnu[i] * S.x()[j] + S.y()[i] * dx[j]; });
   if (a.dQ)                                                      // :61
-    write_outer<T>(a.dQ + (size_t)sc * n * n, n, n, [&](int i, int j) { return T(0.5) * (dx[i] * S.x()[j] + S.x()[i] * dx[j]); });
+    write_outer<T>(a.dQ + (size_t)so * n * n, n, n, [&](int i, int j) { return T(0.5) * (dx[i] * S.x()[j] + S.x()[i] * dx[j]); });
   if (tid == 0 && a.done) a.done[sc] = 1;
   __syncthreads();
   pf.lap(CPH_GRADS);
+}
+
+// One factorisation at the saved solution, then one solve and chain rule per cotangent r in [r0, r1): the
+// factors, W and the structure in shared memory are read-only to solve_kkt, so every round sees the same matrix.
+template <typename T, int NS, int CS, typename PF>
+__device__ __forceinline__ void backward_scene(const CBwdArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc,
+                                               int r0, int r1) {
+  const CPlan& P = a.P;
+  const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x;
+  const T* zh = a.zhat + (size_t)sc * n;
+  const T* lam = a.lam + (size_t)sc * P.m;
+  const T* slk = a.slack + (size_t)sc * P.m;
+  const T* nu = e > 0 ? a.nu + (size_t)sc * e : nullptr;
+  for (int i = tid; i < n; i += NT) S.x()[i] = zh[i];
+  for (int i = tid; i < m; i += NT) {
+    T d = lam[i] / slk[i];                                                              // :44
+    // fp64 only: at the round-off floor (lambda, s ~ 1e-16) d spans 1e+-16 and the condensed matrix
+    // K = Q + G^T (F + 1/d)^-1 G, which inherits the large entries, can no longer be factored (kappa u >= 1,
+    // exact zero pivots). Clamping d to [1e-10, 1e10] moves the KKT diagonal of rows that are converged
+    // to 1e-16 by < 1e-10 -- far below the 1e-4 at which the reference's own gradients are reproducible
+    // there (tests/test_oracle.py) -- and keeps kappa(K) u <= 1e-6.
+    if (sizeof(T) == 8) d = d > T(1e10) ? T(1e10) : (d < T(1e-10) ? T(1e-10) : d);
+    S.z()[i] = lam[i]; S.s()[i] = slk[i]; S.d()[i] = d;
+  }
+  for (int i = tid; i < e; i += NT) S.y()[i] = nu[i];
+  __syncthreads();
+  const bool exact = (a.flags & 1u) != 0;
+  factor_kkt<T, NS, CS>(P, S, st, pf, exact);                                               // :46  (m == 0: K = [[Q, A^T], [A, 0]])
+  for (int r = r0; r < r1; ++r) {
+    const int so = r * a.B + sc;                                  // output row of (cotangent r, scene sc)
+    for (int i = tid; i < n; i += NT) S.rx()[i] = a.g[(size_t)so * n + i];
+    for (int i = tid; i < m; i += NT) S.rs2()[i] = T(0);
+    __syncthreads();
+    solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), nullptr, nullptr, S.dx(), S.ds(), S.dz(), S.dy(), exact);   // :47-50
+    backward_grads<T, CS>(a, S, st, pf, sc, so);
+  }
 }
 
 template <typename T, int NS, bool PROF>
@@ -1580,7 +1601,8 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
   const int n = P.n, m = P.m, e = P.e, tid = threadIdx.x;
   __shared__ int singular_s;
   Prof<PROF> pf(PROF ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr);
-  for (int sc = blockIdx.x; sc < a.B; sc += gridDim.x) {
+  for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
+    const int sc = w / a.chunks, k = w - sc * a.chunks;
     if (a.only && !a.only[sc]) continue;
     if (tid == 0) singular_s = 0;
     __syncthreads();
@@ -1600,13 +1622,14 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
       continue;
     }
     if constexpr (LU_BW < NS - 1) mark_band_lu<T>(P, S, st);   // also after load_structure: the saved column lists give the same answer
+    const int r0 = (int)((long long)a.R * k / a.chunks), r1 = (int)((long long)a.R * (k + 1) / a.chunks);
     switch (st.cs) {
-      case 1: backward_scene<T, NS, 1>(a, S, st, pf, sc); break;
-      case 2: backward_scene<T, NS, 2>(a, S, st, pf, sc); break;
-      case 3: backward_scene<T, NS, 3>(a, S, st, pf, sc); break;
-      case 4: backward_scene<T, NS, 4>(a, S, st, pf, sc); break;
-      case 5: backward_scene<T, NS, 5>(a, S, st, pf, sc); break;
-      default: backward_scene<T, NS, 6>(a, S, st, pf, sc); break;
+      case 1: backward_scene<T, NS, 1>(a, S, st, pf, sc, r0, r1); break;
+      case 2: backward_scene<T, NS, 2>(a, S, st, pf, sc, r0, r1); break;
+      case 3: backward_scene<T, NS, 3>(a, S, st, pf, sc, r0, r1); break;
+      case 4: backward_scene<T, NS, 4>(a, S, st, pf, sc, r0, r1); break;
+      case 5: backward_scene<T, NS, 5>(a, S, st, pf, sc, r0, r1); break;
+      default: backward_scene<T, NS, 6>(a, S, st, pf, sc, r0, r1); break;
     }
     __syncthreads();
   }

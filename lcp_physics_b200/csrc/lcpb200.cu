@@ -3,6 +3,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <algorithm>
+#include <climits>
 #include <new>
 #include <string>
 #include <vector>
@@ -384,6 +385,7 @@ static int launch_backward(lcpb200_handle_s* h, int slot, int B, const void* Q, 
   if (have_cond) {
     c.P = h->cplan;
     c.B = B;
+    c.R = 1; c.chunks = 1;
     c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
     c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
     c.g = (const T*)g;
@@ -816,8 +818,14 @@ extern "C" int lcpb200_engine_forward(lcpb200_handle_t h, int B, int nb, int nc,
                                         iters, resid, st);
 }
 
+// Work items per scene of a backward with R cotangents: enough (scene, chunk) items to fill `target` CTAs, each of
+// which factors its scene once; never more chunks than cotangents.
+static int bwd_chunks(int R, int B, int target) {
+  return std::max(1, std::min(R, (target + B - 1) / B));
+}
+
 template <typename T>
-static int engine_backward_t(lcpb200_handle_s* h, int B, int nb, int nc, int mode, double dt, const void* mass,
+static int engine_backward_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int mode, double dt, const void* mass,
                              const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
                              const void* p2, const int32_t* b1, const int32_t* b2, const int32_t* ncs, const void* mu,
                              const void* rest, const void* A, const void* zhat, const void* nu, const void* lam, const void* slack,
@@ -828,6 +836,7 @@ static int engine_backward_t(lcpb200_handle_s* h, int B, int nb, int nc, int mod
   cnd::CBwdArgs<T> c;
   c.P = h->cplan;
   c.B = B;
+  c.R = R; c.chunks = bwd_chunks(R, B, h->cond_grid);
   c.Q = nullptr; c.G = nullptr; c.F = nullptr; c.A = (const T*)A;
   c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack; c.g = (const T*)g;
   c.dQ = c.dp = c.dG = c.dh = c.dF = nullptr;
@@ -837,7 +846,7 @@ static int engine_backward_t(lcpb200_handle_s* h, int B, int nb, int nc, int mod
   fill_soa<T>(c.soa, h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, b1, b2, mu, rest, ncs);
   c.dmass = (T*)dmass; c.dinertia = (T*)dinertia; c.dv = (T*)dv; c.dfext = (T*)dfext; c.dnormal = (T*)dnormal;
   c.dp1 = (T*)dp1; c.dp2 = (T*)dp2; c.dmu = (T*)dmu; c.drest = (T*)drest;
-  const int cgrid = std::min(B, h->cond_grid);
+  const int cgrid = (int)std::min((long long)B * c.chunks, (long long)h->cond_grid);
 #define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, cgrid, st)
   const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
 #undef CALL_BWD
@@ -845,15 +854,18 @@ static int engine_backward_t(lcpb200_handle_s* h, int B, int nb, int nc, int mod
   return 0;
 }
 
-extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode, double dt,
-                                       const void* mass, const void* inertia, const void* v, const void* fext,
-                                       const void* normal, const void* p1, const void* p2, const int32_t* body1,
-                                       const int32_t* body2, const int32_t* contact_count, const void* mu,
-                                       const void* restitution, const void* A, const void* zhat, const void* nu, const void* lam, const void* slack,
-                                       const void* dl_dzhat, void* dmass, void* dinertia, void* dv, void* dfext,
-                                       void* dnormal, void* dp1, void* dp2, void* dmu, void* drestitution, void* dA,
-                                       void* db, unsigned flags, void* stream) {
+extern "C" int lcpb200_engine_backward_batched(lcpb200_handle_t h, int R, int B, int nb, int nc, int mode, double dt,
+                                               const void* mass, const void* inertia, const void* v, const void* fext,
+                                               const void* normal, const void* p1, const void* p2, const int32_t* body1,
+                                               const int32_t* body2, const int32_t* contact_count, const void* mu,
+                                               const void* restitution, const void* A, const void* zhat, const void* nu,
+                                               const void* lam, const void* slack, const void* dl_dzhat, void* dmass,
+                                               void* dinertia, void* dv, void* dfext, void* dnormal, void* dp1, void* dp2,
+                                               void* dmu, void* drestitution, void* dA, void* db, unsigned flags,
+                                               void* stream) {
   if (int rc = check_engine(h, B, nb, nc, mode)) return rc;
+  if (R < 1) return fail("engine_backward_batched: need R >= 1");
+  if ((long long)R * B > INT_MAX) return fail("engine_backward_batched: R * B exceeds INT_MAX");
   if (!mass || !inertia || !v || !normal || !p1 || !p2 || !body1 || !body2 || !restitution) return fail("engine_backward: NULL input");
   if (mode == 0 && !mu) return fail("engine_backward: mu is needed for mode 0");
   if (!zhat || !lam || !slack || !dl_dzhat) return fail("zhat, lam, slack, dl_dzhat must be non-NULL");
@@ -865,10 +877,13 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   if (use_banded(h)) {
-    if (int rc = ensure_bplan(h, B, nb, nc, mode)) return rc;
+    const int chunks = bwd_chunks(R, B, h->num_sms);
+    const int items = B * chunks;
+    if (int rc = ensure_bplan(h, items, nb, nc, mode)) return rc;     // one L2 workspace per CTA of this grid
     bnd::BBwdArgs a;
     a.P = h->bplan;
     a.B = B;
+    a.R = R; a.chunks = chunks;
     memset(&a.soa, 0, sizeof(a.soa));
     a.soa.mass = (const double*)mass; a.soa.inertia = (const double*)inertia; a.soa.v = (const double*)v;
     a.soa.fext = (const double*)fext; a.soa.normal = (const double*)normal; a.soa.p1 = (const double*)p1;
@@ -884,16 +899,29 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
     a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
     a.prof = h->cprof;
     a.flags = flags;
-    CK(bnd::launch_band_backward(a, std::min(B, h->num_sms), st));
+    CK(bnd::launch_band_backward(a, std::min(items, h->num_sms), st));
     return 0;
   }
   return h->dtype == LCPB200_F32
-             ? engine_backward_t<float>(h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
+             ? engine_backward_t<float>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
                                         contact_count, mu, restitution, A, zhat, nu, lam, slack, dl_dzhat, dmass, dinertia, dv, dfext,
                                         dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, st)
-             : engine_backward_t<double>(h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
+             : engine_backward_t<double>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
                                          contact_count, mu, restitution, A, zhat, nu, lam, slack, dl_dzhat, dmass, dinertia, dv, dfext,
                                          dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, st);
+}
+
+extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode, double dt,
+                                       const void* mass, const void* inertia, const void* v, const void* fext,
+                                       const void* normal, const void* p1, const void* p2, const int32_t* body1,
+                                       const int32_t* body2, const int32_t* contact_count, const void* mu,
+                                       const void* restitution, const void* A, const void* zhat, const void* nu, const void* lam, const void* slack,
+                                       const void* dl_dzhat, void* dmass, void* dinertia, void* dv, void* dfext,
+                                       void* dnormal, void* dp1, void* dp2, void* dmu, void* drestitution, void* dA,
+                                       void* db, unsigned flags, void* stream) {
+  return lcpb200_engine_backward_batched(h, 1, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
+                                         contact_count, mu, restitution, A, zhat, nu, lam, slack, dl_dzhat, dmass, dinertia,
+                                         dv, dfext, dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, stream);
 }
 
 // ------------------------------------------------------------------ assembly

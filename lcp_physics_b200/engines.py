@@ -93,13 +93,69 @@ def assemble_contacts(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, b
     return _AssembleFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2, dt)
 
 
+def _engine_backward(dzhat, meta, saved):
+    """lcpb200_engine_backward_batched: dzhat [..., B, n] -> the 11 gradients (mass ... rest, A, b), each with
+    dzhat's leading dims in front. The leading dims are the R cotangents of one call: each scene's KKT matrix is
+    factored once for all of them."""
+    lib = _lib.load()
+    (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = saved
+    dt, mode, exact, B, nb, nc, e = meta
+    dev = mass.device
+    lead = tuple(dzhat.shape[:-2])
+    g = dzhat.reshape(-1, B, 3 * nb).contiguous()
+    R = g.shape[0]
+    z = lambda t: torch.zeros((R,) + tuple(t.shape), dtype=t.dtype, device=dev)
+    outs = [z(mass), z(inertia), z(v), z(fext), z(normal), z(p1), z(p2), z(mu), z(rest)]
+    dA = z(A) if e > 0 else None
+    db = torch.zeros(R, B, e, dtype=mass.dtype, device=dev) if e > 0 else None
+    ins = [t.contiguous() for t in (mass, inertia, v, fext, normal, p1, p2)]
+    hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, dev.index,
+                         torch.cuda.current_stream(dev).cuda_stream)
+    with torch.cuda.device(dev):
+        _lib.check(lib.lcpb200_engine_backward_batched(
+            hd.raw, R, B, nb, nc, mode, dt, *[_lib.ptr(t) for t in ins],
+            _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu.contiguous()), _lib.ptr(rest.contiguous()),
+            _lib.ptr(A.contiguous() if e > 0 else None), *[_lib.ptr(t) for t in (zhat, nu, lam, slack, g)],
+            *[_lib.ptr(t) for t in outs], _lib.ptr(dA), _lib.ptr(db), 1 if exact else 0, _stream_ptr(dev)))
+    return tuple(None if t is None else t.reshape(lead + tuple(t.shape[1:])) for t in (*outs, dA, db))
+
+
+class _EngineVjpFn(torch.autograd.Function):
+    """The vector-Jacobian product of engine_solve: dl/dzhat and the saved solve in, gradients w.r.t. the contact
+    list out. Under torch.func.vmap (vmap of a torch.func.vjp, jacrev) the cotangents of every vmapped call
+    arrive together and go to ONE batched kernel call, which factors each scene's KKT matrix once for all of them."""
+
+    @staticmethod
+    def forward(dzhat, meta, *saved):
+        return _engine_backward(dzhat, meta, saved)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError("engine_solve: second derivatives are not implemented")
+
+    @staticmethod
+    def vmap(info, in_dims, dzhat, meta, *saved):
+        if any(d is not None for d in in_dims[2:]):
+            raise NotImplementedError(
+                "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
+                "instead (vmap of the vector-Jacobian product -- torch.func.vjp, jacrev -- is supported)")
+        # one more leading cotangent dim; apply (not forward) so that an enclosing vmap level batches it again
+        outs = _EngineVjpFn.apply(dzhat.movedim(in_dims[0], 0), meta, *saved)
+        return outs, tuple(None if t is None else 0 for t in outs)
+
+
 class _EngineSolveFn(torch.autograd.Function):
     """Fused path (lcpb200_engine_forward / _backward): contact structure-of-arrays in, LCP solution out.
     No dense Q / G / F exists anywhere; the backward returns gradients w.r.t. the contact list.
-    mode 0 = solve_dynamics' LCP (engines.py:50-76), mode 1 = post_stabilization's (engines.py:80-116)."""
+    mode 0 = solve_dynamics' LCP (engines.py:50-76), mode 1 = post_stabilization's (engines.py:80-116).
+    Written in setup_context form so that torch.func.vjp / grad / jacrev can trace through it."""
 
     @staticmethod
-    def forward(ctx, mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode, max_iter, exact,
+    def forward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode, max_iter, exact,
                 counts=None):
         lib = _lib.load()
         B, nb = mass.shape
@@ -121,31 +177,30 @@ class _EngineSolveFn(torch.autograd.Function):
                 hd.raw, B, nb, nc, int(mode), float(dt), *[_lib.ptr(t) for t in ins], _lib.ptr(body1), _lib.ptr(body2),
                 _lib.ptr(counts), _lib.ptr(mu_c), _lib.ptr(rest_c), _lib.ptr(A_c), _lib.ptr(b_c), 1e-12, 3, int(max_iter),
                 *[_lib.ptr(t) for t in (zhat, nu, lam, slack, status, iters, resid)], _stream_ptr(dev)))
-        ctx.save_for_backward(*ins, mu_c, rest_c, A_c, body1, body2, zhat, nu, lam, slack, counts)
-        ctx.meta = (float(dt), int(mode), bool(exact), B, nb, nc, e)
         _last_info.update(iters=iters, resid=resid, status=status, lam=lam, slack=slack, nu=nu)
-        ctx.mark_non_differentiable(status)
-        return zhat, status
+        return zhat, status, nu, lam, slack
 
     @staticmethod
-    def backward(ctx, dzhat, _dstatus):
-        lib = _lib.load()
-        (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = ctx.saved_tensors
-        dt, mode, exact, B, nb, nc, e = ctx.meta
-        dev = mass.device
-        z = torch.zeros_like
-        outs = [z(mass), z(inertia), z(v), z(fext), z(normal), z(p1), z(p2), z(mu), z(rest)]
-        dA = z(A) if e > 0 else None
-        db = torch.zeros(B, e, dtype=mass.dtype, device=dev) if e > 0 else None
-        hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, dev.index,
-                             torch.cuda.current_stream(dev).cuda_stream)
-        with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_engine_backward(
-                hd.raw, B, nb, nc, mode, dt, *[_lib.ptr(t) for t in (mass, inertia, v, fext, normal, p1, p2)],
-                _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu), _lib.ptr(rest), _lib.ptr(A),
-                *[_lib.ptr(t) for t in (zhat, nu, lam, slack, dzhat.contiguous())],
-                *[_lib.ptr(t) for t in outs], _lib.ptr(dA), _lib.ptr(db), 1 if exact else 0, _stream_ptr(dev)))
-        return (*outs, dA, db, None, None, None, None, None, None, None)
+    def setup_context(ctx, inputs, output):
+        (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode, max_iter, exact) = inputs[:17]
+        counts = inputs[17] if len(inputs) > 17 else None
+        zhat, status, nu, lam, slack = output
+        B, nb = mass.shape
+        e = A.shape[1] if (A is not None and A.dim() > 1) else 0
+        ctx.save_for_backward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2,
+                              zhat, nu, lam, slack, counts)
+        ctx.meta = (float(dt), int(mode), bool(exact), B, nb, normal.shape[1], e)
+        ctx.mark_non_differentiable(*[t for t in (status, nu, lam, slack) if t is not None])
+
+    @staticmethod
+    def backward(ctx, dzhat, *_):
+        grads = _EngineVjpFn.apply(dzhat, ctx.meta, *ctx.saved_tensors)
+        return (*grads, None, None, None, None, None, None, None)
+
+    @staticmethod
+    def vmap(info, in_dims, *args):
+        raise NotImplementedError(
+            "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 instead")
 
 
 _last_info = {}
@@ -170,8 +225,9 @@ def engine_solve(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2,
     three columns only -- the reference's formulation with the obstacle pinned by a TotalConstraint, reduced by the
     pinned dofs; its p2 is unused (zero gradient). body1 must be a body (< nb)."""
     _lib.require_cuda()
-    return _EngineSolveFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode,
-                                max_iter, exact_adjoint, counts)
+    zhat, status = _EngineSolveFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode,
+                                        max_iter, exact_adjoint, counts)[:2]
+    return zhat, status
 
 
 class B200PdipmEngine(Engine):

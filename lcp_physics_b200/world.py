@@ -188,6 +188,34 @@ def _polar_to_cart(r, th):
     return torch.stack([torch.cos(th) * r, torch.sin(th) * r], 1)
 
 
+class _DetectFn(torch.autograd.Function):
+    """Runs `fn(*tensors)`, a contact-detection kernel call, on plain tensors: under torch.func transforms (vjp in
+    BatchedWorld.linearize) the arguments arrive unwrapped, so the kernel can read their storage. Its outputs --
+    contact indices, counts, features and the kernel's geometry, which is used only when nothing is differentiated --
+    are not differentiable."""
+
+    @staticmethod
+    def forward(fn, *tensors):
+        return fn(*tensors)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.n_inputs = len(inputs)
+        ctx.mark_non_differentiable(*output)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        return (None,) * ctx.n_inputs
+
+
+def _detect(fn, *tensors):
+    """fn(*tensors); through _DetectFn when a torch.func transform has wrapped an argument (such a wrapper has no
+    storage a kernel could read). Ordinary steps call the kernel directly."""
+    if any(t is not None and torch._C._functorch.is_functorch_wrapped_tensor(t) for t in tensors):
+        return _DetectFn.apply(fn, *tensors)
+    return fn(*tensors)
+
+
 def _pad_vertices(v, V):
     """[B, n, V0, 2] -> [B, n, V, 2] (V >= V0) by repeating the last vertex: a zero-length edge, skipped by every rule."""
     if v.shape[2] == V:
@@ -441,30 +469,38 @@ class BatchedWorld:
         lib = _lib.load()
         B, cap, dev = self.B, self.cap, self.device
         pos = self.p[:, :, 1:]
+
+        def walk(pos_c, rad):
+            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            counts = torch.empty(B, dtype=torch.int32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.lcpb200_find_contacts(_lib.dtype_code(self.dtype), B, self.nb, cap, self.eps,
+                                                     _lib.ptr(pos_c), _lib.ptr(rad), _lib.ptr(b1), _lib.ptr(b2),
+                                                     _lib.ptr(counts),
+                                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            return b1, b2, counts
         pos_c = pos.detach().contiguous()
-        b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        counts = torch.empty(B, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_find_contacts(_lib.dtype_code(self.dtype), B, self.nb, cap, self.eps, _lib.ptr(pos_c),
-                                                 _lib.ptr(self.rad), _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts),
-                                                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        b1, b2, counts = _detect(walk, pos_c, self.rad)
         if int(counts.max()) > cap:
             raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
         self.c_b1, self.c_b2, self.counts = b1, b2, counts
         needs_graph = torch.is_grad_enabled() and any(t.requires_grad for t in (self.p, self.rad, self.fric_coeff, self.restitution))
         if not needs_graph:
             # nothing to differentiate: the geometry of the selected pairs in one kernel as well
-            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-            self.c_normal, self.c_p1, self.c_p2 = new(2), new(2), new(2)
-            self.c_pen, self.c_mu, self.c_rest = new(), new(), new()
-            with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_contact_geometry(
-                    _lib.dtype_code(self.dtype), B, self.nb, cap, _lib.ptr(pos_c), _lib.ptr(self.rad.detach().contiguous()),
-                    _lib.ptr(self.fric_coeff.detach().contiguous()), _lib.ptr(self.restitution.detach().contiguous()),
-                    _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts),
-                    *[_lib.ptr(t) for t in (self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest)],
-                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            def geometry(pos_c, rad, fric, rest, b1, b2, counts):
+                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+                geo = (new(2), new(2), new(2), new(), new(), new())
+                with torch.cuda.device(dev):
+                    _lib.check(lib.lcpb200_contact_geometry(
+                        _lib.dtype_code(self.dtype), B, self.nb, cap, _lib.ptr(pos_c), _lib.ptr(rad), _lib.ptr(fric),
+                        _lib.ptr(rest), _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
+                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                return geo
+            d = lambda t: t.detach().contiguous()
+            (self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu,
+             self.c_rest) = _detect(geometry, pos_c, d(self.rad), d(self.fric_coeff), d(self.restitution), b1, b2,
+                                    counts)
             return
         i1, i2 = b1.long(), b2.long()
         take = lambda t, idx: torch.gather(t, 1, idx)
@@ -489,24 +525,27 @@ class BatchedWorld:
         comes from the same call, or from torch ops (_geometry_torch) when something needs autograd."""
         lib = _lib.load()
         B, cap, dev = self.B, self.cap, self.device
-        pos_c = self.p[:, :, 1:].detach().contiguous()
-        b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        counts = torch.empty(B, dtype=torch.int32, device=dev)
         needs_graph = torch.is_grad_enabled() and any(
             t.requires_grad for t in (self.p, self.rad, self.fric_coeff, self.restitution, self.ov, self.ofric, self.orest))
         d = lambda t: t.detach().contiguous()
-        geo = [None] * 6
-        if not needs_graph:
-            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-            geo = [new(2), new(2), new(2), new(), new(), new()]
-        with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_world_contacts(
-                _lib.dtype_code(self.dtype), B, self.nb, self.no, self.nv, cap, self.eps, _lib.ptr(pos_c),
-                *[_lib.ptr(d(t)) for t in (self.rad, self.fric_coeff, self.restitution, self.ov, self.oref, self.ofric,
-                                           self.orest)],
-                _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
-                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+
+        def walk(*ins):
+            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            counts = torch.empty(B, dtype=torch.int32, device=dev)
+            geo = [None] * 6
+            if not needs_graph:
+                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+                geo = [new(2), new(2), new(2), new(), new(), new()]
+            with torch.cuda.device(dev):
+                _lib.check(lib.lcpb200_world_contacts(
+                    _lib.dtype_code(self.dtype), B, self.nb, self.no, self.nv, cap, self.eps,
+                    *[_lib.ptr(t) for t in ins], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
+                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            return (b1, b2, counts) + (() if needs_graph else tuple(geo))
+        out = _detect(walk, *[d(t) for t in (self.p[:, :, 1:], self.rad, self.fric_coeff, self.restitution,
+                                                     self.ov, self.oref, self.ofric, self.orest)])
+        b1, b2, counts, geo = out[0], out[1], out[2], out[3:]
         if int(counts.max()) > cap:
             raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
         self.c_b1, self.c_b2, self.counts = b1, b2, counts
@@ -535,31 +574,37 @@ class BatchedWorld:
         pverts = self.polygon_vertices() if self.np else None
         pcen = self.p[:, nb:, 1:] if self.np else None
         poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
-        b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        feat = torch.empty(B, cap, dtype=torch.int32, device=dev)
-        counts = torch.empty(B, dtype=torch.int32, device=dev)
         obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
         needs_graph = torch.is_grad_enabled() and any(
             t is not None and t.requires_grad
             for t in (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
         d = lambda t: t.detach().contiguous() if t is not None else None
-        geo = [None] * 6
-        if not needs_graph:
-            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-            geo = [new(2), new(2), new(2), new(), new(), new()]
-        # contiguous copies held until the call returns (a temporary's memory could be reused before the kernel runs)
-        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
-               + obst]
         # worlds with no_contact pairs: the same walk reading the pair-exclusion mask (every world kind)
         masked = self.nc_mask is not None
         fn = lib.lcpb200_body_contacts_masked if masked else lib.lcpb200_body_contacts
-        with torch.cuda.device(dev):
-            _lib.check(fn(
-                _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps, *[_lib.ptr(t) for t in ins],
-                _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat), *[_lib.ptr(t) for t in geo],
-                *((_lib.ptr(self.nc_mask),) if masked else ()),
-                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+
+        def walk(*ins):
+            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            feat = torch.empty(B, cap, dtype=torch.int32, device=dev)
+            counts = torch.empty(B, dtype=torch.int32, device=dev)
+            geo = [None] * 6
+            if not needs_graph:
+                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+                geo = [new(2), new(2), new(2), new(), new(), new()]
+            with torch.cuda.device(dev):
+                _lib.check(fn(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps,
+                    *[_lib.ptr(t) for t in ins[:-1]], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat),
+                    *[_lib.ptr(t) for t in geo], *((_lib.ptr(ins[-1]),) if masked else ()),
+                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            return (b1, b2, feat, counts) + (() if needs_graph else tuple(geo))
+        # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the
+        # kernel runs)
+        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
+               + obst]
+        out = _detect(walk, *ins, self.nc_mask)
+        b1, b2, feat, counts, geo = out[0], out[1], out[2], out[3], out[4:]
         if int(counts.max()) > cap:
             raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
         self.c_b1, self.c_b2, self.c_feat, self.counts = b1, b2, feat, counts
@@ -824,3 +869,47 @@ class BatchedWorld:
 
     def get_p(self):
         return self.p.reshape(self.B, self.n)
+
+    # ------------------------------------------------------------------ Jacobian of a step
+    def linearize(self, chunk_size=None):
+        """The Jacobian of one `step()` from the current state, per scene: returns (x_next [B, 2n], A [B, 2n, 2n],
+        Bu [B, 2n, n]) with x = (get_p(), v) and x_next = f(x, u) the state after the step. u is an additive
+        generalised force on the n dofs for this step (zero here; it enters like `external_force`). Rows of A and Bu:
+        p' then v'. What model-predictive control, iLQR and Gauss-Newton identification linearise around.
+
+        It is the Jacobian of the branch `step()` takes: the contact set, each scene's dt-halving count and the hull
+        features are those of the step from this state, held fixed. Post-stabilisation, constraints, `no_contact`,
+        obstacles, polygons and `external_force` are included; the internal state of a `Joint` (its anchor angle) is
+        held fixed and is not part of x. Gradients through the LCP follow `exact_adjoint`: with friction on, only
+        exact_adjoint=True gives the true derivative (DESIGN.md section 3.4).
+
+        One `torch.func.vjp` of the step, then a `vmap` over the 2n one-hot cotangents (each placed in every scene at
+        once: scenes are independent), `chunk_size` of them per pass (all at once by default; smaller chunks bound the
+        memory). Each pass factors every scene's KKT matrix once for all of its cotangents. The world is left as it
+        was (state, joints, contact list); only `last_solve_info()` then describes the linearisation's solves."""
+        B, n = self.B, self.n
+        saved = dict(self.__dict__)
+        saved_joints = [None if st is None else list(st) for st in self._jstate]
+        ef = self.external_force
+        x0 = torch.cat([self.get_p(), self.v], 1).detach()
+
+        def f(x, u):
+            self.p = x[:, :n].reshape(B, self.nd, 3)
+            self.v = x[:, n:]
+            ub = u.reshape(B, self.nd, 3)
+            self.external_force = (lambda t: ub) if ef is None else (lambda t: ef(t) + ub)
+            self.find_contacts()                              # the contact geometry as a function of p
+            self.step_dt(self.dt)
+            return torch.cat([self.get_p(), self.v], 1)
+
+        try:
+            x_next, vjp_fn = torch.func.vjp(f, x0, x0.new_zeros(B, n))
+            eye = torch.eye(2 * n, dtype=x0.dtype, device=x0.device).unsqueeze(1).expand(-1, B, -1)
+            ja, jb = torch.func.vmap(vjp_fn, chunk_size=chunk_size)(eye)          # [2n, B, 2n], [2n, B, n]
+        finally:
+            self.__dict__.clear()
+            self.__dict__.update(saved)
+            for st, old in zip(self._jstate, saved_joints):            # the step moved the joints in place
+                if st is not None:
+                    st[:] = old
+        return x_next.detach(), ja.transpose(0, 1).contiguous(), jb.transpose(0, 1).contiguous()
