@@ -142,63 +142,24 @@ int lcpb200_backward_host(lcpb200_handle_t h, int B,
                           void* dQ, void* dp, void* dG, void* dh, void* dA, void* db, void* dF,
                           unsigned flags);
 
-/* Contact detection for B scenes of nb circles (replaces the pair loop of World.find_contacts,
- * physics/world.py:139-142, with the circle-circle test of physics/contacts.py:68-80: a pair (i < j) is a
- * contact iff rad_i + rad_j - |pos_i - pos_j| >= -eps). Device pointers:
- *   pos[B,nb,2] rad[B,nb]                      body centres and radii (dtype)
- *   body1[B,cap] body2[B,cap] int32            OUT: the touching pairs of every scene in lexicographic pair
- *                                              order (the order the reference appends contacts in), padded
- *                                              with the pair (0, 1)
- *   counts[B] int32                            OUT: number of touching pairs (may exceed cap: then the lists
- *                                              hold the first cap pairs and the caller must grow cap)
- * The contact geometry (normal, p1, p2, penetration) of the selected pairs is the caller's (it is O(cap) and,
- * in the torch mirror, differentiable). */
-int lcpb200_find_contacts(int dtype, int B, int nb, int cap, double eps, const void* pos, const void* rad,
-                          int32_t* body1, int32_t* body2, int32_t* counts, void* stream);
-
-/* Geometry and material of the pairs selected by lcpb200_find_contacts (contacts.py:69-77, world.py:144-151,
- * :213-224), for callers that do not differentiate through the contact generation:
- *   normal[B,cap,2] = (pos1 - pos2) / dist, penetration[B,cap] = r1 + r2 - dist (-1e30 in unused slots),
- *   p1 = -normal (r1 - pen / 2), p2 = normal (r2 - pen / 2), mu / restitution[B,cap] = mean of the two bodies'
- *   fric_coeff[B,nb] / restitution[B,nb]. */
-int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const void* pos, const void* rad,
-                             const void* fric_coeff, const void* restitution, const int32_t* body1,
-                             const int32_t* body2, const int32_t* counts, void* normal, void* p1, void* p2,
-                             void* penetration, void* mu, void* restitution_c, void* stream);
-
-/* Contact detection and geometry for B scenes of nb circles and no static convex polygon obstacles (walls, floors,
- * ramps: no degrees of freedom). The pairs of the body list [circles 0..nb-1, obstacles nb..nb+no-1] are visited in
- * lexicographic order -- circle-circle pairs (i, j) and circle-obstacle pairs (i, nb + k) -- which is the contact
- * order of a reference World whose bodies are [circles..., obstacles...]; obstacles never pair with each other.
- * Circle-circle pairs use the rule of lcpb200_find_contacts / lcpb200_contact_geometry (this call with no == 0 is
- * exactly those two). Circle-obstacle pairs use the circle-hull rule of physics/contacts.py:84-144 with the exact
- * closest point: centre outside, contact iff |c - q| - r <= eps (q the closest point of the polygon), normal =
- * (c - q) / |c - q|, p1 = q - c, p2 = q - oref, penetration = r - |c - q|; centre inside, the edge of largest
- * separation sep (outward unit normal n): normal = n, p1 = -n sep, p2 = c + p1 - oref, penetration = r - sep.
- * Device pointers:
- *   pos[B,nb,2] rad[B,nb] fric[B,nb] rest[B,nb]   circles (fric / rest: only for the geometry)
- *   verts[B,no,nv,2]                               world-frame vertices of every obstacle (convex, either orientation)
- *   oref[B,no,2] ofric[B,no] orest[B,no]           obstacles' reference points (p2 is relative to it), friction and
- *                                                  restitution (only for the geometry)
- *   body1[B,cap] body2[B,cap] counts[B]            OUT: as lcpb200_find_contacts; body2 >= nb names obstacle
- *                                                  body2 - nb, the one-body contacts of lcpb200_engine_forward
- *   normal[B,cap,2] p1 p2 penetration[B,cap] mu restitution_c[B,cap]
- *                                                  OUT, all NULL (detection only) or all non-NULL: geometry and
- *                                                  material (means of the two bodies') of the selected pairs. */
-int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, double eps, const void* pos,
-                           const void* rad, const void* fric, const void* rest, const void* verts, const void* oref,
-                           const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
-                           void* normal, void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
-                           void* stream);
-
-/* Contact detection and geometry for B scenes of nb circles, np DYNAMIC convex polygons (the reference's Rect / Hull
- * bodies) and no static obstacles. The pairs (i, j), i < j, of the body list [circles 0..nb-1, polygons nb..nb+np-1,
- * obstacles nb+np..nb+np+no-1] (obstacles never pair with each other) are visited in lexicographic order, the contact
- * order of a reference World built from [Circle..., Rect / Hull..., pinned Rect / Hull...]. A pair gives 0, 1 or 2
- * contacts, stored in that order:
- *   circle-circle                 as lcpb200_find_contacts;
- *   circle-polygon / -obstacle    the circle-hull rule of lcpb200_world_contacts; p2 = q - centroid (two-body contact
- *                                 for a polygon, one-body for an obstacle);
+/* Contact detection for B scenes of nb circles, np DYNAMIC convex polygons (the reference's Rect / Hull bodies) and no
+ * static convex polygon obstacles (walls, floors, ramps: no degrees of freedom), replacing the pair loop of
+ * World.find_contacts (physics/world.py:139-142), and, in the same call, the geometry and material of the selected
+ * pairs for callers that do not differentiate through the contact generation. The pairs (i, j), i < j, of the body
+ * list [circles 0..nb-1, polygons nb..nb+np-1, obstacles nb+np..nb+np+no-1] (obstacles never pair with each other) are
+ * visited in lexicographic order, the contact order of a reference World built from [Circle..., Rect / Hull...,
+ * pinned Rect / Hull...]. A pair gives 0, 1 or 2 contacts, stored in that order:
+ *   circle-circle                 the circle-circle test of physics/contacts.py:68-80: a pair is a contact iff
+ *                                 rad_i + rad_j - |pos_i - pos_j| >= -eps; geometry (contacts.py:69-77):
+ *                                 normal = (pos1 - pos2) / dist, penetration = r1 + r2 - dist,
+ *                                 p1 = -normal (r1 - pen / 2), p2 = normal (r2 - pen / 2);
+ *   circle-polygon / -obstacle    the circle-hull rule of physics/contacts.py:84-144 with the exact closest point:
+ *                                 centre outside, contact iff |c - q| - r <= eps (q the closest point of the polygon),
+ *                                 normal = (c - q) / |c - q|, p1 = q - c, p2 = q - oref, penetration = r - |c - q|;
+ *                                 centre inside, the edge of largest separation sep (outward unit normal n):
+ *                                 normal = n, p1 = -n sep, p2 = c + p1 - oref, penetration = r - sep; oref is a
+ *                                 dynamic polygon's centroid (a two-body contact) or an obstacle's reference point (a
+ *                                 one-body contact);
  *   polygon-polygon / -obstacle   the hull-hull rule of physics/contacts.py:145-292: SAT both ways (edge normal
  *                                 left_orthogonal(e) / |e|, support with >=, the last maximal vertex wins; separated iff
  *                                 the largest edge separation is > eps; body2 holds the reference face iff its
@@ -209,46 +170,51 @@ int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, do
  *                                 contacts, in the order of the clipped points. SAT scans start at edge 0 (the reference
  *                                 starts at the edge that won last time): the results differ only on an exact tie
  *                                 between two edge separations.
- * Zero-length edges (a vertex repeated to pad a polygon to nv) are skipped everywhere.
+ * Zero-length edges (a vertex repeated to pad a polygon to nv) are skipped everywhere. mu / restitution of a contact
+ * are the mean of the two bodies' (world.py:144-151, :213-224).
  * Device pointers (NULL allowed for an empty group):
  *   pos[B,nb,2] rad[B,nb] fric[B,nb] rest[B,nb]       circles (fric / rest: only for the geometry)
  *   pverts[B,np,nv,2] pcen[B,np,2] pfric[B,np] prest[B,np]
  *                                                     polygons: world-frame vertices (positive shoelace area),
  *                                                     centroids, friction and restitution
  *   overts[B,no,nv,2] oref[B,no,2] ofric[B,no] orest[B,no]
- *                                                     obstacles, as lcpb200_world_contacts (either orientation)
- *   body1[B,cap] body2[B,cap] counts[B]               OUT: as lcpb200_world_contacts; body2 >= nb + np names obstacle
- *                                                     body2 - nb - np (a one-body contact)
+ *                                                     obstacles: world-frame vertices (convex, either orientation),
+ *                                                     reference points (p2 is relative to it), friction and
+ *                                                     restitution (ofric / orest: only for the geometry)
+ *   body1[B,cap] body2[B,cap] int32                   OUT: the contacts' pairs in the order above (the order the
+ *                                                     reference appends contacts in), padded with the pair (0, 1);
+ *                                                     body2 >= nb + np names obstacle body2 - nb - np, the one-body
+ *                                                     contacts of lcpb200_engine_forward
+ *   counts[B] int32                                   OUT: number of contacts (may exceed cap: then the lists hold the
+ *                                                     first cap contacts and the caller must grow cap)
  *   feat[B,cap] int32                                 OUT: per hull-hull contact its discrete features (bits 0-1 the
  *                                                     point: incident endpoint 0 / 1, cut by the first / second clip
  *                                                     plane; bits 2-3 the first clip's outcome; bit 4 body2 holds the
  *                                                     reference face; bits 5-12 reference edge; bits 13-20 incident
- *                                                     edge), from which the geometry is rebuilt; -1 for other contacts
- *   normal p1 p2 penetration mu restitution_c         OUT, all NULL or all non-NULL: as lcpb200_world_contacts
- * 3 <= nv <= 256 when np + no > 0. With np == 0 the pairs, their order and the geometry are those of
- * lcpb200_world_contacts. */
-int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
-                          const void* rad, const void* fric, const void* rest, const void* pverts, const void* pcen,
-                          const void* pfric, const void* prest, const void* overts, const void* oref,
-                          const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
-                          int32_t* feat, void* normal, void* p1, void* p2, void* penetration, void* mu,
-                          void* restitution_c, void* stream);
-
-/* lcpb200_body_contacts with pairs excluded from contact (the reference's Body.add_no_contact: contacts.py:60 returns
- * before any rule when `geom1 in geom2.no_contact`). The arguments are those of lcpb200_body_contacts, plus
- *   no_contact   const uint32_t[ceil(nt * nt / 32)], shared by the batch (device): bit i * nt + j (bit k is bit
- *                k % 32 of word k / 32), i < j, nt = nb + np + no, set iff the pair (i, j) of the body list never
- *                makes contact. Only bits with i < j are read; a pair of two obstacles is never visited anyway.
- * An excluded pair gives no contact and no rule is evaluated for it: the contacts, their order, feat and the geometry
- * are those of lcpb200_body_contacts with the excluded pairs' contacts removed. Covers every world kind (np == 0 and /
- * or no == 0 included). */
-int lcpb200_body_contacts_masked(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
-                                 const void* pos, const void* rad, const void* fric, const void* rest,
-                                 const void* pverts, const void* pcen, const void* pfric, const void* prest,
-                                 const void* overts, const void* oref, const void* ofric, const void* orest,
-                                 int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
-                                 void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
-                                 const uint32_t* no_contact, void* stream);
+ *                                                     edge), from which the geometry is rebuilt; -1 for other
+ *                                                     contacts. Required when np > 0 or no_contact != NULL, NULL
+ *                                                     allowed otherwise
+ *   normal[B,cap,2] p1 p2[B,cap,2] penetration mu restitution_c[B,cap]
+ *                                                     OUT, all NULL (detection only) or all non-NULL: geometry and
+ *                                                     material of the selected pairs (penetration -1e30 in unused
+ *                                                     slots)
+ *   no_contact                                        NULL, or const uint32_t[ceil(nt * nt / 32)], shared by the batch:
+ *                                                     bit i * nt + j (bit k is bit k % 32 of word k / 32), i < j,
+ *                                                     nt = nb + np + no, set iff the pair (i, j) of the body list
+ *                                                     never makes contact (the reference's Body.add_no_contact:
+ *                                                     contacts.py:60 returns before any rule when
+ *                                                     `geom1 in geom2.no_contact`). Only bits with i < j are read; a
+ *                                                     pair of two obstacles is never visited anyway. An excluded pair
+ *                                                     gives no contact and no rule is evaluated for it.
+ * 3 <= nv <= 256 when np + no > 0; oref is required when no > 0. The walk follows the arguments: with no_contact, the
+ * polygon walk reading the mask; else with feat, the polygon walk; else (np == 0) the circle walk, at most one contact
+ * per pair. With np == 0 the pairs, their order and the geometry do not depend on which walk runs. */
+int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
+                     const void* rad, const void* fric, const void* rest, const void* pverts, const void* pcen,
+                     const void* pfric, const void* prest, const void* overts, const void* oref, const void* ofric,
+                     const void* orest, int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
+                     void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
+                     const uint32_t* no_contact, void* stream);
 
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
@@ -297,7 +263,7 @@ int lcpb200_assemble_backward(int dtype, int B, int nb, int nc, double dt,
  * border beyond the limits above) gets status -100 and no result: assemble it with lcpb200_assemble and call
  * lcpb200_forward.
  * Static obstacles: body2[c] >= nb names a body without degrees of freedom (a wall, floor or ramp: the static
- * polygons of lcpb200_world_contacts). Contact c is then a ONE-BODY contact: its rows of G touch body1's three
+ * obstacles of lcpb200_contacts). Contact c is then a ONE-BODY contact: its rows of G touch body1's three
  * columns only, exactly the reference's formulation with the obstacle pinned by a TotalConstraint, reduced by the
  * pinned dofs. p2 is not used by such a contact and its dp2 gradient is zero. body1 must be < nb; body1 == body2, a
  * negative index or a body1 >= nb gets status -100.

@@ -38,11 +38,7 @@ _SIGS = {
                                 [ctypes.c_uint, _vp]),
     "lcpb200_engine_backward_batched": (ctypes.c_int, [_vp] + [ctypes.c_int] * 5 + [ctypes.c_double] + [_vp] * 29 +
                                         [ctypes.c_uint, _vp]),
-    "lcpb200_find_contacts": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 6),
-    "lcpb200_contact_geometry": (ctypes.c_int, [ctypes.c_int] * 4 + [_vp] * 14),
-    "lcpb200_world_contacts": (ctypes.c_int, [ctypes.c_int] * 6 + [ctypes.c_double] + [_vp] * 18),
-    "lcpb200_body_contacts": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 23),
-    "lcpb200_body_contacts_masked": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 24),
+    "lcpb200_contacts": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 24),
     "lcpb200_assemble": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 17),
     "lcpb200_assemble_backward": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 25),
 }

@@ -19,9 +19,9 @@
 //   * polygon-polygon and polygon-obstacle pairs use the hull-hull rule of contacts.py:145-292 (SAT both ways,
 //     reference-face clipping): 0, 1 or 2 contacts per pair, stored in the order of the clipped points;
 //   * obstacles never pair with each other.
-// The walk is templated on HULLS: HULLS == false is the walk of lcpb200_find_contacts (no == 0) and
-// lcpb200_world_contacts (circles and obstacles, np == 0), one contact per pair at most. MASK == true
-// (lcpb200_body_contacts_masked) reads a pair-exclusion bitmask shared by the batch and skips an excluded pair before
+// The walk is templated on HULLS: HULLS == false is the walk of lcpb200_contacts without feat (circles and
+// obstacles, np == 0), one contact per pair at most. MASK == true (lcpb200_contacts with no_contact) reads a
+// pair-exclusion bitmask shared by the batch and skips an excluded pair before
 // any rule is evaluated, as the reference's `if geom1 in geom2.no_contact: return` (contacts.py:60, add_no_contact).
 #pragma once
 #include <cuda_runtime.h>

@@ -924,179 +924,68 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
                                          dv, dfext, dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, stream);
 }
 
-// ------------------------------------------------------------------ assembly
+// ------------------------------------------------------------------ contact detection
+// One body of lcpb200_contacts per dtype. The instantiation is chosen here and only here: the mask walk when the
+// caller passes no_contact, the polygon walk (HULLS) when it passes feat, the circle walk otherwise; the geometry
+// kernel follows the walk's HULLS.
 template <typename T>
-static cts::Bodies<T> bodies(int nb, int np, int no, int nv, const void* pos, const void* rad, const void* fric,
-                             const void* rest, const void* pverts, const void* pcen, const void* pfric,
-                             const void* prest, const void* overts, const void* oref, const void* ofric,
-                             const void* orest) {
+static void contacts_t(int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos, const void* rad,
+                       const void* fric, const void* rest, const void* pverts, const void* pcen, const void* pfric,
+                       const void* prest, const void* overts, const void* oref, const void* ofric, const void* orest,
+                       int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2,
+                       void* pen, void* mu, void* rest_c, const uint32_t* no_contact, int sms, cudaStream_t st) {
   cts::Bodies<T> bd;
   bd.nb = nb; bd.np = np; bd.no = no; bd.nv = nv;
   bd.pos = (const T*)pos; bd.rad = (const T*)rad; bd.fric = (const T*)fric; bd.rest = (const T*)rest;
   bd.pverts = (const T*)pverts; bd.pcen = (const T*)pcen; bd.pfric = (const T*)pfric; bd.prest = (const T*)prest;
   bd.overts = (const T*)overts; bd.oref = (const T*)oref; bd.ofric = (const T*)ofric; bd.orest = (const T*)orest;
-  return bd;
-}
-
-extern "C" int lcpb200_find_contacts(int dtype, int B, int nb, int cap, double eps, const void* pos, const void* rad,
-                                     int32_t* body1, int32_t* body2, int32_t* counts, void* stream) {
-  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
-  if (B < 0 || nb <= 0 || cap <= 0) return fail("find_contacts: need B >= 0, nb > 0, cap > 0");
-  if (!pos || !rad || !body1 || !body2 || !counts) return fail("find_contacts: NULL argument");
-  if (B == 0) return 0;
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32)
-    cts::launch_find_contacts<float, false>(
-        bodies<float>(nb, 0, 0, 0, pos, rad, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, (float)eps, body1, body2, nullptr,
-        counts, sms, st);
+  if (no_contact)
+    cts::launch_find_contacts<T, true, true>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st, no_contact);
+  else if (feat)
+    cts::launch_find_contacts<T, true, false>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st);
   else
-    cts::launch_find_contacts<double, false>(
-        bodies<double>(nb, 0, 0, 0, pos, rad, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, eps, body1, body2, nullptr, counts,
-        sms, st);
-  CK(cudaGetLastError());
-  return 0;
-}
-
-extern "C" int lcpb200_contact_geometry(int dtype, int B, int nb, int cap, const void* pos, const void* rad,
-                                        const void* fric, const void* rest, const int32_t* body1, const int32_t* body2,
-                                        const int32_t* counts, void* normal, void* p1, void* p2, void* pen, void* mu,
-                                        void* rest_c, void* stream) {
-  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
-  if (B < 0 || nb <= 0 || cap <= 0) return fail("contact_geometry: need B >= 0, nb > 0, cap > 0");
-  if (!pos || !rad || !fric || !rest || !body1 || !body2 || !counts || !normal || !p1 || !p2 || !pen || !mu || !rest_c)
-    return fail("contact_geometry: NULL argument");
-  if (B == 0) return 0;
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32)
-    cts::launch_contact_geometry<float, false>(bodies<float>(nb, 0, 0, 0, pos, rad, fric, rest, 0, 0, 0, 0, 0, 0, 0, 0),
-                                               B, cap, body1, body2, nullptr, counts, (float*)normal, (float*)p1,
-                                               (float*)p2, (float*)pen, (float*)mu, (float*)rest_c, sms, st);
+    cts::launch_find_contacts<T, false, false>(bd, B, cap, (T)eps, body1, body2, nullptr, counts, sms, st);
+  if (!normal) return;
+  if (feat)
+    cts::launch_contact_geometry<T, true>(bd, B, cap, body1, body2, feat, counts, (T*)normal, (T*)p1, (T*)p2,
+                                          (T*)pen, (T*)mu, (T*)rest_c, sms, st);
   else
-    cts::launch_contact_geometry<double, false>(
-        bodies<double>(nb, 0, 0, 0, pos, rad, fric, rest, 0, 0, 0, 0, 0, 0, 0, 0), B, cap, body1, body2, nullptr,
-        counts, (double*)normal, (double*)p1, (double*)p2, (double*)pen, (double*)mu, (double*)rest_c, sms, st);
-  CK(cudaGetLastError());
-  return 0;
+    cts::launch_contact_geometry<T, false>(bd, B, cap, body1, body2, nullptr, counts, (T*)normal, (T*)p1, (T*)p2,
+                                           (T*)pen, (T*)mu, (T*)rest_c, sms, st);
 }
 
-template <typename T, bool HULLS, bool MASK = false>
-static void body_contacts_t(const cts::Bodies<T>& bd, int B, int cap, double eps, int32_t* body1, int32_t* body2,
-                            int32_t* feat, int32_t* counts, void* normal, void* p1, void* p2, void* pen, void* mu,
-                            void* rest_c, bool geometry, int sms, cudaStream_t st,
-                            const uint32_t* no_contact = nullptr) {
-  cts::launch_find_contacts<T, HULLS, MASK>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st, no_contact);
-  if (geometry)
-    cts::launch_contact_geometry<T, HULLS>(bd, B, cap, body1, body2, feat, counts, (T*)normal, (T*)p1, (T*)p2, (T*)pen,
-                                           (T*)mu, (T*)rest_c, sms, st);
-}
-
-extern "C" int lcpb200_world_contacts(int dtype, int B, int nb, int no, int nv, int cap, double eps, const void* pos,
-                                      const void* rad, const void* fric, const void* rest, const void* verts,
-                                      const void* oref, const void* ofric, const void* orest, int32_t* body1,
-                                      int32_t* body2, int32_t* counts, void* normal, void* p1, void* p2, void* pen,
-                                      void* mu, void* rest_c, void* stream) {
-  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
-  if (B < 0 || nb <= 0 || no < 0 || cap <= 0) return fail("world_contacts: need B >= 0, nb > 0, no >= 0, cap > 0");
-  if (no > 0 && nv < 3) return fail("world_contacts: obstacles need nv >= 3 vertices");
-  if ((long long)nb + no > 0x7fffffffLL) return fail("world_contacts: too many bodies");
-  if (!pos || !rad || !body1 || !body2 || !counts) return fail("world_contacts: NULL argument");
-  if (no > 0 && !verts) return fail("world_contacts: obstacles need verts");
-  const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
-                   (rest_c != nullptr);
-  if (ngeo != 0 && ngeo != 6) return fail("world_contacts: the geometry outputs are all NULL or all non-NULL");
-  const bool geometry = ngeo == 6;
-  if (geometry && (!fric || !rest || (no > 0 && (!oref || !ofric || !orest))))
-    return fail("world_contacts: the geometry needs fric, rest and, with obstacles, oref, ofric, orest");
-  if (B == 0) return 0;
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32)
-    body_contacts_t<float, false>(bodies<float>(nb, 0, no, nv, pos, rad, fric, rest, 0, 0, 0, 0, verts, oref, ofric,
-                                                orest),
-                                  B, cap, eps, body1, body2, nullptr, counts, normal, p1, p2, pen, mu, rest_c, geometry,
-                                  sms, st);
-  else
-    body_contacts_t<double, false>(bodies<double>(nb, 0, no, nv, pos, rad, fric, rest, 0, 0, 0, 0, verts, oref, ofric,
-                                                  orest),
-                                   B, cap, eps, body1, body2, nullptr, counts, normal, p1, p2, pen, mu, rest_c,
-                                   geometry, sms, st);
-  CK(cudaGetLastError());
-  return 0;
-}
-
-// lcpb200_body_contacts and lcpb200_body_contacts_masked: one argument check, the walk with or without the mask
-template <bool MASK>
-static int body_contacts_impl(const char* name, int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
-                              const void* pos, const void* rad, const void* fric, const void* rest, const void* pverts,
-                              const void* pcen, const void* pfric, const void* prest, const void* overts,
-                              const void* oref, const void* ofric, const void* orest, int32_t* body1, int32_t* body2,
-                              int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2, void* pen, void* mu,
-                              void* rest_c, const uint32_t* no_contact, void* stream) {
-  const std::string nm(name);
+extern "C" int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
+                                const void* rad, const void* fric, const void* rest, const void* pverts,
+                                const void* pcen, const void* pfric, const void* prest, const void* overts,
+                                const void* oref, const void* ofric, const void* orest, int32_t* body1,
+                                int32_t* body2, int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2,
+                                void* pen, void* mu, void* rest_c, const uint32_t* no_contact, void* stream) {
   if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
   if (B < 0 || nb < 0 || np < 0 || no < 0 || cap <= 0 || nb + np <= 0)
-    return fail(nm + ": need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
-  if (np + no > 0 && (nv < 3 || nv > cts::MAX_NV)) return fail(nm + ": polygons need 3 <= nv <= 256 vertices");
-  if ((long long)nb + np + no > 0x7fffffffLL) return fail(nm + ": too many bodies");
+    return fail("contacts: need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
+  if (np + no > 0 && (nv < 3 || nv > cts::MAX_NV)) return fail("contacts: polygons need 3 <= nv <= 256 vertices");
+  if ((long long)nb + np + no > 0x7fffffffLL) return fail("contacts: too many bodies");
   if ((nb > 0 && (!pos || !rad)) || (np > 0 && (!pverts || !pcen)) || (no > 0 && (!overts || !oref)) || !body1 ||
-      !body2 || !counts || !feat || (MASK && !no_contact))
-    return fail(nm + ": NULL argument");
+      !body2 || !counts)
+    return fail("contacts: NULL argument");
+  if ((np > 0 || no_contact) && !feat) return fail("contacts: polygons and no_contact need feat");
   const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
                    (rest_c != nullptr);
-  if (ngeo != 0 && ngeo != 6) return fail(nm + ": the geometry outputs are all NULL or all non-NULL");
-  const bool geometry = ngeo == 6;
-  if (geometry && ((nb > 0 && (!fric || !rest)) || (np > 0 && (!pfric || !prest)) || (no > 0 && (!ofric || !orest))))
-    return fail(nm + ": the geometry needs the friction and restitution of every body group");
+  if (ngeo != 0 && ngeo != 6) return fail("contacts: the geometry outputs are all NULL or all non-NULL");
+  if (ngeo == 6 && ((nb > 0 && (!fric || !rest)) || (np > 0 && (!pfric || !prest)) || (no > 0 && (!ofric || !orest))))
+    return fail("contacts: the geometry needs the friction and restitution of every body group");
   if (B == 0) return 0;
   int dev = 0, sms = 0;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32)
-    body_contacts_t<float, true, MASK>(bodies<float>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric, prest,
-                                                     overts, oref, ofric, orest),
-                                       B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c,
-                                       geometry, sms, st, no_contact);
-  else
-    body_contacts_t<double, true, MASK>(bodies<double>(nb, np, no, nv, pos, rad, fric, rest, pverts, pcen, pfric,
-                                                       prest, overts, oref, ofric, orest),
-                                        B, cap, eps, body1, body2, feat, counts, normal, p1, p2, pen, mu, rest_c,
-                                        geometry, sms, st, no_contact);
+  (dtype == LCPB200_F32 ? contacts_t<float> : contacts_t<double>)(
+      B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest, overts, oref, ofric, orest, body1,
+      body2, counts, feat, normal, p1, p2, pen, mu, rest_c, no_contact, sms, (cudaStream_t)stream);
   CK(cudaGetLastError());
   return 0;
 }
 
-extern "C" int lcpb200_body_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
-                                     const void* pos, const void* rad, const void* fric, const void* rest,
-                                     const void* pverts, const void* pcen, const void* pfric, const void* prest,
-                                     const void* overts, const void* oref, const void* ofric, const void* orest,
-                                     int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
-                                     void* p1, void* p2, void* pen, void* mu, void* rest_c, void* stream) {
-  return body_contacts_impl<false>("body_contacts", dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts,
-                                   pcen, pfric, prest, overts, oref, ofric, orest, body1, body2, counts, feat, normal,
-                                   p1, p2, pen, mu, rest_c, nullptr, stream);
-}
-
-extern "C" int lcpb200_body_contacts_masked(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
-                                            const void* pos, const void* rad, const void* fric, const void* rest,
-                                            const void* pverts, const void* pcen, const void* pfric, const void* prest,
-                                            const void* overts, const void* oref, const void* ofric, const void* orest,
-                                            int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat,
-                                            void* normal, void* p1, void* p2, void* pen, void* mu, void* rest_c,
-                                            const uint32_t* no_contact, void* stream) {
-  return body_contacts_impl<true>("body_contacts_masked", dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest,
-                                  pverts, pcen, pfric, prest, overts, oref, ofric, orest, body1, body2, counts, feat,
-                                  normal, p1, p2, pen, mu, rest_c, no_contact, stream);
-}
-
+// ------------------------------------------------------------------ assembly
 extern "C" int lcpb200_assemble(int dtype, int B, int nb, int nc, double dt, const void* mass, const void* inertia,
                                 const void* v, const void* fext, const void* normal, const void* p1,
                                 const void* p2, const int32_t* body1, const int32_t* body2, const void* mu,

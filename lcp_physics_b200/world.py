@@ -12,7 +12,7 @@ Here the state of B scenes lives in structure-of-arrays tensors on the GPU and o
 
 with contact generation for circle pairs (contacts.py:68-80: normal = (pos1 - pos2)/dist, penetration =
 r1 + r2 - dist, contact when penetration >= -eps, p1 = -n (r1 - pen/2), p2 = n (r2 - pen/2)) on the device:
-the pair test and the ordered compaction of all nb (nb - 1) / 2 pairs by lcpb200_find_contacts
+the pair test and the ordered compaction of all nb (nb - 1) / 2 pairs by lcpb200_contacts
 (csrc/lcp_contacts.cuh), pair order (i < j, lexicographic) as the reference's broadphase callback visits
 them, the geometry of the selected pairs by torch ops (differentiable). Every scene keeps its OWN contact count: the fused kernels take a per-scene count, and a scene
 without contacts gets the equality-constrained solve of engines.py:35-49 inside the same kernel.
@@ -25,10 +25,10 @@ and STATIC convex polygon obstacles -- the reference's `Rect` / `Hull` floors, w
 eliminated exactly and a contact against it is a one-body contact (body2 >= nb, include/lcpb200.h) whose rows touch
 only the circle's three columns (DESIGN.md section 9), and DYNAMIC convex polygons -- the reference's `Rect` / `Hull`
 bodies (`polygons=`), ordered after the circles and before the obstacles, with the hull-hull contact rule of
-contacts.py:145-292 (SAT + reference-face clipping, 0-2 contacts per pair) detected by lcpb200_body_contacts, and
+contacts.py:145-292 (SAT + reference-face clipping, 0-2 contacts per pair) detected by lcpb200_contacts, and
 CONSTRAINTS between bodies (`constraints=`: `Joint`, `FixedJoint`, `XConstraint`, `YConstraint`, `RotConstraint`,
 constraints.py:13-173) as equality rows of the engine's LCP, rebuilt with torch ops at every engine call, pairs excluded
-from contact (`no_contact=`, Body.add_no_contact: skipped in the GPU pair walk, lcpb200_body_contacts_masked) and
+from contact (`no_contact=`, Body.add_no_contact: skipped in the GPU pair walk of lcpb200_contacts) and
 time-dependent external forces (`external_force=`, forces.py ExternalForce). The renderer is not mirrored.
 Everything is differentiable through torch autograd (the LCP through lcpb200_engine_backward). Scenes of up to
 42 dynamic bodies (3 (nb + npoly) + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes
@@ -440,7 +440,7 @@ class BatchedWorld:
             st[1:] = [rot1, pos1, self.p[:, c.i, 1:] + pos1]
 
     def _init_no_contact(self, pairs, nt):
-        """Pair-exclusion bitmask of lcpb200_body_contacts_masked: bit i * nt + j (i < j) per excluded pair."""
+        """Pair-exclusion bitmask (no_contact of lcpb200_contacts): bit i * nt + j (i < j) per excluded pair."""
         words = [0] * ((nt * nt + 31) // 32)
         ex = torch.zeros(nt, nt, dtype=torch.bool)
         for pr in pairs:
@@ -457,102 +457,58 @@ class BatchedWorld:
         self.nc_mask = torch.tensor(words, dtype=torch.int32, device=self.device)
         self.nc_pair_excluded = ex.to(self.device)[self.pi, self.pj]              # per pair of self.pi / self.pj
 
-    # ------------------------------------------------------------------ contacts.py:68-80, batched
+    # ------------------------------------------------------------------ contacts.py:60-292, batched
     def find_contacts(self):
-        """Pair test + ordered compaction on the GPU (lcpb200_find_contacts: all nb (nb - 1) / 2 pairs of every
-        scene, lexicographic order = the reference's contact order), then the contact geometry of the selected
-        pairs with torch ops (differentiable w.r.t. the positions)."""
-        if self.np or self.nc_mask is not None:
-            return self._find_contacts_bodies()
-        if self.no:
-            return self._find_contacts_obstacles()
+        """Pair walk + ordered compaction on the GPU (lcpb200_contacts: the pairs of the body list [circles...,
+        polygons..., obstacles...] of every scene in lexicographic order = the reference's contact order;
+        circle-circle, circle-polygon and hull-hull rules, 0-2 contacts per pair; the `no_contact` pairs skipped),
+        then the contact geometry of the selected pairs: from the same call when nothing needs autograd, else from
+        torch ops (_geometry_torch, which rebuilds hull-hull contacts from the kernel's features), differentiable
+        w.r.t. positions, radii, materials and the polygon / obstacle vertices."""
         lib = _lib.load()
-        B, cap, dev = self.B, self.cap, self.device
-        pos = self.p[:, :, 1:]
-
-        def walk(pos_c, rad):
-            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            counts = torch.empty(B, dtype=torch.int32, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_find_contacts(_lib.dtype_code(self.dtype), B, self.nb, cap, self.eps,
-                                                     _lib.ptr(pos_c), _lib.ptr(rad), _lib.ptr(b1), _lib.ptr(b2),
-                                                     _lib.ptr(counts),
-                                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-            return b1, b2, counts
-        pos_c = pos.detach().contiguous()
-        b1, b2, counts = _detect(walk, pos_c, self.rad)
-        if int(counts.max()) > cap:
-            raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
-        self.c_b1, self.c_b2, self.counts = b1, b2, counts
-        needs_graph = torch.is_grad_enabled() and any(t.requires_grad for t in (self.p, self.rad, self.fric_coeff, self.restitution))
-        if not needs_graph:
-            # nothing to differentiate: the geometry of the selected pairs in one kernel as well
-            def geometry(pos_c, rad, fric, rest, b1, b2, counts):
-                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-                geo = (new(2), new(2), new(2), new(), new(), new())
-                with torch.cuda.device(dev):
-                    _lib.check(lib.lcpb200_contact_geometry(
-                        _lib.dtype_code(self.dtype), B, self.nb, cap, _lib.ptr(pos_c), _lib.ptr(rad), _lib.ptr(fric),
-                        _lib.ptr(rest), _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
-                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-                return geo
-            d = lambda t: t.detach().contiguous()
-            (self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu,
-             self.c_rest) = _detect(geometry, pos_c, d(self.rad), d(self.fric_coeff), d(self.restitution), b1, b2,
-                                    counts)
-            return
-        i1, i2 = b1.long(), b2.long()
-        take = lambda t, idx: torch.gather(t, 1, idx)
-        d = torch.gather(pos, 1, i1.unsqueeze(2).expand(-1, -1, 2)) - torch.gather(pos, 1, i2.unsqueeze(2).expand(-1, -1, 2))
-        dist = d.norm(dim=2)                                                       # b1.pos - b2.pos   contacts.py:69-71
-        r1, r2 = take(self.rad, i1), take(self.rad, i2)
-        pen_c = r1 + r2 - dist
-        normal = d / dist.unsqueeze(2)
-        valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
-        self.c_normal = normal
-        self.c_p1 = -normal * (r1 - pen_c / 2).unsqueeze(2)                        # contacts.py:75-77
-        self.c_p2 = normal * (r2 - pen_c / 2).unsqueeze(2)
-        self.c_pen = torch.where(valid, pen_c, pen_c.new_full((), -1e30))
-        self.c_b1, self.c_b2 = b1, b2
-        self.c_mu = 0.5 * (take(self.fric_coeff, i1) + take(self.fric_coeff, i2))              # world.py:213-224
-        self.c_rest = 0.5 * (take(self.restitution, i1) + take(self.restitution, i2))          # world.py:144-151
-        self.counts = counts
-
-    def _find_contacts_obstacles(self):
-        """find_contacts for worlds with static obstacles: lcpb200_world_contacts walks circle-circle and
-        circle-obstacle pairs in the order of a reference World with bodies [circles..., obstacles...]; the geometry
-        comes from the same call, or from torch ops (_geometry_torch) when something needs autograd."""
-        lib = _lib.load()
-        B, cap, dev = self.B, self.cap, self.device
+        B, cap, dev, nb = self.B, self.cap, self.device, self.nb
+        pverts = self.polygon_vertices() if self.np else None
+        poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
+        obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
         needs_graph = torch.is_grad_enabled() and any(
-            t.requires_grad for t in (self.p, self.rad, self.fric_coeff, self.restitution, self.ov, self.ofric, self.orest))
-        d = lambda t: t.detach().contiguous()
+            t is not None and t.requires_grad
+            for t in (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
+        # feat selects the polygon walk, which worlds with polygons or no_contact pairs need; the others keep the
+        # circle walk
+        with_feat = self.np > 0 or self.nc_mask is not None
+        d = lambda t: t.detach().contiguous() if t is not None else None
 
         def walk(*ins):
-            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            counts = torch.empty(B, dtype=torch.int32, device=dev)
-            geo = [None] * 6
-            if not needs_graph:
-                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-                geo = [new(2), new(2), new(2), new(), new(), new()]
+            i32 = lambda *s_: torch.empty(*s_, dtype=torch.int32, device=dev)
+            b1, b2, counts = i32(B, cap), i32(B, cap), i32(B)
+            feat = i32(B, cap) if with_feat else None
+            new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
+            geo = [None] * 6 if needs_graph else [new(2), new(2), new(2), new(), new(), new()]
             with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_world_contacts(
-                    _lib.dtype_code(self.dtype), B, self.nb, self.no, self.nv, cap, self.eps,
-                    *[_lib.ptr(t) for t in ins], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), *[_lib.ptr(t) for t in geo],
+                _lib.check(lib.lcpb200_contacts(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps,
+                    *[_lib.ptr(t) for t in ins[:-1]], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat),
+                    *[_lib.ptr(t) for t in geo], _lib.ptr(ins[-1]),
                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-            return (b1, b2, counts) + (() if needs_graph else tuple(geo))
-        out = _detect(walk, *[d(t) for t in (self.p[:, :, 1:], self.rad, self.fric_coeff, self.restitution,
-                                                     self.ov, self.oref, self.ofric, self.orest)])
-        b1, b2, counts, geo = out[0], out[1], out[2], out[3:]
+            # tensors only: _DetectFn marks every output non-differentiable
+            return tuple(t for t in (b1, b2, counts, feat, *geo) if t is not None)
+        # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the
+        # kernel runs)
+        pcen = self.p[:, nb:, 1:] if self.np else None
+        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
+               + obst]
+        out = _detect(walk, *ins, self.nc_mask)
+        b1, b2, counts = out[:3]
+        feat = out[3] if with_feat else None
         if int(counts.max()) > cap:
             raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
         self.c_b1, self.c_b2, self.counts = b1, b2, counts
+        if with_feat:
+            self.c_feat = feat
         if not needs_graph:
-            self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest = geo
+            self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest = out[3 + with_feat:]
             return
-        self.c_normal, self.c_p1, self.c_p2, pen, self.c_mu, self.c_rest = self._geometry_torch(b1, b2)
+        self.c_normal, self.c_p1, self.c_p2, pen, self.c_mu, self.c_rest = self._geometry_torch(b1, b2, feat, pverts)
         valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
         self.c_pen = torch.where(valid, pen, pen.new_full((), -1e30))
 
@@ -563,57 +519,6 @@ class BatchedWorld:
         c, s = torch.cos(q[:, :, 0:1]), torch.sin(q[:, :, 0:1])
         lx, ly = self.plocal[..., 0], self.plocal[..., 1]
         return torch.stack([q[:, :, 1:2] + (c * lx - s * ly), q[:, :, 2:3] + (s * lx + c * ly)], 3)
-
-    def _find_contacts_bodies(self):
-        """find_contacts for worlds with dynamic polygons: lcpb200_body_contacts walks the pairs of the body list
-        [circles..., polygons..., obstacles...] (circle-circle, circle-polygon and hull-hull rules; 0-2 contacts per
-        pair) and returns each hull-hull contact's features; the geometry comes from the same call, or from torch ops
-        that rebuild it from those features (_geometry_torch) when something needs autograd."""
-        lib = _lib.load()
-        B, cap, dev, nb = self.B, self.cap, self.device, self.nb
-        pverts = self.polygon_vertices() if self.np else None
-        pcen = self.p[:, nb:, 1:] if self.np else None
-        poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
-        obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
-        needs_graph = torch.is_grad_enabled() and any(
-            t is not None and t.requires_grad
-            for t in (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
-        d = lambda t: t.detach().contiguous() if t is not None else None
-        # worlds with no_contact pairs: the same walk reading the pair-exclusion mask (every world kind)
-        masked = self.nc_mask is not None
-        fn = lib.lcpb200_body_contacts_masked if masked else lib.lcpb200_body_contacts
-
-        def walk(*ins):
-            b1 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            b2 = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            feat = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            counts = torch.empty(B, dtype=torch.int32, device=dev)
-            geo = [None] * 6
-            if not needs_graph:
-                new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
-                geo = [new(2), new(2), new(2), new(), new(), new()]
-            with torch.cuda.device(dev):
-                _lib.check(fn(
-                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps,
-                    *[_lib.ptr(t) for t in ins[:-1]], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat),
-                    *[_lib.ptr(t) for t in geo], *((_lib.ptr(ins[-1]),) if masked else ()),
-                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-            return (b1, b2, feat, counts) + (() if needs_graph else tuple(geo))
-        # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the
-        # kernel runs)
-        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
-               + obst]
-        out = _detect(walk, *ins, self.nc_mask)
-        b1, b2, feat, counts, geo = out[0], out[1], out[2], out[3], out[4:]
-        if int(counts.max()) > cap:
-            raise RuntimeError("BatchedWorld: a scene has %d contacts, capacity %d" % (int(counts.max()), cap))
-        self.c_b1, self.c_b2, self.c_feat, self.counts = b1, b2, feat, counts
-        if not needs_graph:
-            self.c_normal, self.c_p1, self.c_p2, self.c_pen, self.c_mu, self.c_rest = geo
-            return
-        self.c_normal, self.c_p1, self.c_p2, pen, self.c_mu, self.c_rest = self._geometry_torch(b1, b2, feat, pverts)
-        valid = torch.arange(cap, device=dev).unsqueeze(0) < counts.unsqueeze(1)
-        self.c_pen = torch.where(valid, pen, pen.new_full((), -1e30))
 
     def _hull_torch(self, i1, i2, feat, verts, ref):
         """Torch mirror of the hull-hull geometry of csrc/lcp_contacts.cuh (contacts.py:156-201, clip_segment_to_line
@@ -691,7 +596,7 @@ class BatchedWorld:
 
     def _geometry_torch(self, b1, b2, feat=None, pverts=None):
         """Differentiable geometry and material of the selected pairs (circle-circle: contacts.py:69-77;
-        circle-polygon: contacts.py:84-144, as lcpb200_world_contacts; hull-hull: _hull_torch, from the kernel's
+        circle-polygon: contacts.py:84-144, as lcpb200_contacts; hull-hull: _hull_torch, from the kernel's
         features feat), gradients reaching positions, radii, materials and the polygon / obstacle vertices.
         pverts: the dynamic polygons' world-frame vertices (worlds with polygons)."""
         nb = self.nb
@@ -760,8 +665,8 @@ class BatchedWorld:
 
     def find_contacts_torch(self):
         """The same contact list with torch ops only (O(nb^2) tensors, a stable sort for the compaction): the
-        independent implementation tests/test_gpu_world.py checks lcpb200_find_contacts against (and
-        tests/test_gpu_obstacles.py lcpb200_world_contacts). Returns (counts, b1, b2). Not available for worlds with
+        independent implementation tests/test_gpu_world.py and tests/test_gpu_obstacles.py check lcpb200_contacts'
+        circle walk against. Returns (counts, b1, b2). Not available for worlds with
         dynamic polygons: their hull-hull rule is checked against the CPU oracle (oracle/polygon_oracle.py)."""
         if self.np:
             raise NotImplementedError("find_contacts_torch: worlds with dynamic polygons (see oracle/polygon_oracle.py)")

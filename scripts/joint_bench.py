@@ -2,8 +2,8 @@
   1. 1024 chain_demo worlds (10 Rect links: XConstraint + YConstraint on the top link, 9 Joints, no_contact between
      neighbours, Gravity on links 1-9, a projectile circle under a horizontal impulse for t < 0.1, post-stabilisation),
      in fp64 and in fp32;
-  2. the contact walk with geometry of those worlds: lcpb200_body_contacts_masked (the 9 neighbour pairs excluded)
-     against lcpb200_body_contacts (no pair excluded) on the same bodies.
+  2. the contact walk with geometry of those worlds: lcpb200_contacts with no_contact (the 9 neighbour pairs
+     excluded) against lcpb200_contacts without it (no pair excluded) on the same bodies.
 Legs of a pairing alternate inside every round; prints one JSON line per pairing with the median and the spread
 (min, max) of every leg, plus the card and its power limit.
 
@@ -53,10 +53,7 @@ def walk_time(w, masked, reps=50):
     ins = [t.contiguous() for t in (w.p[:, :w.nb, 1:], w.rad, w.fric_coeff, w.restitution, pv, pcen, w.pfric, w.prest)]
     args = [_lib.dtype_code(w.dtype), B, w.nb, w.np, w.no, w.nv, cap, w.eps, *[_lib.ptr(t) for t in ins],
             None, None, None, None, *[_lib.ptr(t) for t in (b1, b2, counts, feat)], *[_lib.ptr(t) for t in geo]]
-    if masked:
-        call = lambda: lib.lcpb200_body_contacts_masked(*args, _lib.ptr(w.nc_mask), st)
-    else:
-        call = lambda: lib.lcpb200_body_contacts(*args, st)
+    call = lambda: lib.lcpb200_contacts(*args, _lib.ptr(w.nc_mask) if masked else None, st)
     for _ in range(5):
         _lib.check(call())
     torch.cuda.synchronize()

@@ -1,8 +1,8 @@
 """World-steps per second of `BatchedWorld` with dynamic polygons, and the time of its contact walk:
   1. 1024 worlds of 12 boxes + 12 circles in a bin of 3 obstacles (condensed kernels, fp64);
   2. one large mixed bin, 80 boxes + 16 hulls + 24 circles (3 * 120 > 128: banded kernel);
-  3. the contact walk (lcpb200_body_contacts, detection + geometry) of pairing 1's worlds against the circle-only walk
-     (lcpb200_world_contacts) over the same number of bodies, all of them circles.
+  3. the contact walk (lcpb200_contacts with feat: the polygon walk, detection + geometry) of pairing 1's worlds against
+     the circle-only walk (lcpb200_contacts without feat) over the same number of bodies, all of them circles.
 Legs of a pairing alternate inside every round; prints one JSON line per pairing with the median and the spread
 (min, max) of every leg, plus the card and its power limit.
 
@@ -85,17 +85,17 @@ def walk_time(w, circles_only, reps=50):
         pos = w.p[:, :, 1:].contiguous()
         rad = torch.full((B, w.nd), 8.0, dtype=f64, device=dev)
         mat = torch.full((B, w.nd), 0.5, dtype=f64, device=dev)
-        args = (_lib.dtype_code(f64), B, w.nd, w.no, w.nv, cap, w.eps,
-                *[_lib.ptr(t) for t in (pos, rad, mat, mat, w.ov, w.oref, w.ofric, w.orest, b1, b2, counts)],
-                *[_lib.ptr(t) for t in geo], st)
-        call = lambda: lib.lcpb200_world_contacts(*args)
+        args = (_lib.dtype_code(f64), B, w.nd, 0, w.no, w.nv, cap, w.eps,
+                *[_lib.ptr(t) for t in (pos, rad, mat, mat, None, None, None, None, w.ov, w.oref, w.ofric, w.orest,
+                                        b1, b2, counts, None)],
+                *[_lib.ptr(t) for t in geo], None, st)
     else:
         pv, pcen = w.polygon_vertices().contiguous(), w.p[:, w.nb:, 1:].contiguous()
         ins = [t.contiguous() for t in (w.p[:, :w.nb, 1:], w.rad, w.fric_coeff, w.restitution, pv, pcen, w.pfric,
                                         w.prest, w.ov, w.oref, w.ofric, w.orest)]         # held for every call
         args = (_lib.dtype_code(f64), B, w.nb, w.np, w.no, w.nv, cap, w.eps, *[_lib.ptr(t) for t in ins],
-                *[_lib.ptr(t) for t in (b1, b2, counts, feat)], *[_lib.ptr(t) for t in geo], st)
-        call = lambda: lib.lcpb200_body_contacts(*args)
+                *[_lib.ptr(t) for t in (b1, b2, counts, feat)], *[_lib.ptr(t) for t in geo], None, st)
+    call = lambda: lib.lcpb200_contacts(*args)
     for _ in range(5):
         _lib.check(call())
     torch.cuda.synchronize()

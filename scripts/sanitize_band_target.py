@@ -1,6 +1,6 @@
 """Tiny banded-kernel calls for compute-sanitizer (memcheck / racecheck / synccheck): forward + backward of the
 large-scene kernels forced onto small scenes (with equality rows and per-scene counts), one step of a 60-ball
-world (n = 183: natively banded, includes lcpb200_find_contacts)."""
+world (n = 183: natively banded, includes lcpb200_contacts)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ["LCPB200_FORCE_BANDED"] = "1"

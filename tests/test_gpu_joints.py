@@ -2,7 +2,7 @@
 (`constraints=`, `no_contact=`, `external_force=`): the recorded reference engine calls with two-body equality rows
 replayed through engine_solve and B200PdipmEngine, the trajectories recorded from the unmodified reference
 (tests/golden/bworld_joints.npz), a batch of seeded chains against the joint oracle (oracle/joint_oracle.py), the masked
-contact walk (lcpb200_body_contacts_masked) against the unmasked one, rollout gradients against central differences,
+contact walk (lcpb200_contacts with no_contact) against the unmasked one, rollout gradients against central differences,
 fp32 against fp64, the large-scene kernel with a joint, and the constructor checks."""
 import ctypes
 import os
@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from oracle.joint_oracle import OracleJointWorld
-from tests.test_gpu_polygons import body_contacts, random_scene
+from tests.test_gpu_polygons import polygon_walk, random_scene
 from tests.test_joint_oracle import constraint_list
 
 pytestmark = pytest.mark.gpu
@@ -231,8 +231,8 @@ def test_batch_of_seeded_chains_matches_joint_oracle():
 
 
 # ---------------------------------------------------------------------------------------------------- masked walk
-def masked_contacts(scs, dtype, cap, excl):
-    """lcpb200_body_contacts_masked on scenes of equal shapes with the pairs `excl` excluded"""
+def mask_walk(scs, dtype, cap, excl):
+    """lcpb200_contacts with no_contact (the mask walk) on scenes of equal shapes with the pairs `excl` excluded"""
     from lcp_physics_b200 import _lib
     from lcp_physics_b200.world import polygon_centroid
     lib = _lib.load()
@@ -255,7 +255,7 @@ def masked_contacts(scs, dtype, cap, excl):
     b1, b2, feat, counts = i32(B, cap), i32(B, cap), i32(B, cap), i32(B)
     new = lambda *s: torch.empty(B, cap, *s, dtype=dtype, device="cuda")
     geo = [new(2), new(2), new(2), new(), new(), new()]
-    _lib.check(lib.lcpb200_body_contacts_masked(
+    _lib.check(lib.lcpb200_contacts(
         _lib.dtype_code(dtype), B, nb, npoly, no, 6, cap, 0.1,
         *[_lib.ptr(t) for t in (pos, rad, fr, rs, pv, pcen, pfr, prs, ov, oref, ofr, ors, b1, b2, counts, feat)],
         *[_lib.ptr(t) for t in geo], _lib.ptr(mask), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
@@ -264,20 +264,20 @@ def masked_contacts(scs, dtype, cap, excl):
 
 
 @pytest.mark.parametrize("sizes", [(14, 0, 0, 60.0), (12, 0, 3, 80.0), (3, 8, 2, 60.0), (10, 36, 4, 140.0)])
-def test_masked_walk_equals_unmasked_walk_without_excluded_pairs(sizes):
+def test_mask_walk_equals_polygon_walk_without_excluded_pairs(sizes):
     """circles only, circles + obstacles, mixed polygon scenes (the last spans two 1024-pair chunks): the masked walk
     gives the unmasked walk's contacts minus the excluded pairs, in the same order, with the same feat and bitwise
     equal geometry"""
     nc, npoly, no, spread = sizes
     scs = [random_scene(100 + s, nc, npoly, no, spread) for s in range(4)]
-    full = body_contacts(scs, f64, cap=1024)
+    full = polygon_walk(scs, f64, cap=1024)
     nd, nt = nc + npoly, nc + npoly + no
     pairs = set()
     for s in range(4):                                        # exclude about half of the pairs that make contact
         n = int(full["counts"][s])
         pairs |= {(int(a), int(b)) for a, b in zip(full["b1"][s, :n].tolist(), full["b2"][s, :n].tolist())}
     excl = sorted(pairs)[::2] + [(nd, nt - 1)] if no > 1 else sorted(pairs)[::2]   # + an obstacle-obstacle pair
-    got = masked_contacts(scs, f64, 1024, excl)
+    got = mask_walk(scs, f64, 1024, excl)
     ex = set(excl)
     removed = 0
     for s in range(4):

@@ -1,6 +1,6 @@
 """GPU: static convex polygon obstacles in `BatchedWorld` (one-body contacts, body2 >= nb).
 
-* lcpb200_world_contacts' pair lists / counts equal `find_contacts_torch`'s bitwise (several 1024-pair chunks,
+* lcpb200_contacts' pair lists / counts equal `find_contacts_torch`'s bitwise (several 1024-pair chunks,
   fp64 / fp32), its geometry equals the differentiable torch geometry (outside and centre-inside cases) and the
   contact list the unmodified reference recorded (tests/golden/bworld_obstacles.npz);
 * engine_solve with one-body contacts equals the reference's pinned formulation (the obstacle an extra body with

@@ -1,6 +1,6 @@
 """GPU: dynamic convex polygons in BatchedWorld (`polygons=`): the hull-hull and circle-polygon contact walk
-(lcpb200_body_contacts) against the CPU oracle (oracle/polygon_oracle.py) on seeded random scenes, the torch geometry
-rebuilt from the kernel's features against the kernel's, trajectories recorded from the unmodified reference
+(lcpb200_contacts with feat) against the CPU oracle (oracle/polygon_oracle.py) on seeded random scenes, the torch
+geometry rebuilt from the kernel's features against the kernel's, trajectories recorded from the unmodified reference
 (tests/golden/bworld_polygons.npz), a mixed scene on the banded kernel, rollout gradients and fp32."""
 import ctypes
 import math
@@ -79,8 +79,8 @@ def _oracle(sc, eps=0.1):
     return o
 
 
-def body_contacts(scs, dtype, cap, geometry=True, eps=0.1):
-    """lcpb200_body_contacts on a batch of scenes of equal shapes"""
+def polygon_walk(scs, dtype, cap, geometry=True, eps=0.1):
+    """lcpb200_contacts with feat (the polygon walk) on a batch of scenes of equal shapes"""
     from lcp_physics_b200 import _lib
     from lcp_physics_b200.world import polygon_centroid
     lib = _lib.load()
@@ -96,10 +96,10 @@ def body_contacts(scs, dtype, cap, geometry=True, eps=0.1):
     b1, b2, feat, counts = i32(B, cap), i32(B, cap), i32(B, cap), i32(B)
     new = lambda *s: torch.empty(B, cap, *s, dtype=dtype, device="cuda")
     geo = [new(2), new(2), new(2), new(), new(), new()] if geometry else [None] * 6
-    _lib.check(lib.lcpb200_body_contacts(
+    _lib.check(lib.lcpb200_contacts(
         _lib.dtype_code(dtype), B, nb, npoly, no, 6, cap, eps,
         *[_lib.ptr(t) for t in (pos, rad, fr, rs, pv, pcen, pfr, prs, ov, oref, ofr, ors, b1, b2, counts, feat)],
-        *[_lib.ptr(t) for t in geo], ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+        *[_lib.ptr(t) for t in geo], None, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
     return dict(b1=b1, b2=b2, feat=feat, counts=counts, geo=geo, pv=pv, pcen=pcen, ov=ov, oref=oref, pfr=pfr, ofr=ofr,
                 pos=pos, rad=rad, fr=fr, rs=rs, prs=prs, ors=ors)
@@ -107,10 +107,10 @@ def body_contacts(scs, dtype, cap, geometry=True, eps=0.1):
 
 # ---------------------------------------------------------------------------------------------------- contact lists
 @pytest.mark.parametrize("sizes", [(3, 8, 2, 60.0), (10, 36, 4, 140.0)])   # the second: 1 300+ pairs, 2 chunks
-def test_body_contacts_match_polygon_oracle(sizes):
+def test_polygon_walk_matches_polygon_oracle(sizes):
     nc, npoly, no, spread = sizes
     scs = [random_scene(100 + s, nc, npoly, no, spread) for s in range(4)]
-    res = body_contacts(scs, f64, cap=1024)
+    res = polygon_walk(scs, f64, cap=1024)
     nb, nd = nc, nc + npoly
     seen_two = seen_one = 0
     for s, sc in enumerate(scs):
@@ -135,11 +135,11 @@ def test_body_contacts_match_polygon_oracle(sizes):
 
 
 @pytest.mark.parametrize("dtype", [f64, torch.float32])
-def test_body_contacts_torch_geometry_from_features_matches_kernel(dtype):
+def test_polygon_walk_torch_geometry_from_features_matches_kernel(dtype):
     """The torch (graph) geometry BatchedWorld builds from feat equals the kernel's geometry."""
     from lcp_physics_b200.world import BatchedWorld
     scs = [random_scene(200 + s, 3, 8, 2, 60.0) for s in range(8)]
-    res = body_contacts(scs, dtype, cap=256)
+    res = polygon_walk(scs, dtype, cap=256)
     w = object.__new__(BatchedWorld)                                               # the torch mirror needs only these
     w.nb, w.np, w.no, w.nv = 3, 8, 2, 6
     w.p = torch.cat([torch.zeros(8, 11, 1, dtype=dtype, device="cuda"),
@@ -155,20 +155,21 @@ def test_body_contacts_torch_geometry_from_features_matches_kernel(dtype):
             assert float((a[s, :n] - b[s, :n]).abs().max()) <= tol * scale
 
 
-def test_body_contacts_without_polygons_equal_world_contacts():
-    """np == 0 through lcpb200_body_contacts selects the same pairs as lcpb200_world_contacts."""
+def test_polygon_walk_without_polygons_equals_circle_walk():
+    """np == 0 through the polygon walk (lcpb200_contacts with feat) selects the same pairs as the circle walk
+    (lcpb200_contacts without feat)."""
     from lcp_physics_b200 import _lib
     scs = [random_scene(300 + s, 12, 0, 3, 80.0) for s in range(4)]
-    res = body_contacts(scs, f64, cap=256)
+    res = polygon_walk(scs, f64, cap=256)
     lib = _lib.load()
     B, cap = 4, 256
     i32 = lambda *s: torch.empty(*s, dtype=torch.int32, device="cuda")
     b1, b2, counts = i32(B, cap), i32(B, cap), i32(B)
-    _lib.check(lib.lcpb200_world_contacts(_lib.dtype_code(f64), B, 12, 3, 6, cap, 0.1,
-                                          *[_lib.ptr(t) for t in (res["pos"], res["rad"], None, None, res["ov"], None,
-                                                                  None, None, b1, b2, counts)],
-                                          None, None, None, None, None, None,
-                                          ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    _lib.check(lib.lcpb200_contacts(_lib.dtype_code(f64), B, 12, 0, 3, 6, cap, 0.1,
+                                    *[_lib.ptr(t) for t in (res["pos"], res["rad"], None, None, None, None, None, None,
+                                                            res["ov"], res["oref"], None, None, b1, b2, counts)],
+                                    None, None, None, None, None, None, None, None,
+                                    ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
     assert torch.equal(counts, res["counts"]) and torch.equal(b1, res["b1"]) and torch.equal(b2, res["b2"])
     assert bool((res["feat"] == -1).all())

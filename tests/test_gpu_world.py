@@ -47,8 +47,8 @@ def test_batched_world_is_differentiable():
 
 @pytest.mark.parametrize("nballs,cols,dtype", [(24, 6, torch.float64), (24, 6, torch.float32), (300, 20, torch.float64)])
 def test_find_contacts_kernel_matches_torch_pair_scan(nballs, cols, dtype):
-    """lcpb200_find_contacts (pair test + ordered compaction, csrc/lcp_contacts.cuh) against the independent torch
-    implementation (all-pairs tensors + stable sort): identical counts and identical ordered pair lists, on
+    """lcpb200_contacts' circle walk (pair test + ordered compaction, csrc/lcp_contacts.cuh) against the independent
+    torch implementation (all-pairs tensors + stable sort): identical counts and identical ordered pair lists, on
     loose drops (0..few contacts per scene) and on a dense pile (~850 contacts)."""
     from lcp_physics_b200.scenes import make_ball_drop, make_ball_pile
     from lcp_physics_b200.world import BatchedWorld
@@ -78,7 +78,7 @@ def test_find_contacts_reports_overflow():
 
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32])
 def test_fused_contact_geometry_matches_torch_geometry(dtype):
-    """lcpb200_contact_geometry (used when nothing needs autograd) against the differentiable torch geometry of the
+    """lcpb200_contacts' geometry (used when nothing needs autograd) against the differentiable torch geometry of the
     same selected pairs: normal, p1, p2, penetration, mu, restitution."""
     from lcp_physics_b200.scenes import make_ball_pile
     from lcp_physics_b200.world import BatchedWorld
