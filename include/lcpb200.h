@@ -182,7 +182,8 @@ int lcpb200_backward_host(lcpb200_handle_t h, int B,
  *                                                     reference points (p2 is relative to it), friction and
  *                                                     restitution (ofric / orest: only for the geometry)
  *   body1[B,cap] body2[B,cap] int32                   OUT: the contacts' pairs in the order above (the order the
- *                                                     reference appends contacts in), padded with the pair (0, 1);
+ *                                                     reference appends contacts in), padded with the pair (0, 1)
+ *                                                     ((0, 0) when nb + np + no == 1);
  *                                                     body2 >= nb + np names obstacle body2 - nb - np, the one-body
  *                                                     contacts of lcpb200_engine_forward
  *   counts[B] int32                                   OUT: number of contacts (may exceed cap: then the lists hold the
@@ -192,7 +193,9 @@ int lcpb200_backward_host(lcpb200_handle_t h, int B,
  *                                                     plane; bits 2-3 the first clip's outcome; bit 4 body2 holds the
  *                                                     reference face; bits 5-12 reference edge; bits 13-20 incident
  *                                                     edge), from which the geometry is rebuilt; -1 for other
- *                                                     contacts. Required when np > 0 or no_contact != NULL, NULL
+ *                                                     contacts and unused slots (0 in unused slots when nb == 0:
+ *                                                     a hull-hull padding pair). Required when np > 0 or
+ *                                                     no_contact != NULL, NULL
  *                                                     allowed otherwise
  *   normal[B,cap,2] p1 p2[B,cap,2] penetration mu restitution_c[B,cap]
  *                                                     OUT, all NULL (detection only) or all non-NULL: geometry and

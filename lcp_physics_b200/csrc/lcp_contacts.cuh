@@ -9,7 +9,8 @@
 // the LCP the engine builds -- and compacts the contacts IN THAT ORDER with a block-wide exclusive scan of the
 // per-thread contact counts (warp prefix through shuffles, warp totals through shared memory): deterministic, no
 // atomics, no sort.
-// Outputs: the pair list body1 / body2 [B, cap] (padded with the pair (0, 1)), and the TRUE number of contacts per
+// Outputs: the pair list body1 / body2 [B, cap] (padded with the pair (0, 1), or (0, 0) when the list holds one
+// body), and the TRUE number of contacts per
 // scene (which may exceed cap: the caller checks). The contact geometry (normal, p1, p2, penetration) is evaluated
 // on the selected pairs only (contact_geometry_kernel, or differentiable torch ops), so the walk replaces the
 // O(nb^2) part: at nb = 513 it tests 131 328 pairs per scene.
@@ -379,7 +380,7 @@ __global__ void __launch_bounds__(NT) find_contacts_kernel(Bodies<T> bd, int B, 
       base += total;
       __syncthreads();                                           // warp_tot is rewritten by the next chunk
     }
-    const int pad2 = nt > 1 ? 1 : 0;                             // padding: a valid pair, (0, 1)
+    const int pad2 = nt > 1 ? 1 : 0;                             // padding: (0, 1), or (0, 0) for one body
     for (int k = base + tid; k < cap; k += NT) {
       o1[k] = 0; o2[k] = pad2;
       if (HULLS && feat) feat[(size_t)sc * cap + k] = nb == 0 ? 0 : -1;   // a hull-hull padding pair: edge 0, v0
@@ -398,7 +399,8 @@ __global__ void __launch_bounds__(NT) find_contacts_kernel(Bodies<T> bd, int B, 
 // n . (v - v_ref), pt = v - n dist; reference = body2: normal = n, p1 = pt + c2 - c1, p2 = pt; reference = body1:
 // normal = -n, p1 = pt, p2 = pt + c1 - c2; penetration = -dist.
 // mu / restitution = mean of the two bodies' (world.py:144-151, :213-224). Unused slots (k >= counts[scene]) get the
-// geometry of the padding pair and penetration = -1e30.
+// geometry of the padding pair and penetration = -1e30; the pair (0, 0) of one circle gets the normal (1, 0) (a unit
+// offset instead of 0 / 0), so every slot is finite.
 template <typename T, bool HULLS>
 __global__ void __launch_bounds__(NT) contact_geometry_kernel(Bodies<T> bd, int B, int cap,
                                                               const int32_t* __restrict__ body1,
@@ -416,7 +418,8 @@ __global__ void __launch_bounds__(NT) contact_geometry_kernel(Bodies<T> bd, int 
     const T* R = bd.rad + (size_t)sc * nb;
     T nx, ny, a1x, a1y, a2x, a2y, pn;
     if (j < nb) {
-      const T dx = P[2 * i] - P[2 * j], dy = P[2 * i + 1] - P[2 * j + 1];
+      // the padding pair (0, 0) of a one-body list gets a unit offset, as _geometry_torch: finite, never a contact
+      const T dx = i != j ? P[2 * i] - P[2 * j] : T(1), dy = i != j ? P[2 * i + 1] - P[2 * j + 1] : T(0);
       const T dist = sqrt(dx * dx + dy * dy);
       const T r1 = R[i], r2 = R[j];
       pn = r1 + r2 - dist;

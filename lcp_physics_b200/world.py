@@ -341,7 +341,8 @@ class BatchedWorld:
             most = int(self.pi.numel()) + int((self.pi >= nb).sum())
             self.cap = int(contact_capacity) if contact_capacity else max(1, min(most, (4 if self.no else 3) * nb + 8 * self.np))
         else:
-            self.cap = int(contact_capacity) if contact_capacity else min(int(self.pi.numel()), (4 if self.no else 3) * nb)
+            # a world of one circle has no pair but still needs one (unused) contact slot
+            self.cap = int(contact_capacity) if contact_capacity else max(1, min(int(self.pi.numel()), (4 if self.no else 3) * nb))
         # 3 (nb + npoly) + 3 n_static <= 128 and <= 256 contacts: condensed-KKT kernels (fp32 / fp64,
         # differentiable); larger scenes: the banded large-scene kernels (fp64; lcp_banded.cuh)
         self.large = self.n + self.ne > 128 or 4 * self.cap > 1024
@@ -628,8 +629,9 @@ class BatchedWorld:
         r1 = take(self.rad, i1)
         one = torch.zeros_like(c)
         one[..., 0] = 1.0
-        # circle-circle (slots of obstacle pairs get a harmless unit offset: no 0 / 0 in either pass)
-        dcc = torch.where(cc.unsqueeze(2), c - take2(pos, j), one)
+        # circle-circle (slots of obstacle pairs and the padding pair (0, 0) of a one-body world get a harmless unit
+        # offset: no 0 / 0 in either pass)
+        dcc = torch.where((cc & (i1 != j)).unsqueeze(2), c - take2(pos, j), one)
         dist = dcc.norm(dim=2)
         r2 = take(self.rad, j)
         pen_cc = r1 + r2 - dist
