@@ -306,6 +306,25 @@ int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode,
  * into chunks only to fill the GPU when B is small, and the results do not depend on that split. The same NULL
  * rules and flags as lcpb200_engine_backward; a scene with status -100 gets zero gradients in every slot.
  * lcpb200_engine_backward is this call with R = 1. */
+/* lcpb200_engine_jvp_batched: R >= 1 Jacobian-vector products of the same saved solves in one call -- the
+ * forward-mode derivative of zhat along R directions of the inputs (R = 1: one torch.func.jvp; R = k: the k columns
+ * of a jacfwd). Same primal inputs and saved solve as lcpb200_engine_backward_batched; every tangent is [R,B,...]
+ * with the shape of its input (t_mass[R,B,nb], t_v[R,B,n], t_normal[R,B,nc,2], t_A[R,B,e,n], t_b[R,B,e], ...) or
+ * NULL, which means zero and is not read. dz[R,B,n] receives the tangents of zhat. Each scene's KKT matrix K (not
+ * transposed) is factored once per chunk of tangents at the backward's d clamp, so the result is the transpose of
+ * the LCPB200_BWD_EXACT_ADJOINT backward: the true derivative of the solve. A scene with status -100 gets zero
+ * rows. Same kernel selection as the backward (the large-scene kernel when the condensed one cannot take the
+ * sizes, or LCPB200_FORCE_BANDED=1 for fp64). */
+int lcpb200_engine_jvp_batched(lcpb200_handle_t h, int R, int B, int nb, int nc, int mode, double dt,
+                               const void* mass, const void* inertia, const void* v, const void* fext,
+                               const void* normal, const void* p1, const void* p2,
+                               const int32_t* body1, const int32_t* body2, const int32_t* contact_count,
+                               const void* mu, const void* restitution, const void* A,
+                               const void* zhat, const void* nu, const void* lam, const void* slack,
+                               const void* t_mass, const void* t_inertia, const void* t_v, const void* t_fext,
+                               const void* t_normal, const void* t_p1, const void* t_p2, const void* t_mu,
+                               const void* t_restitution, const void* t_A, const void* t_b,
+                               void* dz, void* stream);
 int lcpb200_engine_backward_batched(lcpb200_handle_t h, int R, int B, int nb, int nc, int mode, double dt,
                                     const void* mass, const void* inertia, const void* v, const void* fext,
                                     const void* normal, const void* p1, const void* p2,

@@ -38,6 +38,7 @@ _SIGS = {
                                 [ctypes.c_uint, _vp]),
     "lcpb200_engine_backward_batched": (ctypes.c_int, [_vp] + [ctypes.c_int] * 5 + [ctypes.c_double] + [_vp] * 29 +
                                         [ctypes.c_uint, _vp]),
+    "lcpb200_engine_jvp_batched": (ctypes.c_int, [_vp] + [ctypes.c_int] * 5 + [ctypes.c_double] + [_vp] * 30),
     "lcpb200_contacts": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 24),
     "lcpb200_assemble": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 17),
     "lcpb200_assemble_backward": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 25),

@@ -8,6 +8,7 @@ namespace bnd {
 
 cudaError_t launch_band_forward(const BArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_band_backward(const BBwdArgs& a, int grid, cudaStream_t st);
+cudaError_t launch_band_jvp(const BJvpArgs& a, int grid, cudaStream_t st);
 cudaError_t configure_band(int smem_bytes, int dyn_max, int* occ);
 
 }  // namespace bnd

@@ -21,11 +21,21 @@ cudaError_t launch_cond_backward_t<LCP_T, LCP_NS>(const CBwdArgs<LCP_T>& a, int 
 }
 
 template <>
+cudaError_t launch_cond_jvp_t<LCP_T, LCP_NS>(const CJvpArgs<LCP_T>& a, int grid, cudaStream_t st) {
+  if (a.prof) cond_jvp_kernel<LCP_T, LCP_NS, true><<<grid, NT, a.P.smem_bytes, st>>>(a);
+  else cond_jvp_kernel<LCP_T, LCP_NS, false><<<grid, NT, a.P.smem_bytes, st>>>(a);
+  return cudaGetLastError();
+}
+
+template <>
 cudaError_t configure_cond_t<LCP_T, LCP_NS>(int smem_bytes, int dyn_max, int* occ) {
   cudaError_t e;
   const void* fns[4] = {(const void*)cond_forward_kernel<LCP_T, LCP_NS, false>, (const void*)cond_backward_kernel<LCP_T, LCP_NS, false>,
                         (const void*)cond_forward_kernel<LCP_T, LCP_NS, true>, (const void*)cond_backward_kernel<LCP_T, LCP_NS, true>};
   for (const void* f : fns)
+    if ((e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max)) != cudaSuccess) return e;
+  const void* jvp[2] = {(const void*)cond_jvp_kernel<LCP_T, LCP_NS, false>, (const void*)cond_jvp_kernel<LCP_T, LCP_NS, true>};
+  for (const void* f : jvp)
     if ((e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max)) != cudaSuccess) return e;
   // the grid is sized by the production kernels; the profiling ones run on the same grid
   int of = 0, ob = 0;

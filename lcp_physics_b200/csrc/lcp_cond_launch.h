@@ -9,6 +9,7 @@ namespace cnd {
 
 template <typename T, int NS> cudaError_t launch_cond_forward_t(const CFwdArgs<T>& a, int grid, cudaStream_t st);
 template <typename T, int NS> cudaError_t launch_cond_backward_t(const CBwdArgs<T>& a, int grid, cudaStream_t st);
+template <typename T, int NS> cudaError_t launch_cond_jvp_t(const CJvpArgs<T>& a, int grid, cudaStream_t st);
 template <typename T, int NS> cudaError_t configure_cond_t(int smem_bytes, int dyn_max, int* occ);
 
 }  // namespace cnd

@@ -1635,5 +1635,191 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
   }
 }
 
+// ------------------------------------------------------------------ Jacobian-vector products, engine path
+// Forward-mode derivative of the engine solve (DESIGN.md section 8). At the saved iterate (zhat, lam, slack, nu)
+// with the backward's clamp of d = lam / slack, the PDIPM residuals (pdipm.py:82-90) linearised in the inputs give
+//     K [dx; ds; dz; dy] = -(r_x, 0, r_z, r_y),
+//     r_x = dQ zhat + dp + dG^T lam + dA^T nu,   r_z = dG zhat - dF lam - dh,   r_y = dA zhat - db,
+// K the NON-transposed matrix the forward factors; the tangent of zhat is dx. d(Q, p, G, h, F) is the directional
+// derivative of the assembly (build_structure_soa), evaluated per contact and per dof, never as a dense matrix.
+// Every tangent is [R][B][...] like CBwdArgs' cotangents, nullptr = zero.
+template <typename T>
+struct CJvpArgs {
+  CPlan P;
+  int B, R, chunks;           // work items (scene, chunk of tangents), as CBwdArgs
+  const T* A;
+  const T *zhat, *nu, *lam, *slack;
+  EngineSoA<T> soa;
+  const T *t_mass, *t_inertia, *t_v, *t_fext, *t_normal, *t_p1, *t_p2, *t_mu, *t_rest, *t_A, *t_b;
+  T* dz;                      // [R][B][n]
+  long long* prof;
+};
+
+// Tangent of contact_row along (dx, dy) when the points move by (tp1, tp2) and the direction by (tdx, tdy).
+template <typename T>
+__device__ __forceinline__ void contact_row_tangent(T p1x, T p1y, T p2x, T p2y, T dx, T dy, T t1x, T t1y, T t2x,
+                                                    T t2y, T tdx, T tdy, T (&r1)[3], T (&r2)[3]) {
+  r1[0] = t1x * dy + p1x * tdy - t1y * dx - p1y * tdx; r1[1] = tdx; r1[2] = tdy;
+  r2[0] = -(t2x * dy + p2x * tdy - t2y * dx - p2y * tdx); r2[1] = -tdx; r2[2] = -tdy;
+}
+
+// Right-hand side (r_x, r_z, r_y) of tangent slot so into S.rx, S.rz, S.ry; the saved iterate is in S.x, S.z, S.y.
+template <typename T>
+__device__ __noinline__ void jvp_rhs(const CJvpArgs<T>& a, CSmem<T> S, Struct st, int sc, int so) {
+  const CPlan& P = a.P;
+  const EngineSoA<T>& E = a.soa;
+  const int n = P.n, e = P.e, tid = threadIdx.x, nb = E.nb, ncs = E.nc, nc = st.ncomp;
+  const int32_t* tb1 = E.b1 + (E.nc_s ? (size_t)sc * ncs : 0);
+  const int32_t* tb2 = E.b2 + (E.nc_s ? (size_t)sc * ncs : 0);
+  const T* v = E.v + (size_t)sc * n;
+  const T* tv = a.t_v ? a.t_v + (size_t)so * n : nullptr;
+  const T* zh = S.x(); const T* lm = S.z();
+  auto tget = [](const T* t, size_t i) { return t ? t[i] : T(0); };
+  // r_z, one thread per contact: rows {c, nc + 2c, nc + 2c + 1, 3nc + c} (mode 0) or {c} (mode 1)
+  for (int c = tid; c < nc; c += NT) {
+    const size_t ic = (size_t)sc * ncs + c, oc = (size_t)so * ncs + c;
+    const int b1 = tb1[c], b2 = tb2[c];
+    const bool two = b2 < nb;
+    const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
+    const T p1x = E.p1[ic * 2], p1y = E.p1[ic * 2 + 1], p2x = E.p2[ic * 2], p2y = E.p2[ic * 2 + 1];
+    const T tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
+    const T t1x = tget(a.t_p1, oc * 2), t1y = tget(a.t_p1, oc * 2 + 1);
+    const T t2x = tget(a.t_p2, oc * 2), t2y = tget(a.t_p2, oc * 2 + 1);
+    T r1[3], r2[3], d1[3], d2[3];
+    contact_row<T>(p1x, p1y, p2x, p2y, nx, ny, r1, r2);
+    contact_row_tangent<T>(p1x, p1y, p2x, p2y, nx, ny, t1x, t1y, t2x, t2y, tnx, tny, d1, d2);
+    T jv = 0, tjv = 0, gz = 0;                    // Jc v, d(Jc v), dJc zhat
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const int j1 = 3 * b1 + q;
+      jv += r1[q] * v[j1];
+      tjv += d1[q] * v[j1] + (tv ? r1[q] * tv[j1] : T(0));
+      gz += d1[q] * zh[j1];
+      if (two) {
+        const int j2 = 3 * b2 + q;
+        jv += r2[q] * v[j2];
+        tjv += d2[q] * v[j2] + (tv ? r2[q] * tv[j2] : T(0));
+        gz += d2[q] * zh[j2];
+      }
+    }
+    const T rc = E.rest[ic], trc = tget(a.t_rest, oc);
+    if (E.mode == 0) {
+      S.rz()[c] = gz - (trc * jv + rc * tjv);                          // h_c = (Jc v) rest
+      contact_row<T>(p1x, p1y, p2x, p2y, ny, -nx, r1, r2);
+      contact_row_tangent<T>(p1x, p1y, p2x, p2y, ny, -nx, t1x, t1y, t2x, t2y, tny, -tnx, d1, d2);
+      T fz = 0;                                                        // dJf zhat (row f2 = -row f1)
+#pragma unroll
+      for (int q = 0; q < 3; ++q) { fz += d1[q] * zh[3 * b1 + q]; if (two) fz += d2[q] * zh[3 * b2 + q]; }
+      S.rz()[nc + 2 * c] = fz;
+      S.rz()[nc + 2 * c + 1] = -fz;
+      S.rz()[3 * nc + c] = -(tget(a.t_mu, oc) * lm[c]);              // F[gamma_c][c] = mu_c
+    } else {
+      S.rz()[c] = gz - (tjv * (T(1) - rc) - trc * jv);                 // h_c = (Jc v)(1 - rest)
+    }
+  }
+  // r_x, one thread per dof; dG^T lam is gathered through the dof's contact list (ascending: deterministic)
+  for (int j = tid; j < n; j += NT) {
+    const int body = j / 3, comp = j - 3 * body;
+    const T q = comp == 0 ? E.inertia[(size_t)sc * nb + body] : E.mass[(size_t)sc * nb + body];
+    const T tq = comp == 0 ? tget(a.t_inertia, (size_t)so * nb + body) : tget(a.t_mass, (size_t)so * nb + body);
+    T acc = tq * zh[j];
+    if (E.mode == 0) acc += tq * v[j] + q * (tv ? tv[j] : T(0)) + E.dt * tget(a.t_fext, (size_t)so * n + j);
+    const int cnt = S.clcnt()[j];
+    for (int l = 0; l < cnt; ++l) {
+      const int c = S.clist()[l * n + j] >> 3;
+      const size_t ic = (size_t)sc * ncs + c, oc = (size_t)so * ncs + c;
+      const bool side1 = tb1[c] == body;
+      const T* pp = side1 ? E.p1 : E.p2;
+      const T* tp = side1 ? a.t_p1 : a.t_p2;
+      const T px = pp[ic * 2], py = pp[ic * 2 + 1], tpx = tget(tp, oc * 2), tpy = tget(tp, oc * 2 + 1);
+      const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
+      const T tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
+      // d(row entry) along direction (dx, dy): [p x d, d] of this body (negated for body2)
+      auto drow = [&](T dx, T dy, T tdx, T tdy) {
+        return comp == 0 ? tpx * dy + px * tdy - tpy * dx - py * tdx : (comp == 1 ? tdx : tdy);
+      };
+      T g = drow(nx, ny, tnx, tny) * lm[c];
+      if (E.mode == 0) g += drow(ny, -nx, tny, -tnx) * (lm[nc + 2 * c] - lm[nc + 2 * c + 1]);
+      acc += side1 ? g : -g;
+    }
+    if (e > 0 && a.t_A) {
+      const T* tA = a.t_A + (size_t)so * e * n;
+      for (int k = 0; k < e; ++k) acc += tA[(size_t)k * n + j] * S.y()[k];
+    }
+    S.rx()[j] = acc;
+  }
+  for (int k = tid; k < e; k += NT) {
+    T acc = -tget(a.t_b, (size_t)so * e + k);
+    if (a.t_A) {
+      const T* tA = a.t_A + (size_t)so * e * n + (size_t)k * n;
+      for (int j = 0; j < n; ++j) acc += tA[j] * zh[j];
+    }
+    S.ry()[k] = acc;
+  }
+  __syncthreads();
+}
+
+// One factorisation of K (not transposed) at the saved solution, then one right-hand side and one solve per
+// tangent r in [r0, r1). The prologue is backward_scene's, kept separate so that the backward's code is unchanged.
+template <typename T, int NS, int CS, typename PF>
+__device__ __forceinline__ void jvp_scene(const CJvpArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc,
+                                          int r0, int r1) {
+  const CPlan& P = a.P;
+  const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x;
+  const T* zh = a.zhat + (size_t)sc * n;
+  const T* lam = a.lam + (size_t)sc * P.m;
+  const T* slk = a.slack + (size_t)sc * P.m;
+  for (int i = tid; i < n; i += NT) S.x()[i] = zh[i];
+  for (int i = tid; i < m; i += NT) {
+    T d = lam[i] / slk[i];
+    if (sizeof(T) == 8) d = d > T(1e10) ? T(1e10) : (d < T(1e-10) ? T(1e-10) : d);   // backward_scene's clamp
+    S.z()[i] = lam[i]; S.s()[i] = slk[i]; S.d()[i] = d; S.rs2()[i] = T(0);
+  }
+  for (int i = tid; i < e; i += NT) S.y()[i] = a.nu[(size_t)sc * e + i];
+  __syncthreads();
+  factor_kkt<T, NS, CS>(P, S, st, pf, false);
+  for (int r = r0; r < r1; ++r) {
+    const int so = r * a.B + sc;
+    jvp_rhs<T>(a, S, st, sc, so);
+    solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), S.rz(), e > 0 ? S.ry() : nullptr, S.dx(), S.ds(), S.dz(),
+                         S.dy());
+    for (int i = tid; i < n; i += NT) a.dz[(size_t)so * n + i] = S.dx()[i];
+    __syncthreads();
+    pf.lap(CPH_GRADS);
+  }
+}
+
+template <typename T, int NS, bool PROF>
+__global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_jvp_kernel(const __grid_constant__ CJvpArgs<T> a) {
+  const CPlan& P = a.P;
+  CSmem<T> S(P);
+  const int n = P.n, e = P.e, tid = threadIdx.x;
+  __shared__ int singular_s;
+  Prof<PROF> pf(PROF ? a.prof + (size_t)blockIdx.x * CPH_COUNT : nullptr);
+  for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
+    const int sc = w / a.chunks, k = w - sc * a.chunks;
+    const int r0 = (int)((long long)a.R * k / a.chunks), r1 = (int)((long long)a.R * (k + 1) / a.chunks);
+    if (tid == 0) singular_s = 0;
+    __syncthreads();
+    pf.start();
+    Struct st;
+    const bool ok = build_structure_soa<T>(P, S, st, a.soa, sc, e > 0 ? a.A + (size_t)sc * e * n : nullptr, &singular_s);
+    __syncthreads();
+    pf.lap(CPH_STRUCT);
+    if (!ok) {                                    // the forward reported it (status -100 / -1): zero tangents
+      for (int r = r0; r < r1; ++r)
+        for (int i = tid; i < n; i += NT) a.dz[((size_t)r * a.B + sc) * n + i] = T(0);
+      __syncthreads();
+      continue;
+    }
+    if constexpr (LU_BW < NS - 1) mark_band_lu<T>(P, S, st);
+    switch (st.cs) {
+      case 1: jvp_scene<T, NS, 1>(a, S, st, pf, sc, r0, r1); break;
+      default: jvp_scene<T, NS, 4>(a, S, st, pf, sc, r0, r1); break;   // the engine builds 1 (mode 1) or 4 rows
+    }
+    __syncthreads();
+  }
+}
+
 }  // namespace cnd
 }  // namespace lcpb200

@@ -911,6 +911,89 @@ extern "C" int lcpb200_engine_backward_batched(lcpb200_handle_t h, int R, int B,
                                          dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, st);
 }
 
+template <typename T>
+static int engine_jvp_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int mode, double dt, const void* mass,
+                        const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
+                        const void* p2, const int32_t* b1, const int32_t* b2, const int32_t* ncs, const void* mu,
+                        const void* rest, const void* A, const void* zhat, const void* nu, const void* lam,
+                        const void* slack, const void* const (&tg)[11], void* dz, cudaStream_t st) {
+  CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
+  cnd::CJvpArgs<T> c;
+  c.P = h->cplan;
+  c.B = B;
+  c.R = R; c.chunks = bwd_chunks(R, B, h->cond_grid);
+  c.A = (const T*)A;
+  c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
+  fill_soa<T>(c.soa, h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, b1, b2, mu, rest, ncs);
+  c.t_mass = (const T*)tg[0]; c.t_inertia = (const T*)tg[1]; c.t_v = (const T*)tg[2]; c.t_fext = (const T*)tg[3];
+  c.t_normal = (const T*)tg[4]; c.t_p1 = (const T*)tg[5]; c.t_p2 = (const T*)tg[6]; c.t_mu = (const T*)tg[7];
+  c.t_rest = (const T*)tg[8]; c.t_A = (const T*)tg[9]; c.t_b = (const T*)tg[10];
+  c.dz = (T*)dz;
+  c.prof = h->cprof;
+  const int cgrid = (int)std::min((long long)B * c.chunks, (long long)h->cond_grid);
+#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, cgrid, st)
+  const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
+#undef CALL_JVP
+  CK(ce);
+  return 0;
+}
+
+extern "C" int lcpb200_engine_jvp_batched(lcpb200_handle_t h, int R, int B, int nb, int nc, int mode, double dt,
+                                          const void* mass, const void* inertia, const void* v, const void* fext,
+                                          const void* normal, const void* p1, const void* p2, const int32_t* body1,
+                                          const int32_t* body2, const int32_t* contact_count, const void* mu,
+                                          const void* restitution, const void* A, const void* zhat, const void* nu,
+                                          const void* lam, const void* slack, const void* t_mass,
+                                          const void* t_inertia, const void* t_v, const void* t_fext,
+                                          const void* t_normal, const void* t_p1, const void* t_p2, const void* t_mu,
+                                          const void* t_restitution, const void* t_A, const void* t_b, void* dz,
+                                          void* stream) {
+  if (int rc = check_engine(h, B, nb, nc, mode)) return rc;
+  if (R < 1) return fail("engine_jvp_batched: need R >= 1");
+  if ((long long)R * B > INT_MAX) return fail("engine_jvp_batched: R * B exceeds INT_MAX");
+  if (!mass || !inertia || !v || !normal || !p1 || !p2 || !body1 || !body2 || !restitution) return fail("engine_jvp: NULL input");
+  if (mode == 0 && !mu) return fail("engine_jvp: mu is needed for mode 0");
+  if (!zhat || !lam || !slack || !dz) return fail("zhat, lam, slack, dz must be non-NULL");
+  if (h->e > 0 && (!A || !nu)) return fail("A and nu must be non-NULL when e > 0");
+  if (B == 0) return 0;
+  const void* const tg[11] = {t_mass, t_inertia, t_v, t_fext, t_normal, t_p1, t_p2, mode == 0 ? t_mu : nullptr,
+                              t_restitution, h->e > 0 ? t_A : nullptr, h->e > 0 ? t_b : nullptr};
+  DeviceGuard dg_;
+  CK(dg_.set(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (use_banded(h)) {
+    const int chunks = bwd_chunks(R, B, h->num_sms);
+    const int items = B * chunks;
+    if (int rc = ensure_bplan(h, items, nb, nc, mode)) return rc;     // one L2 workspace per CTA of this grid
+    bnd::BJvpArgs a;
+    a.P = h->bplan;
+    a.B = B;
+    a.R = R; a.chunks = chunks;
+    memset(&a.soa, 0, sizeof(a.soa));
+    a.soa.mass = (const double*)mass; a.soa.inertia = (const double*)inertia; a.soa.v = (const double*)v;
+    a.soa.fext = (const double*)fext; a.soa.normal = (const double*)normal; a.soa.p1 = (const double*)p1;
+    a.soa.p2 = (const double*)p2; a.soa.mu = (const double*)mu; a.soa.rest = (const double*)restitution;
+    a.soa.b1 = body1; a.soa.b2 = body2; a.soa.nc_s = contact_count; a.soa.nb = nb; a.soa.nc = nc; a.soa.mode = mode;
+    a.soa.dt = dt;
+    a.A = (const double*)A;
+    a.zhat = (const double*)zhat; a.nu = (const double*)nu; a.lam = (const double*)lam; a.slack = (const double*)slack;
+    a.t_mass = (const double*)tg[0]; a.t_inertia = (const double*)tg[1]; a.t_v = (const double*)tg[2];
+    a.t_fext = (const double*)tg[3]; a.t_normal = (const double*)tg[4]; a.t_p1 = (const double*)tg[5];
+    a.t_p2 = (const double*)tg[6]; a.t_mu = (const double*)tg[7]; a.t_rest = (const double*)tg[8];
+    a.t_A = (const double*)tg[9]; a.t_b = (const double*)tg[10];
+    a.dz = (double*)dz;
+    a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
+    a.prof = h->cprof;
+    CK(bnd::launch_band_jvp(a, std::min(items, h->num_sms), st));
+    return 0;
+  }
+  return h->dtype == LCPB200_F32
+             ? engine_jvp_t<float>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
+                                   contact_count, mu, restitution, A, zhat, nu, lam, slack, tg, dz, st)
+             : engine_jvp_t<double>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
+                                    contact_count, mu, restitution, A, zhat, nu, lam, slack, tg, dz, st);
+}
+
 extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode, double dt,
                                        const void* mass, const void* inertia, const void* v, const void* fext,
                                        const void* normal, const void* p1, const void* p2, const int32_t* body1,

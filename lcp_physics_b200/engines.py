@@ -21,6 +21,7 @@ and per-body `fric_coeff`, `restitution`; `world.fric_dirs` must be 2
 (world.py:191-192 hard-codes dir2 = -dir1).
 """
 import ctypes
+import math
 
 import torch
 
@@ -148,6 +149,72 @@ class _EngineVjpFn(torch.autograd.Function):
         return outs, tuple(None if t is None else 0 for t in outs)
 
 
+_TANGENT_INPUTS = 11      # mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b: the inputs a tangent may move
+
+
+def _engine_jvp(tangents, meta, saved):
+    """lcpb200_engine_jvp_batched: tangents of (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b), each
+    [..., *input shape] or None (zero), -> the tangent of zhat [..., B, n]. The leading dims, the same for every
+    tangent, are the R directions of one call: each scene's KKT matrix is factored once for all of them."""
+    lib = _lib.load()
+    (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = saved
+    dt, mode, _exact, B, nb, nc, e = meta
+    dev = mass.device
+    shapes = [t.shape for t in (mass, inertia, v, fext, normal, p1, p2, mu, rest)]
+    shapes += [A.shape, (B, e)] if e > 0 else [None, None]
+    lead = next((tuple(t.shape[:t.dim() - len(s)]) for t, s in zip(tangents, shapes) if t is not None and s is not None),
+                ())
+    R = math.prod(lead)
+    ts = [None if (t is None or s is None) else t.to(mass.dtype).reshape((R,) + tuple(s)).contiguous()
+          for t, s in zip(tangents, shapes)]
+    dz = torch.zeros((R, B, 3 * nb), dtype=mass.dtype, device=dev)
+    if any(t is not None for t in ts) and R > 0:
+        ins = [t.contiguous() for t in (mass, inertia, v, fext, normal, p1, p2)]
+        hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, dev.index,
+                             torch.cuda.current_stream(dev).cuda_stream)
+        with torch.cuda.device(dev):
+            _lib.check(lib.lcpb200_engine_jvp_batched(
+                hd.raw, R, B, nb, nc, mode, dt, *[_lib.ptr(t) for t in ins],
+                _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu.contiguous()), _lib.ptr(rest.contiguous()),
+                _lib.ptr(A.contiguous() if e > 0 else None), *[_lib.ptr(t) for t in (zhat, nu, lam, slack)],
+                *[_lib.ptr(t) for t in ts], _lib.ptr(dz), _stream_ptr(dev)))
+    return dz.reshape(lead + (B, 3 * nb))
+
+
+class _EngineJvpFn(torch.autograd.Function):
+    """The Jacobian-vector product of engine_solve: tangents of the contact list and the saved solve in, the tangent
+    of zhat out. Under torch.func.vmap (jacfwd, vmap of a torch.func.jvp) the tangents of every vmapped call arrive
+    together and go to ONE batched kernel call, which factors each scene's KKT matrix once for all of them."""
+
+    @staticmethod
+    def forward(meta, *args):
+        return _engine_jvp(args[:_TANGENT_INPUTS], meta, args[_TANGENT_INPUTS:])
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError("engine_solve: second derivatives are not implemented")
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise NotImplementedError("engine_solve: second derivatives are not implemented")
+
+    @staticmethod
+    def vmap(info, in_dims, meta, *args):
+        if any(d is not None for d in in_dims[1 + _TANGENT_INPUTS:]):
+            raise NotImplementedError(
+                "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
+                "instead (vmap of the Jacobian-vector product -- torch.func.jvp, jacfwd -- is supported)")
+        # one more leading tangent dim; a tangent this level does not batch is the same for every direction
+        ts = [None if t is None else (t.movedim(d, 0) if d is not None else t.expand((info.batch_size,) + t.shape))
+              for t, d in zip(args[:_TANGENT_INPUTS], in_dims[1:1 + _TANGENT_INPUTS])]
+        out = _EngineJvpFn.apply(meta, *ts, *args[_TANGENT_INPUTS:])
+        return out, 0
+
+
 class _EngineSolveFn(torch.autograd.Function):
     """Fused path (lcpb200_engine_forward / _backward): contact structure-of-arrays in, LCP solution out.
     No dense Q / G / F exists anywhere; the backward returns gradients w.r.t. the contact list.
@@ -189,6 +256,8 @@ class _EngineSolveFn(torch.autograd.Function):
         e = A.shape[1] if (A is not None and A.dim() > 1) else 0
         ctx.save_for_backward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2,
                               zhat, nu, lam, slack, counts)
+        ctx.save_for_forward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2,
+                             zhat, nu, lam, slack, counts)
         ctx.meta = (float(dt), int(mode), bool(exact), B, nb, normal.shape[1], e)
         ctx.mark_non_differentiable(*[t for t in (status, nu, lam, slack) if t is not None])
 
@@ -196,6 +265,12 @@ class _EngineSolveFn(torch.autograd.Function):
     def backward(ctx, dzhat, *_):
         grads = _EngineVjpFn.apply(dzhat, ctx.meta, *ctx.saved_tensors)
         return (*grads, None, None, None, None, None, None, None)
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        # the true derivative whatever exact_adjoint says: K is factored as the forward factors it
+        dzhat = _EngineJvpFn.apply(ctx.meta, *tangents[:_TANGENT_INPUTS], *ctx.saved_tensors)
+        return dzhat, None, None, None, None
 
     @staticmethod
     def vmap(info, in_dims, *args):
@@ -223,7 +298,12 @@ def engine_solve(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2,
     counts [B] int32 (batched worlds): scene s uses its first counts[s] contacts; body1/body2 are then [B,nc].
     body2 >= nb names a static obstacle (no dofs: a wall, floor or ramp): a one-body contact whose rows touch body1's
     three columns only -- the reference's formulation with the obstacle pinned by a TotalConstraint, reduced by the
-    pinned dofs; its p2 is unused (zero gradient). body1 must be a body (< nb)."""
+    pinned dofs; its p2 is unused (zero gradient). body1 must be a body (< nb).
+    Differentiable in reverse mode (backward, torch.func.vjp / grad / jacrev) and in forward mode (torch.func.jvp /
+    jacfwd, torch.autograd.forward_ad dual tensors); the k directions of a jacfwd or vmap(jvp) go to one kernel call.
+    Forward mode is always the true derivative of the solve, the transpose of the exact_adjoint=True backward; with
+    exact_adjoint=False the backward gives the reference's gradients, so jacfwd and jacrev then differ whenever
+    friction is on (DESIGN.md section 3.4). Second derivatives are not implemented."""
     _lib.require_cuda()
     zhat, status = _EngineSolveFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b, body1, body2, dt, mode,
                                         max_iter, exact_adjoint, counts)[:2]

@@ -38,6 +38,7 @@ import ctypes
 import math
 
 import torch
+import torch.autograd.forward_ad as fwAD
 
 from . import _lib
 from .engines import engine_solve
@@ -201,11 +202,22 @@ class _DetectFn(torch.autograd.Function):
     @staticmethod
     def setup_context(ctx, inputs, output):
         ctx.n_inputs = len(inputs)
+        ctx.n_outputs = len(output)
         ctx.mark_non_differentiable(*output)
 
     @staticmethod
     def backward(ctx, *grads):
         return (None,) * ctx.n_inputs
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        return (None,) * ctx.n_outputs
+
+    @staticmethod
+    def vmap(info, in_dims, fn, *tensors):
+        # reached only when an argument is batched at this vmap level (jacfwd batches tangents, not the state)
+        raise NotImplementedError("BatchedWorld: vmap over the world's state is not supported; batch scenes along "
+                                  "dim 0 instead")
 
 
 def _detect(fn, *tensors):
@@ -214,6 +226,12 @@ def _detect(fn, *tensors):
     if any(t is not None and torch._C._functorch.is_functorch_wrapped_tensor(t) for t in tensors):
         return _DetectFn.apply(fn, *tensors)
     return fn(*tensors)
+
+
+def _has_tangent(t):
+    """True when t carries a forward-mode tangent: an input of torch.func.jvp / jacfwd (a functorch-wrapped tensor) or
+    a torch.autograd.forward_ad dual tensor. Forward mode leaves requires_grad False."""
+    return t is not None and fwAD.unpack_dual(t).tangent is not None
 
 
 def _pad_vertices(v, V):
@@ -471,9 +489,9 @@ class BatchedWorld:
         pverts = self.polygon_vertices() if self.np else None
         poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
         obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
-        needs_graph = torch.is_grad_enabled() and any(
-            t is not None and t.requires_grad
-            for t in (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
+        tracked = (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst
+        needs_graph = (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tracked)) or any(
+            _has_tangent(t) for t in tracked)
         # feat selects the polygon walk, which worlds with polygons or no_contact pairs need; the others keep the
         # circle walk
         with_feat = self.np > 0 or self.nc_mask is not None
