@@ -67,7 +67,7 @@ extern "C" {
 /* flags for lcpb200_backward */
 #define LCPB200_BWD_BUG_COMPATIBLE   0u /* reference behaviour: un-transposed KKT (SURVEY.md F6) */
 #define LCPB200_BWD_EXACT_ADJOINT    1u /* transposed KKT system (true adjoint)                  */
-#define LCPB200_BWD_REUSE_STRUCTURE  2u /* lcpb200_backward only: (Q, G, A, F) are the inputs of the
+#define LCPB200_BWD_REUSE_STRUCTURE  2u /* dense calls only: (Q, G, A, F) are the inputs of the
                                           * last lcpb200_forward on this handle (same B): reuse the
                                           * block structure it found instead of scanning the dense
                                           * matrices again (19 KB instead of 0.4 MB per scene at
@@ -123,6 +123,39 @@ int lcpb200_backward(lcpb200_handle_t h, int B,
                      void* dQ, void* dp, void* dG, void* dh, void* dA, void* db, void* dF,
                      const void* Rsave /* from lcpb200_forward, or NULL = recompute */,
                      unsigned flags, void* stream);
+
+/* lcpb200_backward_batched: R >= 1 cotangents of the same saved solves in one call -- the rows of a
+ * vector-Jacobian product (R = n one-hot cotangents per scene: the whole Jacobian of zhat). Same inputs as
+ * lcpb200_backward, but dl_dzhat is [R,B,n] and every output is [R,B,...] or NULL (dQ[R,B,n,n], dp[R,B,n], ...):
+ * slot r holds exactly what lcpb200_backward returns for dl_dzhat[r]. Each scene's KKT matrix is factored once
+ * per chunk of cotangents, not once per cotangent; a scene's cotangents are split into chunks only to fill the GPU
+ * when B is small, and the results do not depend on that split. Flags, Rsave and LCPB200_BWD_REUSE_STRUCTURE as
+ * for lcpb200_backward, and the same kernel family serves each scene (fp32: condensed, the dual form for
+ * unstructured scenes; fp64: the dual form, the condensed kernel for scenes whose dual LU broke down;
+ * LCPB200_DUAL_BACKWARD=1: the dual form first for fp32 too). lcpb200_backward is this call with R = 1. */
+int lcpb200_backward_batched(lcpb200_handle_t h, int R, int B,
+                             const void* Q, const void* G, const void* A, const void* F,
+                             const void* zhat, const void* nu, const void* lam, const void* slack,
+                             const void* dl_dzhat,
+                             void* dQ, void* dp, void* dG, void* dh, void* dA, void* db, void* dF,
+                             const void* Rsave, unsigned flags, void* stream);
+
+/* lcpb200_jvp_batched: R >= 1 Jacobian-vector products of the same saved solves in one call -- the forward-mode
+ * derivative of zhat along R directions of (Q, p, G, h, A, b, F) (R = 1: one torch.func.jvp; R = k: the k columns
+ * of a jacfwd). Same inputs and saved solve as lcpb200_backward_batched; every tangent is [R,B,...] with the shape
+ * of its input (tQ[R,B,n,n], tp[R,B,n], tG[R,B,m,n], th[R,B,m], tA[R,B,e,n], tb[R,B,e], tF[R,B,m,m]) or NULL,
+ * which means zero and is not read. dz[R,B,n] receives the tangents of zhat. Each scene's KKT matrix K (not
+ * transposed) is factored once per chunk of tangents at the saved iterate, with each kernel family's d (the
+ * condensed kernel clamps d = lam / slack to [1e-10, 1e10] in fp64, the dual form does not), so the result is the
+ * transpose of the LCPB200_BWD_EXACT_ADJOINT backward: the true derivative of the solve. tQ enters as tQ zhat, as
+ * given: the backward returns the symmetrised dQ, so the two agree along symmetric tQ. Scenes are routed as in
+ * lcpb200_backward_batched. flags: 0 or LCPB200_BWD_REUSE_STRUCTURE. */
+int lcpb200_jvp_batched(lcpb200_handle_t h, int R, int B,
+                        const void* Q, const void* G, const void* A, const void* F,
+                        const void* zhat, const void* nu, const void* lam, const void* slack,
+                        const void* tQ, const void* tp, const void* tG, const void* th,
+                        const void* tA, const void* tb, const void* tF,
+                        void* dz, const void* Rsave, unsigned flags, void* stream);
 
 /* Same two calls with HOST buffers: copies in, solves, copies out. The timed
  * "e2e" path of bench.py. Synchronous on return. forward_host leaves its inputs,

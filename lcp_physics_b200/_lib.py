@@ -29,6 +29,8 @@ _SIGS = {
     "lcpb200_forward": (ctypes.c_int, [_vp, ctypes.c_int] + [_vp] * 7 +
                         [ctypes.c_double, ctypes.c_int, ctypes.c_int] + [_vp] * 9),
     "lcpb200_backward": (ctypes.c_int, [_vp, ctypes.c_int] + [_vp] * 17 + [ctypes.c_uint, _vp]),
+    "lcpb200_backward_batched": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int] + [_vp] * 17 + [ctypes.c_uint, _vp]),
+    "lcpb200_jvp_batched": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int] + [_vp] * 17 + [ctypes.c_uint, _vp]),
     "lcpb200_forward_host": (ctypes.c_int, [_vp, ctypes.c_int] + [_vp] * 7 +
                              [ctypes.c_double, ctypes.c_int, ctypes.c_int] + [_vp] * 7),
     "lcpb200_backward_host": (ctypes.c_int, [_vp, ctypes.c_int] + [_vp] * 16 + [ctypes.c_uint]),

@@ -22,8 +22,14 @@ cudaError_t launch_cond_backward_t<LCP_T, LCP_NS>(const CBwdArgs<LCP_T>& a, int 
 
 template <>
 cudaError_t launch_cond_jvp_t<LCP_T, LCP_NS>(const CJvpArgs<LCP_T>& a, int grid, cudaStream_t st) {
-  if (a.prof) cond_jvp_kernel<LCP_T, LCP_NS, true><<<grid, NT, a.P.smem_bytes, st>>>(a);
-  else cond_jvp_kernel<LCP_T, LCP_NS, false><<<grid, NT, a.P.smem_bytes, st>>>(a);
+  const bool dense = a.soa.mass == nullptr;
+  if (a.prof) {
+    if (dense) cond_jvp_kernel<LCP_T, LCP_NS, true, true><<<grid, NT, a.P.smem_bytes, st>>>(a);
+    else cond_jvp_kernel<LCP_T, LCP_NS, true, false><<<grid, NT, a.P.smem_bytes, st>>>(a);
+  } else {
+    if (dense) cond_jvp_kernel<LCP_T, LCP_NS, false, true><<<grid, NT, a.P.smem_bytes, st>>>(a);
+    else cond_jvp_kernel<LCP_T, LCP_NS, false, false><<<grid, NT, a.P.smem_bytes, st>>>(a);
+  }
   return cudaGetLastError();
 }
 
@@ -34,7 +40,8 @@ cudaError_t configure_cond_t<LCP_T, LCP_NS>(int smem_bytes, int dyn_max, int* oc
                         (const void*)cond_forward_kernel<LCP_T, LCP_NS, true>, (const void*)cond_backward_kernel<LCP_T, LCP_NS, true>};
   for (const void* f : fns)
     if ((e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max)) != cudaSuccess) return e;
-  const void* jvp[2] = {(const void*)cond_jvp_kernel<LCP_T, LCP_NS, false>, (const void*)cond_jvp_kernel<LCP_T, LCP_NS, true>};
+  const void* jvp[4] = {(const void*)cond_jvp_kernel<LCP_T, LCP_NS, false, false>, (const void*)cond_jvp_kernel<LCP_T, LCP_NS, true, false>,
+                        (const void*)cond_jvp_kernel<LCP_T, LCP_NS, false, true>, (const void*)cond_jvp_kernel<LCP_T, LCP_NS, true, true>};
   for (const void* f : jvp)
     if ((e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max)) != cudaSuccess) return e;
   // the grid is sized by the production kernels; the profiling ones run on the same grid

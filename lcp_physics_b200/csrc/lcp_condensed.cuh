@@ -1643,14 +1643,20 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
 // K the NON-transposed matrix the forward factors; the tangent of zhat is dx. d(Q, p, G, h, F) is the directional
 // derivative of the assembly (build_structure_soa), evaluated per contact and per dof, never as a dense matrix.
 // Every tangent is [R][B][...] like CBwdArgs' cotangents, nullptr = zero.
+// Dense inputs (soa.mass == nullptr): the structure comes from Q, G, A, F (or sload) as in cond_backward_kernel and
+// d(Q, p, G, h, F) are the dense tangents tQ ... tF; t_A, t_b serve both paths.
 template <typename T>
 struct CJvpArgs {
   CPlan P;
   int B, R, chunks;           // work items (scene, chunk of tangents), as CBwdArgs
-  const T* A;
+  const T *Q, *G, *A, *F;
   const T *zhat, *nu, *lam, *slack;
   EngineSoA<T> soa;
   const T *t_mass, *t_inertia, *t_v, *t_fext, *t_normal, *t_p1, *t_p2, *t_mu, *t_rest, *t_A, *t_b;
+  const T *tQ, *tp, *tG, *th, *tF;   // dense path: [R][B][...] or nullptr
+  int* done;                  // dense path, as CBwdArgs
+  const int* only;
+  const unsigned char* sload;
   T* dz;                      // [R][B][n]
   long long* prof;
 };
@@ -1759,9 +1765,41 @@ __device__ __noinline__ void jvp_rhs(const CJvpArgs<T>& a, CSmem<T> S, Struct st
   __syncthreads();
 }
 
+// Right-hand side of tangent slot so for dense inputs (CJvpArgs::tQ ... tF): r_x by columns (thread j walks column j
+// of tG and tA: coalesced, no atomics), r_z and r_y by rows.
+template <typename T>
+__device__ __noinline__ void jvp_rhs_dense(const CJvpArgs<T>& a, CSmem<T> S, Struct st, int sc, int so) {
+  const CPlan& P = a.P;
+  const int n = P.n, m = st.m, e = P.e, tid = threadIdx.x;
+  const T* zh = S.x(); const T* lm = S.z(); const T* nu = S.y();
+  const T* tQ = a.tQ ? a.tQ + (size_t)so * n * n : nullptr;
+  const T* tG = a.tG ? a.tG + (size_t)so * m * n : nullptr;
+  const T* tF = a.tF ? a.tF + (size_t)so * m * m : nullptr;
+  const T* tA = (a.t_A && e > 0) ? a.t_A + (size_t)so * e * n : nullptr;
+  for (int j = tid; j < n; j += NT) {
+    T acc = a.tp ? a.tp[(size_t)so * n + j] : T(0);
+    if (tQ) for (int i = 0; i < n; ++i) acc = fma(tQ[(size_t)j * n + i], zh[i], acc);
+    if (tG) for (int i = 0; i < m; ++i) acc = fma(tG[(size_t)i * n + j], lm[i], acc);
+    if (tA) for (int k = 0; k < e; ++k) acc = fma(tA[(size_t)k * n + j], nu[k], acc);
+    S.rx()[j] = acc;
+  }
+  for (int i = tid; i < m; i += NT) {
+    T acc = a.th ? -a.th[(size_t)so * m + i] : T(0);
+    if (tG) for (int j = 0; j < n; ++j) acc = fma(tG[(size_t)i * n + j], zh[j], acc);
+    if (tF) for (int k = 0; k < m; ++k) acc = fma(-tF[(size_t)i * m + k], lm[k], acc);
+    S.rz()[i] = acc;
+  }
+  for (int k = tid; k < e; k += NT) {
+    T acc = a.t_b ? -a.t_b[(size_t)so * e + k] : T(0);
+    if (tA) for (int j = 0; j < n; ++j) acc = fma(tA[(size_t)k * n + j], zh[j], acc);
+    S.ry()[k] = acc;
+  }
+  __syncthreads();
+}
+
 // One factorisation of K (not transposed) at the saved solution, then one right-hand side and one solve per
 // tangent r in [r0, r1). The prologue is backward_scene's, kept separate so that the backward's code is unchanged.
-template <typename T, int NS, int CS, typename PF>
+template <typename T, int NS, int CS, bool DENSE, typename PF>
 __device__ __forceinline__ void jvp_scene(const CJvpArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc,
                                           int r0, int r1) {
   const CPlan& P = a.P;
@@ -1780,16 +1818,19 @@ __device__ __forceinline__ void jvp_scene(const CJvpArgs<T>& a, CSmem<T>& S, con
   factor_kkt<T, NS, CS>(P, S, st, pf, false);
   for (int r = r0; r < r1; ++r) {
     const int so = r * a.B + sc;
-    jvp_rhs<T>(a, S, st, sc, so);
+    if constexpr (DENSE) jvp_rhs_dense<T>(a, S, st, sc, so);
+    else jvp_rhs<T>(a, S, st, sc, so);
     solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), S.rz(), e > 0 ? S.ry() : nullptr, S.dx(), S.ds(), S.dz(),
                          S.dy());
     for (int i = tid; i < n; i += NT) a.dz[(size_t)so * n + i] = S.dx()[i];
+    if (DENSE && tid == 0 && a.done) a.done[sc] = 1;
     __syncthreads();
     pf.lap(CPH_GRADS);
   }
 }
 
-template <typename T, int NS, bool PROF>
+// DENSE (soa.mass == nullptr): the dense branch, its own instantiation so that the engine's is compiled without it.
+template <typename T, int NS, bool PROF, bool DENSE>
 __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_jvp_kernel(const __grid_constant__ CJvpArgs<T> a) {
   const CPlan& P = a.P;
   CSmem<T> S(P);
@@ -1799,23 +1840,44 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_jvp_kernel(const _
   for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
     const int sc = w / a.chunks, k = w - sc * a.chunks;
     const int r0 = (int)((long long)a.R * k / a.chunks), r1 = (int)((long long)a.R * (k + 1) / a.chunks);
+    if (DENSE && a.only && !a.only[sc]) continue;
     if (tid == 0) singular_s = 0;
     __syncthreads();
     pf.start();
     Struct st;
-    const bool ok = build_structure_soa<T>(P, S, st, a.soa, sc, e > 0 ? a.A + (size_t)sc * e * n : nullptr, &singular_s);
+    const bool ok = !DENSE
+        ? build_structure_soa<T>(P, S, st, a.soa, sc, e > 0 ? a.A + (size_t)sc * e * n : nullptr, &singular_s)
+        : a.sload
+              ? load_structure(P, st, a.sload + (size_t)sc * P.sbytes)
+              : build_structure<T>(P, S, st, a.Q + (size_t)sc * n * n, a.G + (size_t)sc * P.m * n,
+                                   e > 0 ? a.A + (size_t)sc * e * n : nullptr, a.F + (size_t)sc * P.m * P.m, &singular_s);
     __syncthreads();
     pf.lap(CPH_STRUCT);
-    if (!ok) {                                    // the forward reported it (status -100 / -1): zero tangents
-      for (int r = r0; r < r1; ++r)
-        for (int i = tid; i < n; i += NT) a.dz[((size_t)r * a.B + sc) * n + i] = T(0);
+    if (!ok) {
+      if (!DENSE) {                               // the forward reported it (status -100 / -1): zero tangents
+        for (int r = r0; r < r1; ++r)
+          for (int i = tid; i < n; i += NT) a.dz[((size_t)r * a.B + sc) * n + i] = T(0);
+      } else if (tid == 0 && a.done) {
+        a.done[sc] = 0;                           // dense: left to the dual-form kernel
+      }
       __syncthreads();
       continue;
     }
     if constexpr (LU_BW < NS - 1) mark_band_lu<T>(P, S, st);
-    switch (st.cs) {
-      case 1: jvp_scene<T, NS, 1>(a, S, st, pf, sc, r0, r1); break;
-      default: jvp_scene<T, NS, 4>(a, S, st, pf, sc, r0, r1); break;   // the engine builds 1 (mode 1) or 4 rows
+    if constexpr (!DENSE) {
+      switch (st.cs) {
+        case 1: jvp_scene<T, NS, 1, false>(a, S, st, pf, sc, r0, r1); break;
+        default: jvp_scene<T, NS, 4, false>(a, S, st, pf, sc, r0, r1); break;   // the engine builds 1 (mode 1) or 4 rows
+      }
+    } else {
+      switch (st.cs) {                            // dense scenes: any component size, as in cond_backward_kernel
+        case 1: jvp_scene<T, NS, 1, true>(a, S, st, pf, sc, r0, r1); break;
+        case 2: jvp_scene<T, NS, 2, true>(a, S, st, pf, sc, r0, r1); break;
+        case 3: jvp_scene<T, NS, 3, true>(a, S, st, pf, sc, r0, r1); break;
+        case 4: jvp_scene<T, NS, 4, true>(a, S, st, pf, sc, r0, r1); break;
+        case 5: jvp_scene<T, NS, 5, true>(a, S, st, pf, sc, r0, r1); break;
+        default: jvp_scene<T, NS, 6, true>(a, S, st, pf, sc, r0, r1); break;
+      }
     }
     __syncthreads();
   }

@@ -8,7 +8,8 @@ namespace lcpb200 {
 
 template <typename T, int MODE> cudaError_t launch_forward_t(const FwdArgs<T>& a, int grid, cudaStream_t st);
 template <typename T, int MODE> cudaError_t launch_backward_t(const BwdArgs<T>& a, int grid, cudaStream_t st);
-// sets the dynamic shared memory limit of both kernels and returns min occupancy (CTAs / SM)
+template <typename T, int MODE> cudaError_t launch_jvp_t(const JvpArgs<T>& a, int grid, cudaStream_t st);
+// sets the dynamic shared memory limit of the three kernels and returns their min occupancy (CTAs / SM)
 template <typename T, int MODE> cudaError_t configure_t(int nt, int smem_bytes, int dyn_max, int* occ);
 
 }  // namespace lcpb200

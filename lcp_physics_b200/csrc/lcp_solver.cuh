@@ -964,6 +964,10 @@ template <typename T>
 struct BwdArgs {
   Plan P;
   int B;
+  // R cotangents per scene: g and every gradient output are [R][B][...], slot r of scene sc at row r B + sc.
+  // A work item is (scene, chunk): chunk k of `chunks` factors the scene's KKT matrix once and solves for the
+  // cotangents [R k / chunks, R (k + 1) / chunks).
+  int R, chunks;
   const T *Q, *G, *A, *F;
   const T *zhat, *nu, *lam, *slack, *g;
   T *dQ, *dp, *dG, *dh, *dA, *db, *dF;
@@ -972,8 +976,45 @@ struct BwdArgs {
   const T* Rsave;             // nullptr (recompute R) or the matrices saved by the forward pass
   long long* prof;
   const int* skip;            // nullptr or [B]: non-zero = gradients already written by lcp_condensed.cuh
-  int* bad;                   // nullptr or [B]: set to 1 when the solve produced non-finite dx / dlam (LU broke down)
+  int* bad;                   // nullptr or [B], zeroed by the caller: set to 1 when a solve of the scene produced
+                              // non-finite dx / dlam (LU broke down); the OR over its chunks and cotangents
 };
+
+// The saved iterate (zhat, lam, slack, nu) of scene sc into x, z, s, y, with d = lam / slack (:44, no clamp) and
+// rs2 = 0; then K (transposed for the exact adjoint) is factored once for every right-hand side of the work item.
+template <typename T, int MODE>
+__device__ __forceinline__ void factor_saved(SceneCtx<T, MODE>& c, const Plan& P, T* sm, int* flag, int sc,
+                                             const T* Q, const T* G, const T* A, const T* F, const T* zhat,
+                                             const T* nu, const T* lam_, const T* slack, const T* Rsave, bool transF) {
+  const int n = P.n, m = P.m, e = P.e, tid = threadIdx.x, NT = blockDim.x;
+  Vecs<T> v = c.vecs();
+  bind_scene(c, P, sm, Q + (size_t)sc * n * n, G + (size_t)sc * m * n, e > 0 ? A + (size_t)sc * e * n : nullptr,
+             F + (size_t)sc * m * m);
+  const T* zh = zhat + (size_t)sc * n;
+  const T* lam = lam_ + (size_t)sc * m;
+  const T* slk = slack + (size_t)sc * m;
+  const T* nus = e > 0 ? nu + (size_t)sc * e : nullptr;
+  c.transF = transF;                   // the saved R holds F, so it is not used for the transposed system
+  if (Rsave && !c.transF) { c.R = const_cast<T*>(Rsave) + (size_t)sc * m * m; c.Rsaved = true; }
+  prefactor(c, flag);                  // singular Q was already reported by the forward pass
+  prof_lap(c, PH_PREFACTOR);
+  for (int i = tid; i < n; i += NT) v.x[i] = zh[i];
+  for (int i = tid; i < m; i += NT) { v.z[i] = lam[i]; v.s[i] = slk[i]; v.d[i] = lam[i] / slk[i]; v.rs2[i] = T(0); }   // :44
+  for (int i = tid; i < e; i += NT) v.y[i] = nus[i];
+  __syncthreads();
+  factor_kkt(c);                                            // :46
+}
+
+// bad[sc] = 1 when the solve left a non-finite dx or dlam (the LU broke down); never cleared here.
+template <typename T>
+__device__ __forceinline__ void flag_nonfinite(int* bad, int sc, const T* dx, const T* dlam, int n, int m) {
+  const int tid = threadIdx.x, NT = blockDim.x;
+  int nf = 0;
+  for (int i = tid; i < n; i += NT) nf |= !isfinite((double)dx[i]);
+  for (int i = tid; i < m; i += NT) nf |= !isfinite((double)dlam[i]);
+  nf = __syncthreads_or(nf);
+  if (tid == 0 && nf) bad[sc] = 1;
+}
 
 template <typename T, int MODE>
 __global__ void __launch_bounds__(512, 1) lcp_backward_kernel(const BwdArgs<T> a) {
@@ -988,55 +1029,117 @@ __global__ void __launch_bounds__(512, 1) lcp_backward_kernel(const BwdArgs<T> a
   T* const sb = sm;
   auto off = [&](const T* p_) { return (int)(p_ - sb); };
 
-  for (int sc = blockIdx.x; sc < a.B; sc += gridDim.x) {
+  for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
+    const int sc = w / a.chunks, k = w - sc * a.chunks;
     if (a.skip && a.skip[sc]) continue;
     prof_start(c);
-    bind_scene(c, P, sm, a.Q + (size_t)sc * n * n, a.G + (size_t)sc * m * n,
-               e > 0 ? a.A + (size_t)sc * e * n : nullptr, a.F + (size_t)sc * m * m);
-    const T* zh = a.zhat + (size_t)sc * n;
-    const T* lam = a.lam + (size_t)sc * m;
-    const T* slk = a.slack + (size_t)sc * m;
-    const T* nu = e > 0 ? a.nu + (size_t)sc * e : nullptr;
-    c.transF = (a.flags & 1u) != 0;      // LCPB200_BWD_EXACT_ADJOINT (the saved R holds F, so it is not used then)
-    if (a.Rsave && !c.transF) { c.R = const_cast<T*>(a.Rsave) + (size_t)sc * m * m; c.Rsaved = true; }
-    prefactor(c, &flag);     // singular Q was already reported by the forward pass
-    prof_lap(c, PH_PREFACTOR);
-    for (int i = tid; i < n; i += NT) { v.x[i] = zh[i]; v.rx[i] = a.g[(size_t)sc * n + i]; }
-    for (int i = tid; i < m; i += NT) { v.z[i] = lam[i]; v.s[i] = slk[i]; v.d[i] = lam[i] / slk[i]; v.rs2[i] = T(0); }   // :44
-    for (int i = tid; i < e; i += NT) v.y[i] = nu[i];
-    __syncthreads();
-    factor_kkt(c);                                            // :46
-    solve_kkt(c, off(v.rx), off(v.rs2), -1, -1, off(v.dxa), off(v.dsa), off(v.dza), off(v.dya));   // :47-50
-    prof_lap(c, PH_SOLVE);
-    const T* dx = v.dxa; const T* dlam = v.dza; const T* dnu = v.dya;
-    if (a.bad) {
-      int nf = 0;
-      for (int i = tid; i < n; i += NT) nf |= !isfinite((double)dx[i]);
-      for (int i = tid; i < m; i += NT) nf |= !isfinite((double)dlam[i]);
-      nf = __syncthreads_or(nf);
-      if (tid == 0) a.bad[sc] = nf ? 1 : 0;
+    factor_saved(c, P, sm, &flag, sc, a.Q, a.G, a.A, a.F, a.zhat, a.nu, a.lam, a.slack, a.Rsave, (a.flags & 1u) != 0);
+    const int r0 = (int)((long long)a.R * k / a.chunks), r1 = (int)((long long)a.R * (k + 1) / a.chunks);
+    for (int r = r0; r < r1; ++r) {
+      const size_t so = (size_t)r * a.B + sc;                   // output row of (cotangent r, scene sc)
+      for (int i = tid; i < n; i += NT) v.rx[i] = a.g[so * n + i];
+      __syncthreads();
+      solve_kkt(c, off(v.rx), off(v.rs2), -1, -1, off(v.dxa), off(v.dsa), off(v.dza), off(v.dya));   // :47-50
+      prof_lap(c, PH_SOLVE);
+      const T* dx = v.dxa; const T* dlam = v.dza; const T* dnu = v.dya;
+      if (a.bad) flag_nonfinite(a.bad, sc, dx, dlam, n, m);
+      if (a.dp) for (int i = tid; i < n; i += NT) a.dp[so * n + i] = dx[i];                       // :52
+      if (a.dh) for (int i = tid; i < m; i += NT) a.dh[so * m + i] = -dlam[i];                    // :55
+      if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[so * e + i] = -dnu[i];            // :58
+      if (a.dG) {                                                    // :53  dlam (x) zhat + lam (x) dx
+        T* o = a.dG + so * m * n;
+        for (int t = tid; t < m * n; t += NT) { int i = t / n, j = t - i * n; o[t] = dlam[i] * v.x[j] + v.z[i] * dx[j]; }
+      }
+      if (a.dF) {                                                    // :54  -dlam (x) lam
+        T* o = a.dF + so * m * m;
+        for (int t = tid; t < m * m; t += NT) { int i = t / m, j = t - i * m; o[t] = -(dlam[i] * v.z[j]); }
+      }
+      if (a.dA && e > 0) {                                           // :57
+        T* o = a.dA + so * e * n;
+        for (int t = tid; t < e * n; t += NT) { int i = t / n, j = t - i * n; o[t] = dnu[i] * v.x[j] + v.y[i] * dx[j]; }
+      }
+      if (a.dQ) {                                                    // :61
+        T* o = a.dQ + so * n * n;
+        for (int t = tid; t < n * n; t += NT) { int i = t / n, j = t - i * n; o[t] = T(0.5) * (dx[i] * v.x[j] + v.x[i] * dx[j]); }
+      }
+      __syncthreads();
+      prof_lap(c, PH_STEP);
     }
-    if (a.dp) for (int i = tid; i < n; i += NT) a.dp[(size_t)sc * n + i] = dx[i];                       // :52
-    if (a.dh) for (int i = tid; i < m; i += NT) a.dh[(size_t)sc * m + i] = -dlam[i];                    // :55
-    if (a.db && e > 0) for (int i = tid; i < e; i += NT) a.db[(size_t)sc * e + i] = -dnu[i];            // :58
-    if (a.dG) {                                                    // :53  dlam (x) zhat + lam (x) dx
-      T* o = a.dG + (size_t)sc * m * n;
-      for (int t = tid; t < m * n; t += NT) { int i = t / n, j = t - i * n; o[t] = dlam[i] * v.x[j] + v.z[i] * dx[j]; }
+  }
+}
+
+// ------------------------------------------------------------------ Jacobian-vector products (dense inputs)
+// Forward-mode derivative of the solve (DESIGN.md section 8, dense path). At the saved iterate, with d = lam / slack
+// unclamped as in the backward, the PDIPM residuals (pdipm.py:82-90) linearised in the inputs give
+//     K [dx; ds; dz; dy] = -(r_x, 0, r_z, r_y),
+//     r_x = tQ zhat + tp + tG^T lam + tA^T nu,   r_z = tG zhat - tF lam - th,   r_y = tA zhat - tb,
+// K the NON-transposed matrix the forward factors; the tangent of zhat is dx. Every tangent is [R][B][...] with the
+// shape of its input, nullptr = zero; work items are (scene, chunk of tangents) as in BwdArgs.
+template <typename T>
+struct JvpArgs {
+  Plan P;
+  int B, R, chunks;
+  const T *Q, *G, *A, *F;
+  const T *zhat, *nu, *lam, *slack;
+  const T *tQ, *tp, *tG, *th, *tA, *tb, *tF;
+  T* dz;                      // [R][B][n]
+  T* ws;
+  const T* Rsave;
+  long long* prof;
+  const int* skip;            // as BwdArgs
+  int* bad;
+};
+
+template <typename T, int MODE>
+__global__ void __launch_bounds__(512, 1) lcp_jvp_kernel(const JvpArgs<T> a) {
+  T* sm = smem_base<T>();
+  __shared__ int flag;
+  __shared__ int lu_flag_s;
+  const Plan& P = a.P;
+  const int n = P.n, m = P.m, e = P.e, tid = threadIdx.x, NT = blockDim.x;
+  SceneCtx<T, MODE> c;
+  setup_ctx<T, MODE>(c, P, sm, a.ws + (size_t)blockIdx.x * P.ws_per_cta, &lu_flag_s, a.prof);
+  Vecs<T> v = c.vecs();
+  T* const sb = sm;
+  auto off = [&](const T* p_) { return (int)(p_ - sb); };
+
+  for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
+    const int sc = w / a.chunks, k = w - sc * a.chunks;
+    if (a.skip && a.skip[sc]) continue;
+    prof_start(c);
+    factor_saved(c, P, sm, &flag, sc, a.Q, a.G, a.A, a.F, a.zhat, a.nu, a.lam, a.slack, a.Rsave, false);
+    const int r0 = (int)((long long)a.R * k / a.chunks), r1 = (int)((long long)a.R * (k + 1) / a.chunks);
+    for (int r = r0; r < r1; ++r) {
+      const size_t so = (size_t)r * a.B + sc;
+      const T* tQ = a.tQ ? a.tQ + so * n * n : nullptr;
+      const T* tG = a.tG ? a.tG + so * m * n : nullptr;
+      const T* tF = a.tF ? a.tF + so * m * m : nullptr;
+      const T* tA = (a.tA && e > 0) ? a.tA + so * e * n : nullptr;
+      // row products first (one warp per row), then the column sums: thread j walks column j of tG and tA
+      if (tQ) gemv_rows_v(tQ, n, n, n, v.x, [&](int i, T acc) { v.rx[i] = acc; });
+      else { for (int i = tid; i < n; i += NT) v.rx[i] = T(0); }
+      // r_z: each row is written by one GEMV epilogue at a time (gemv_rows_v syncs at its end, not at its start)
+      if (tG) gemv_rows_v(tG, n, m, n, v.x, [&](int i, T acc) { v.rz[i] = acc; });
+      if (tF) gemv_rows_v(tF, m, m, m, v.z, [&](int i, T acc) { v.rz[i] = (tG ? v.rz[i] : T(0)) - acc; });
+      if (!tG && !tF) { for (int i = tid; i < m; i += NT) v.rz[i] = T(0); }
+      if (tA) gemv_rows_v(tA, n, e, n, v.x, [&](int i, T acc) { v.ry[i] = acc; });
+      else { for (int i = tid; i < e; i += NT) v.ry[i] = T(0); }
+      __syncthreads();
+      for (int j = tid; j < n; j += NT) {
+        T acc = a.tp ? a.tp[so * n + j] : T(0);
+        if (tG) for (int i = 0; i < m; ++i) acc = fma(tG[(size_t)i * n + j], v.z[i], acc);
+        if (tA) for (int i = 0; i < e; ++i) acc = fma(tA[(size_t)i * n + j], v.y[i], acc);
+        v.rx[j] += acc;
+      }
+      if (a.th) for (int i = tid; i < m; i += NT) v.rz[i] -= a.th[so * m + i];
+      if (a.tb && e > 0) for (int i = tid; i < e; i += NT) v.ry[i] -= a.tb[so * e + i];
+      __syncthreads();
+      solve_kkt(c, off(v.rx), off(v.rs2), off(v.rz), e > 0 ? off(v.ry) : -1, off(v.dxa), off(v.dsa), off(v.dza), off(v.dya));
+      prof_lap(c, PH_SOLVE);
+      if (a.bad) flag_nonfinite(a.bad, sc, v.dxa, v.dza, n, m);
+      for (int i = tid; i < n; i += NT) a.dz[so * n + i] = v.dxa[i];
+      __syncthreads();
     }
-    if (a.dF) {                                                    // :54  -dlam (x) lam
-      T* o = a.dF + (size_t)sc * m * m;
-      for (int t = tid; t < m * m; t += NT) { int i = t / m, j = t - i * m; o[t] = -(dlam[i] * v.z[j]); }
-    }
-    if (a.dA && e > 0) {                                           // :57
-      T* o = a.dA + (size_t)sc * e * n;
-      for (int t = tid; t < e * n; t += NT) { int i = t / n, j = t - i * n; o[t] = dnu[i] * v.x[j] + v.y[i] * dx[j]; }
-    }
-    if (a.dQ) {                                                    // :61
-      T* o = a.dQ + (size_t)sc * n * n;
-      for (int t = tid; t < n * n; t += NT) { int i = t / n, j = t - i * n; o[t] = T(0.5) * (dx[i] * v.x[j] + v.x[i] * dx[j]); }
-    }
-    __syncthreads();
-    prof_lap(c, PH_STEP);
   }
 }
 

@@ -365,70 +365,153 @@ static int launch_forward(lcpb200_handle_s* h, int slot, int B, const void* Q, c
   return 0;
 }
 
+// Work items per scene of a call with R cotangents or tangents: enough (scene, chunk) items to fill `target` CTAs,
+// each of which factors its scene once; never more chunks than right-hand sides.
+static int bwd_chunks(int R, int B, int target) {
+  return std::max(1, std::min(R, (target + B - 1) / B));
+}
+
+// Scene routing shared by the dense backward and JVP. fp32: condensed-KKT kernel first, the dual form only for the
+// scenes it flags as unstructured. fp64: the dual form first -- at the fp64 round-off floor (lambda, s ~ 1e-16,
+// d = lambda/s spanning 1e+-16) the condensed matrix loses dx (DESIGN.md "Parity") -- and the condensed kernel only
+// as a rescue for scenes on which the dual LU (pivoting restricted to its diagonal blocks) broke down (non-finite
+// dx). LCPB200_DUAL_BACKWARD=1 puts the dual form first for fp32 too.
+struct Route {
+  bool have_cond, cond_first;
+  int* flagbuf;              // [B]: the condensed kernel's done verdicts, or the dual form's bad flags
+  int cchunks, cgrid;        // condensed work items and grid
+  int dchunks, dgrid;        // dual-form work items and grid (the workspace is per CTA)
+};
+
 template <typename T>
-static int launch_backward(lcpb200_handle_s* h, int slot, int B, const void* Q, const void* G, const void* A,
+static int make_route(lcpb200_handle_s* h, int slot, int R, int B, cudaStream_t st, Route& r) {
+  r.have_cond = h->cplan.ok != 0;
+  r.cond_first = r.have_cond && sizeof(T) == 4 && !getenv("LCPB200_DUAL_BACKWARD");
+  r.flagbuf = nullptr;
+  if (r.have_cond) {
+    CK(h->d_flag[slot].ensure(sizeof(int) * (size_t)B));
+    r.flagbuf = (int*)h->d_flag[slot].p;
+    // the dual form's bad flags are an OR over a scene's chunks and right-hand sides: start from 0
+    if (!r.cond_first) CK(cudaMemsetAsync(r.flagbuf, 0, sizeof(int) * (size_t)B, st));
+  }
+  r.cchunks = bwd_chunks(R, B, h->cond_grid);
+  r.cgrid = (int)std::min((long long)B * r.cchunks, (long long)std::max(h->cond_grid, 1));
+  r.dchunks = bwd_chunks(R, B, h->max_grid);
+  if (int rc = ensure_ws(h, B * r.dchunks)) return rc;
+  r.dgrid = (int)std::min((long long)B * r.dchunks, (long long)h->ws_ctas);
+  return 0;
+}
+
+template <typename T>
+static int launch_backward(lcpb200_handle_s* h, int slot, int R, int B, const void* Q, const void* G, const void* A,
                            const void* F, const void* zhat, const void* nu, const void* lam, const void* slack,
                            const void* g, void* dQ, void* dp, void* dG, void* dh, void* dA, void* db, void* dF,
                            const void* Rsave, unsigned flags, cudaStream_t st, const unsigned char* sload = nullptr) {
-  // fp32: condensed-KKT backward first, the dual form only for the scenes it flags as unstructured.
-  // fp64: the dual form first -- at the fp64 round-off floor (lambda, s ~ 1e-16, d = lambda/s spanning
-  // 1e+-16) the condensed matrix loses dx (DESIGN.md "Parity") -- and the condensed kernel only as a rescue
-  // for scenes on which the dual LU (pivoting restricted to its diagonal blocks) broke down (non-finite dx).
-  const bool have_cond = h->cplan.ok != 0;
-  const bool cond_first = have_cond && sizeof(T) == 4 && !getenv("LCPB200_DUAL_BACKWARD");
-  int* flagbuf = nullptr;
-  if (have_cond) {
-    CK(h->d_flag[slot].ensure(sizeof(int) * (size_t)B));
-    flagbuf = (int*)h->d_flag[slot].p;
-  }
+  Route rt;
+  if (int rc = make_route<T>(h, slot, R, B, st, rt)) return rc;
   cnd::CBwdArgs<T> c;
-  if (have_cond) {
+  if (rt.have_cond) {
     c.P = h->cplan;
     c.B = B;
-    c.R = 1; c.chunks = 1;
+    c.R = R; c.chunks = rt.cchunks;
     c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
     c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
     c.g = (const T*)g;
     c.dQ = (T*)dQ; c.dp = (T*)dp; c.dG = (T*)dG; c.dh = (T*)dh; c.dA = (T*)dA; c.db = (T*)db; c.dF = (T*)dF;
-    c.done = cond_first ? flagbuf : nullptr;
-    c.only = cond_first ? nullptr : flagbuf;
+    c.done = rt.cond_first ? rt.flagbuf : nullptr;
+    c.only = rt.cond_first ? nullptr : rt.flagbuf;
     c.flags = flags;
     c.sload = sload;
     memset(&c.soa, 0, sizeof(c.soa));
     c.dmass = c.dinertia = c.dv = c.dfext = c.dnormal = c.dp1 = c.dp2 = c.dmu = c.drest = nullptr;
     c.prof = h->cprof ? h->cprof + (size_t)slot * h->cond_grid * cnd::CPH_COUNT : nullptr;
   }
-  const int cgrid = std::min(B, std::max(h->cond_grid, 1));
-  if (cond_first) {
-#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, cgrid, st)
+  if (rt.cond_first) {
+#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, rt.cgrid, st)
     const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
 #undef CALL_BWD
     CK(ce);
   }
-  if (int rc = ensure_ws(h, B)) return rc;
   BwdArgs<T> a;
   a.P = h->plan;
   a.B = B;
+  a.R = R; a.chunks = rt.dchunks;
   a.Q = (const T*)Q; a.G = (const T*)G; a.A = (const T*)A; a.F = (const T*)F;
   a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
   a.g = (const T*)g;
   a.dQ = (T*)dQ; a.dp = (T*)dp; a.dG = (T*)dG; a.dh = (T*)dh; a.dA = (T*)dA; a.db = (T*)db; a.dF = (T*)dF;
   a.flags = flags;
-  a.Rsave = have_cond ? nullptr : (const T*)Rsave;    // R is only formed when the forward ran on the dual form
-  a.skip = cond_first ? flagbuf : nullptr;
-  a.bad = (have_cond && !cond_first) ? flagbuf : nullptr;
+  a.Rsave = rt.have_cond ? nullptr : (const T*)Rsave;    // R is only formed when the forward ran on the dual form
+  a.skip = rt.cond_first ? rt.flagbuf : nullptr;
+  a.bad = (rt.have_cond && !rt.cond_first) ? rt.flagbuf : nullptr;
   a.ws = (T*)h->ws + (size_t)slot * h->plan.ws_per_cta * h->ws_ctas;
   a.prof = h->prof ? h->prof + (size_t)slot * h->max_grid * PH_COUNT : nullptr;
-  const int grid = std::min(B, h->ws_ctas);
   const int mode = h->plan.mode;
-  const cudaError_t le = mode == 0   ? launch_backward_t<T, 0>(a, grid, st)
-                         : mode == 1 ? launch_backward_t<T, 1>(a, grid, st)
-                                     : launch_backward_t<T, 2>(a, grid, st);
+  const cudaError_t le = mode == 0   ? launch_backward_t<T, 0>(a, rt.dgrid, st)
+                         : mode == 1 ? launch_backward_t<T, 1>(a, rt.dgrid, st)
+                                     : launch_backward_t<T, 2>(a, rt.dgrid, st);
   CK(le);
-  if (have_cond && !cond_first) {
-#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, cgrid, st)
+  if (rt.have_cond && !rt.cond_first) {
+#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, rt.cgrid, st)
     const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
 #undef CALL_BWD
+    CK(ce);
+  }
+  return 0;
+}
+
+// tg: tangents of (Q, p, G, h, A, b, F), each [R,B,...] or nullptr
+template <typename T>
+static int launch_jvp(lcpb200_handle_s* h, int R, int B, const void* Q, const void* G, const void* A, const void* F,
+                      const void* zhat, const void* nu, const void* lam, const void* slack, const void* const (&tg)[7],
+                      void* dz, const void* Rsave, cudaStream_t st, const unsigned char* sload) {
+  Route rt;
+  if (int rc = make_route<T>(h, 0, R, B, st, rt)) return rc;
+  cnd::CJvpArgs<T> c;
+  if (rt.have_cond) {
+    memset(&c, 0, sizeof(c));
+    c.P = h->cplan;
+    c.B = B;
+    c.R = R; c.chunks = rt.cchunks;
+    c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
+    c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
+    c.tQ = (const T*)tg[0]; c.tp = (const T*)tg[1]; c.tG = (const T*)tg[2]; c.th = (const T*)tg[3];
+    c.t_A = (const T*)tg[4]; c.t_b = (const T*)tg[5]; c.tF = (const T*)tg[6];
+    c.done = rt.cond_first ? rt.flagbuf : nullptr;
+    c.only = rt.cond_first ? nullptr : rt.flagbuf;
+    c.sload = sload;
+    c.dz = (T*)dz;
+    c.prof = h->cprof;
+  }
+  if (rt.cond_first) {
+#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, rt.cgrid, st)
+    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
+#undef CALL_JVP
+    CK(ce);
+  }
+  JvpArgs<T> a;
+  a.P = h->plan;
+  a.B = B;
+  a.R = R; a.chunks = rt.dchunks;
+  a.Q = (const T*)Q; a.G = (const T*)G; a.A = (const T*)A; a.F = (const T*)F;
+  a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
+  a.tQ = (const T*)tg[0]; a.tp = (const T*)tg[1]; a.tG = (const T*)tg[2]; a.th = (const T*)tg[3];
+  a.tA = (const T*)tg[4]; a.tb = (const T*)tg[5]; a.tF = (const T*)tg[6];
+  a.dz = (T*)dz;
+  a.Rsave = rt.have_cond ? nullptr : (const T*)Rsave;
+  a.skip = rt.cond_first ? rt.flagbuf : nullptr;
+  a.bad = (rt.have_cond && !rt.cond_first) ? rt.flagbuf : nullptr;
+  a.ws = (T*)h->ws;
+  a.prof = h->prof;
+  const int mode = h->plan.mode;
+  const cudaError_t le = mode == 0   ? launch_jvp_t<T, 0>(a, rt.dgrid, st)
+                         : mode == 1 ? launch_jvp_t<T, 1>(a, rt.dgrid, st)
+                                     : launch_jvp_t<T, 2>(a, rt.dgrid, st);
+  CK(le);
+  if (rt.have_cond && !rt.cond_first) {
+#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, rt.cgrid, st)
+    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
+#undef CALL_JVP
     CK(ce);
   }
   return 0;
@@ -475,29 +558,69 @@ extern "C" int lcpb200_forward(lcpb200_handle_t h, int B, const void* Q, const v
   return rc;
 }
 
-extern "C" int lcpb200_backward(lcpb200_handle_t h, int B, const void* Q, const void* G, const void* A,
-                                const void* F, const void* zhat, const void* nu, const void* lam,
-                                const void* slack, const void* g, void* dQ, void* dp, void* dG, void* dh, void* dA,
-                                void* db, void* dF, const void* Rsave, unsigned flags, void* stream) {
+static int check_dense_derivative(lcpb200_handle_t h, int R, int B, const void* Q, const void* G, const void* F,
+                                  const void* A, const void* zhat, const void* nu, const void* lam, const void* slack) {
   if (!h) return fail("null handle");
   if (!h->dual_ok) return fail("this handle serves the engine entry points only (problem too large for the dense API)");
+  if (R < 1) return fail("need R >= 1");
   if (B < 0) return fail("B < 0");
-  if (!Q || !G || !F || !zhat || !lam || !slack || !g) return fail("Q, G, F, zhat, lam, slack, dl_dzhat must be non-NULL");
+  if ((long long)R * B > INT_MAX) return fail("R * B exceeds INT_MAX");
+  if (!Q || !G || !F || !zhat || !lam || !slack) return fail("Q, G, F, zhat, lam, slack must be non-NULL");
   if (h->e > 0 && (!A || !nu)) return fail("A and nu must be non-NULL when e > 0");
+  return 0;
+}
+
+// LCPB200_BWD_REUSE_STRUCTURE: the caller states that (Q, G, A, F) are the inputs of the last lcpb200_forward on
+// this handle; ignored when nothing (or another batch size) was saved
+static const unsigned char* saved_structure(const lcpb200_handle_s* h, int B, unsigned flags) {
+  return ((flags & LCPB200_BWD_REUSE_STRUCTURE) && h->cplan.ok && h->struct_B == B) ? (const unsigned char*)h->d_struct.p
+                                                                                      : nullptr;
+}
+
+extern "C" int lcpb200_backward_batched(lcpb200_handle_t h, int R, int B, const void* Q, const void* G, const void* A,
+                                        const void* F, const void* zhat, const void* nu, const void* lam,
+                                        const void* slack, const void* g, void* dQ, void* dp, void* dG, void* dh,
+                                        void* dA, void* db, void* dF, const void* Rsave, unsigned flags, void* stream) {
+  if (int rc = check_dense_derivative(h, R, B, Q, G, F, A, zhat, nu, lam, slack)) return rc;
+  if (!g) return fail("dl_dzhat must be non-NULL");
   if (flags & ~(LCPB200_BWD_EXACT_ADJOINT | LCPB200_BWD_REUSE_STRUCTURE))
     return fail("flags: LCPB200_BWD_EXACT_ADJOINT | LCPB200_BWD_REUSE_STRUCTURE are the defined bits");
   if (B == 0) return 0;
   DeviceGuard dg_;
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
-  // LCPB200_BWD_REUSE_STRUCTURE: the caller states that (Q, G, A, F) are the inputs of the last lcpb200_forward on
-  // this handle; ignored when nothing (or another batch size) was saved
-  const unsigned char* sload = ((flags & LCPB200_BWD_REUSE_STRUCTURE) && h->cplan.ok && h->struct_B == B)
-                                   ? (const unsigned char*)h->d_struct.p : nullptr;
+  const unsigned char* sload = saved_structure(h, B, flags);
   const unsigned kf = flags & LCPB200_BWD_EXACT_ADJOINT;
   return h->dtype == LCPB200_F32
-             ? launch_backward<float>(h, 0, B, Q, G, A, F, zhat, nu, lam, slack, g, dQ, dp, dG, dh, dA, db, dF, Rsave, kf, st, sload)
-             : launch_backward<double>(h, 0, B, Q, G, A, F, zhat, nu, lam, slack, g, dQ, dp, dG, dh, dA, db, dF, Rsave, kf, st, sload);
+             ? launch_backward<float>(h, 0, R, B, Q, G, A, F, zhat, nu, lam, slack, g, dQ, dp, dG, dh, dA, db, dF, Rsave, kf, st, sload)
+             : launch_backward<double>(h, 0, R, B, Q, G, A, F, zhat, nu, lam, slack, g, dQ, dp, dG, dh, dA, db, dF, Rsave, kf, st, sload);
+}
+
+extern "C" int lcpb200_backward(lcpb200_handle_t h, int B, const void* Q, const void* G, const void* A,
+                                const void* F, const void* zhat, const void* nu, const void* lam,
+                                const void* slack, const void* g, void* dQ, void* dp, void* dG, void* dh, void* dA,
+                                void* db, void* dF, const void* Rsave, unsigned flags, void* stream) {
+  return lcpb200_backward_batched(h, 1, B, Q, G, A, F, zhat, nu, lam, slack, g, dQ, dp, dG, dh, dA, db, dF, Rsave,
+                                  flags, stream);
+}
+
+extern "C" int lcpb200_jvp_batched(lcpb200_handle_t h, int R, int B, const void* Q, const void* G, const void* A,
+                                   const void* F, const void* zhat, const void* nu, const void* lam, const void* slack,
+                                   const void* tQ, const void* tp, const void* tG, const void* th, const void* tA,
+                                   const void* tb, const void* tF, void* dz, const void* Rsave, unsigned flags,
+                                   void* stream) {
+  if (int rc = check_dense_derivative(h, R, B, Q, G, F, A, zhat, nu, lam, slack)) return rc;
+  if (!dz) return fail("dz must be non-NULL");
+  if (flags & ~LCPB200_BWD_REUSE_STRUCTURE) return fail("flags: LCPB200_BWD_REUSE_STRUCTURE is the only defined bit");
+  if (B == 0) return 0;
+  DeviceGuard dg_;
+  CK(dg_.set(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const void* const tg[7] = {tQ, tp, tG, th, h->e > 0 ? tA : nullptr, h->e > 0 ? tb : nullptr, tF};
+  const unsigned char* sload = saved_structure(h, B, flags);
+  return h->dtype == LCPB200_F32
+             ? launch_jvp<float>(h, R, B, Q, G, A, F, zhat, nu, lam, slack, tg, dz, Rsave, st, sload)
+             : launch_jvp<double>(h, R, B, Q, G, A, F, zhat, nu, lam, slack, tg, dz, Rsave, st, sload);
 }
 
 extern "C" int lcpb200_profile(lcpb200_handle_t h, int enable, long long* out) {
@@ -669,9 +792,9 @@ extern "C" int lcpb200_backward_host(lcpb200_handle_t h, int B, const void* Q, c
     const void* rs = (retained && h->retained_R) ? (const char*)h->d_R.p + m * m * w * s0 : nullptr;
     auto ao = [&](int i) -> void* { return (out_sz[i] && out_dst[i]) ? (char*)out_buf[i]->p + out_sz[i] * s0 : nullptr; };
     int rc = h->dtype == LCPB200_F32
-                 ? launch_backward<float>(h, slot, cb, ai(0), ai(1), ai(2), ai(3), ai(4), ai(5), ai(6), ai(7), ai(8),
+                 ? launch_backward<float>(h, slot, 1, cb, ai(0), ai(1), ai(2), ai(3), ai(4), ai(5), ai(6), ai(7), ai(8),
                                           ao(0), ao(1), ao(2), ao(3), ao(4), ao(5), ao(6), rs, flags, st)
-                 : launch_backward<double>(h, slot, cb, ai(0), ai(1), ai(2), ai(3), ai(4), ai(5), ai(6), ai(7), ai(8),
+                 : launch_backward<double>(h, slot, 1, cb, ai(0), ai(1), ai(2), ai(3), ai(4), ai(5), ai(6), ai(7), ai(8),
                                            ao(0), ao(1), ao(2), ao(3), ao(4), ao(5), ao(6), rs, flags, st);
     if (rc) return rc;
     for (int i = 0; i < 7; ++i)
@@ -818,12 +941,6 @@ extern "C" int lcpb200_engine_forward(lcpb200_handle_t h, int B, int nb, int nc,
                                         iters, resid, st);
 }
 
-// Work items per scene of a backward with R cotangents: enough (scene, chunk) items to fill `target` CTAs, each of
-// which factors its scene once; never more chunks than cotangents.
-static int bwd_chunks(int R, int B, int target) {
-  return std::max(1, std::min(R, (target + B - 1) / B));
-}
-
 template <typename T>
 static int engine_backward_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int mode, double dt, const void* mass,
                              const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
@@ -919,6 +1036,7 @@ static int engine_jvp_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int m
                         const void* slack, const void* const (&tg)[11], void* dz, cudaStream_t st) {
   CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
   cnd::CJvpArgs<T> c;
+  memset(&c, 0, sizeof(c));              // the dense-path fields (Q, G, F, tQ ... tF, done, only, sload) stay NULL
   c.P = h->cplan;
   c.B = B;
   c.R = R; c.chunks = bwd_chunks(R, B, h->cond_grid);

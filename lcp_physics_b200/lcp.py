@@ -158,34 +158,198 @@ def solve_backward(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need=(True,) * 7,
     return tuple(outs)
 
 
-class _LCPFn(torch.autograd.Function):
+def _to_device(ts, dev):
+    return [None if t is None else t.to(dev) for t in ts]
+
+
+def _device_call(dev):
+    """(device to run on, device the results go back to): CPU inputs run on the current CUDA device."""
+    if dev.type == "cuda":
+        return dev, dev
+    return torch.device("cuda", torch.cuda.current_device()), dev
+
+
+def _reuse_flag(saved, hd, B):
+    tok = saved.get("struct") if saved else None
+    return 2 if (tok is not None and tok[0] is hd and tok[1] == hd.fwd_generation and tok[2] == B) else 0
+
+
+def solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need=(True,) * 7, saved=None,
+                           exact_adjoint=False):
+    """lcpb200_backward_batched: dl_dzhat [..., B, n] -> (dQ, dp, dG, dh, dA, db, dF), each with dl_dzhat's leading
+    dims in front; entries not needed (or dA/db when e == 0) are None. The leading dims are the R cotangents of one
+    call: each scene's KKT matrix is factored once for all of them. Slot r equals solve_backward(dl_dzhat[r]).
+    CPU inputs are copied to the current CUDA device and the gradients copied back."""
+    _lib.require_cuda()
+    lib = _lib.load()
+    B, m, n = G.shape
+    e = A.shape[1] if (A is not None and A.dim() > 1) else 0
+    dtype = G.dtype
+    run, home = _device_call(G.device)
+    lead = tuple(dl_dzhat.shape[:-2])
+    R = 1
+    for d in lead:
+        R *= d
+    shapes = [(n, n), (n,), (m, n), (m,), (e, n), (e,), (m, m)]
+    outs = [torch.empty((R, B) + s, dtype=dtype, device=run) if (need[k] and not (k in (4, 5) and e == 0)) else None
+            for k, s in enumerate(shapes)]
+    if R > 0 and B > 0:
+        ins = _to_device([Q, G, A if e > 0 else None, F, zhat, nu if e > 0 else None, lam, slack], run)
+        ins = [None if t is None else t.contiguous() for t in ins]
+        g = dl_dzhat.to(device=run, dtype=dtype).reshape(R, B, n).contiguous()
+        hd = _lib.get_handle(dtype, n, m, e, run.index, torch.cuda.current_stream(run).cuda_stream)
+        flags = (1 if exact_adjoint else 0) | (_reuse_flag(saved, hd, B) if home.type == "cuda" else 0)
+        with torch.cuda.device(run):
+            _lib.check(lib.lcpb200_backward_batched(hd.raw, R, B, *[_lib.ptr(t) for t in ins], _lib.ptr(g),
+                                                    *[_lib.ptr(t) for t in outs], None, flags, _stream_ptr(run)))
+    return tuple(None if t is None else t.to(home).reshape(lead + tuple(t.shape[1:])) for t in outs)
+
+
+def solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, tangents, saved=None):
+    """lcpb200_jvp_batched: tangents of (Q, p, G, h, A, b, F), each [..., *input shape] or None (zero), -> the
+    tangent of zhat [..., B, n]. The leading dims, the same for every tangent, are the R directions of one call:
+    each scene's KKT matrix is factored once for all of them. tQ enters as tQ zhat, as given (the backward's dQ is
+    symmetrised: the two agree along symmetric tQ). CPU inputs run on the current CUDA device."""
+    _lib.require_cuda()
+    lib = _lib.load()
+    B, m, n = G.shape
+    e = A.shape[1] if (A is not None and A.dim() > 1) else 0
+    dtype = G.dtype
+    run, home = _device_call(G.device)
+    shapes = [(B, n, n), (B, n), (B, m, n), (B, m), (B, e, n), (B, e), (B, m, m)]
+    if e == 0:
+        tangents = list(tangents[:4]) + [None, None] + [tangents[6]]
+    lead = next((tuple(t.shape[:t.dim() - len(s)]) for t, s in zip(tangents, shapes) if t is not None), ())
+    R = 1
+    for d in lead:
+        R *= d
+    ts = [None if t is None else t.to(device=run, dtype=dtype).reshape((R,) + s).contiguous()
+          for t, s in zip(tangents, shapes)]
+    dz = torch.zeros((R, B, n), dtype=dtype, device=run)
+    if R > 0 and B > 0 and any(t is not None for t in ts):
+        ins = _to_device([Q, G, A if e > 0 else None, F, zhat, nu if e > 0 else None, lam, slack], run)
+        ins = [None if t is None else t.contiguous() for t in ins]
+        hd = _lib.get_handle(dtype, n, m, e, run.index, torch.cuda.current_stream(run).cuda_stream)
+        flags = _reuse_flag(saved, hd, B) if home.type == "cuda" else 0
+        with torch.cuda.device(run):
+            _lib.check(lib.lcpb200_jvp_batched(hd.raw, R, B, *[_lib.ptr(t) for t in ins], *[_lib.ptr(t) for t in ts],
+                                               _lib.ptr(dz), None, flags, _stream_ptr(run)))
+    return dz.to(home).reshape(lead + (B, n))
+
+
+_SECOND = "LCPFunction: second derivatives are not implemented"
+_BATCHED_PRIMAL = ("LCPFunction: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
+                   "instead (vmap of its vector-Jacobian and Jacobian-vector products -- jacrev, jacfwd -- is supported)")
+
+
+class _LCPVjpFn(torch.autograd.Function):
+    """The vector-Jacobian product of LCPFunction: dl/dzhat and the saved solve in, the seven gradients out. One
+    cotangent [B, n] is today's backward (solve_backward); under torch.func.vmap (vmap of a torch.func.vjp, jacrev)
+    the cotangents of every vmapped call arrive together and go to ONE lcpb200_backward_batched call."""
+
     @staticmethod
-    def forward(ctx, Q, p, G, h, A, b, F, opts):
-        need_bwd = any(ctx.needs_input_grad[:7])
-        ctx.saved_state = {} if need_bwd else None
+    def forward(dzhat, meta, *saved):
+        need, state, exact = meta
+        zhat, Q, G, A, F, nu, lam, slack = saved
+        if dzhat.dim() == 2:
+            return solve_backward(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
+        return solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError(_SECOND)
+
+    @staticmethod
+    def vmap(info, in_dims, dzhat, meta, *saved):
+        if any(d is not None for d in in_dims[2:]):
+            raise NotImplementedError(_BATCHED_PRIMAL)
+        # one more leading cotangent dim; apply (not forward) so that an enclosing vmap level batches it again
+        outs = _LCPVjpFn.apply(dzhat.movedim(in_dims[0], 0), meta, *saved)
+        return outs, tuple(None if t is None else 0 for t in outs)
+
+
+class _LCPJvpFn(torch.autograd.Function):
+    """The Jacobian-vector product of LCPFunction: tangents of (Q, p, G, h, A, b, F) and the saved solve in, the
+    tangent of zhat out. Under torch.func.vmap (jacfwd, vmap of a torch.func.jvp) the tangents of every vmapped call
+    arrive together and go to ONE lcpb200_jvp_batched call."""
+
+    @staticmethod
+    def forward(state, *args):
+        zhat, Q, G, A, F, nu, lam, slack = args[7:]
+        return solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, args[:7], saved=state)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError(_SECOND)
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise NotImplementedError(_SECOND)
+
+    @staticmethod
+    def vmap(info, in_dims, state, *args):
+        if any(d is not None for d in in_dims[8:]):
+            raise NotImplementedError(_BATCHED_PRIMAL)
+        # one more leading tangent dim; a tangent this level does not batch is the same for every direction
+        ts = [None if t is None else (t.movedim(d, 0) if d is not None else t.expand((info.batch_size,) + t.shape))
+              for t, d in zip(args[:7], in_dims[1:8])]
+        return _LCPJvpFn.apply(state, *ts, *args[7:]), 0
+
+
+class _LCPFn(torch.autograd.Function):
+    """Written in setup_context form so that torch.func (vjp, grad, jacrev, jvp, jacfwd) and forward-mode dual
+    tensors can trace through it. The primal outputs nu, lam, slack are not differentiable."""
+
+    @staticmethod
+    def forward(Q, p, G, h, A, b, F, opts):
+        state = {}
         zhat, nu, lam, slack, status, iters, resid = solve_forward(
-            Q, p, G, h, A, b, F, opts.eps, opts.not_improved_lim, opts.max_iter, save=ctx.saved_state)
+            Q, p, G, h, A, b, F, opts.eps, opts.not_improved_lim, opts.max_iter, save=state)
         if bool((status == _lib.STATUS_SINGULAR_Q).any()):
             raise RuntimeError(SINGULAR_Q_MSG)
         if opts.verbose >= 0 and bool((resid > 1.0).any()):
             print(INACCURATE_MSG)
             print(resid.max())
-        e = A.shape[1] if A.dim() > 1 else 0
-        ctx.e = e
-        ctx.exact_adjoint = bool(getattr(opts, "exact_adjoint", False))
-        ctx.save_for_backward(zhat, Q, G, A if e > 0 else None, F, nu, lam, slack)
-        ctx.AB_proto = (A, b)
         opts.nus, opts.lams, opts.slacks = nu, lam, slack          # lcp.py:29 stashes these on self
         opts.status, opts.iters, opts.resids = status, iters, resid
-        return zhat
+        opts._solve_state = state                                  # picked up by setup_context, right after
+        return zhat, nu, lam, slack
 
     @staticmethod
-    def backward(ctx, dl_dzhat):
-        zhat, Q, G, A, F, nu, lam, slack = ctx.saved_tensors
-        need = list(ctx.needs_input_grad[:7])
-        dQ, dp, dG, dh, dA, db, dF = solve_backward(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need,
-                                                    saved=ctx.saved_state, exact_adjoint=ctx.exact_adjoint)
-        return dQ, dp, dG, dh, dA, db, dF, None
+    def setup_context(ctx, inputs, output):
+        Q, p, G, h, A, b, F, opts = inputs
+        zhat, nu, lam, slack = output
+        e = A.shape[1] if A.dim() > 1 else 0
+        ctx.state = opts.__dict__.pop("_solve_state", None)
+        ctx.exact_adjoint = bool(getattr(opts, "exact_adjoint", False))
+        saved = (zhat, Q, G, A if e > 0 else None, F, nu, lam, slack)
+        ctx.save_for_backward(*saved)
+        ctx.save_for_forward(*saved)
+        ctx.mark_non_differentiable(*[t for t in (nu, lam, slack) if t is not None])
+
+    @staticmethod
+    def backward(ctx, dl_dzhat, *_):
+        need = tuple(ctx.needs_input_grad[:7])
+        grads = _LCPVjpFn.apply(dl_dzhat, (need, ctx.state, ctx.exact_adjoint), *ctx.saved_tensors)
+        return (*grads, None)
+
+    @staticmethod
+    def jvp(ctx, tQ, tp, tG, th, tA, tb, tF, _):
+        # the true derivative whatever exact_adjoint says: K is factored as the forward factors it
+        dz = _LCPJvpFn.apply(ctx.state, tQ, tp, tG, th, tA, tb, tF, *ctx.saved_tensors)
+        return dz, None, None, None
+
+    @staticmethod
+    def vmap(info, in_dims, *args):
+        raise NotImplementedError(_BATCHED_PRIMAL)
 
 
 class LCPFunction:
@@ -205,4 +369,10 @@ class LCPFunction:
         self.status = self.iters = self.resids = None
 
     def __call__(self, Q, p, G, h, A, b, F):
-        return _LCPFn.apply(Q, p, G, h, A, b, F, self)
+        """zhat [B, n]. Differentiable in reverse mode (backward, torch.func.vjp / grad / jacrev, where the
+        cotangents of a vmap go to one batched kernel call) and in forward mode (torch.func.jvp / jacfwd,
+        torch.autograd.forward_ad dual tensors). Forward mode is the true derivative of the solve, the transpose
+        of exact_adjoint=True; it takes tQ as given while the backward's dQ is symmetrised, so jacfwd and
+        jacrev agree along symmetric directions of Q. Second derivatives and vmap over the inputs raise
+        NotImplementedError."""
+        return _LCPFn.apply(Q, p, G, h, A, b, F, self)[0]
