@@ -141,7 +141,7 @@ struct BJvpArgs {
   cnd::EngineSoA<double> soa;
   const double* A;
   const double *zhat, *nu, *lam, *slack;
-  const double *t_mass, *t_inertia, *t_v, *t_fext, *t_normal, *t_p1, *t_p2, *t_mu, *t_rest, *t_A, *t_b;
+  cnd::EngineTangents<double> t;
   double* dz;
   double* wsd;
   int* wsi;
@@ -1441,6 +1441,15 @@ __global__ void __launch_bounds__(NT, 1) band_forward_kernel(const __grid_consta
 // the entries the assembly writes (same formulas as lcp_condensed.cuh's engine path). flags bit 0 (exact adjoint)
 // factors and solves the transposed system K^T instead (DESIGN.md section 3.4); the chain rule is the same.
 //
+// Zero gradients of the contact slot at output offset oc (an unused slot, or a scene the forward rejected).
+__device__ __forceinline__ void zero_contact_grads(const BBwdArgs& a, size_t oc) {
+  if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
+  if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
+  if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
+  if (a.drest) a.drest[oc] = 0;
+  if (a.dmu) a.dmu[oc] = 0;
+}
+
 // The gradients of one cotangent from the solve's dx, dlam, dnu in c: inputs of scene sc, outputs at row so.
 __device__ __forceinline__ void backward_grads(const BBwdArgs& a, Ctx& c, BProf& pf, int sc, int so) {
   const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, ncap = c.ncap, nb = c.nb;
@@ -1454,11 +1463,7 @@ __device__ __forceinline__ void backward_grads(const BBwdArgs& a, Ctx& c, BProf&
   for (int k = tid; k < ncs; k += NT) {
     const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
     if (k >= nc) {                                                          // unused slots of a scene with fewer contacts
-      if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
-      if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
-      if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
-      if (a.drest) a.drest[oc] = 0;
-      if (a.dmu) a.dmu[oc] = 0;
+      zero_contact_grads(a, oc);
       continue;
     }
     const double nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
@@ -1534,13 +1539,14 @@ __device__ __forceinline__ void backward_grads(const BBwdArgs& a, Ctx& c, BProf&
   pf.lap(BPH_GRADS);
 }
 
-// One factorisation at the saved solution, then one solve and chain rule per cotangent r in [r0, r1); each
-// round streams the factor blocks back from the L2 workspace.
-__device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf& pf, int sc, int r0, int r1) {
+// The saved solution of scene sc (zhat, lam, slack, nu of BBwdArgs or BJvpArgs) into c.x, c.z, c.s, c.y -- the
+// rows of contact k move from out_row to slot-major r ncap + k -- with d = lam / slack clamped to [1e-10, 1e10] as in
+// the condensed fp64 backward and c.rs zeroed, then one factorisation of K (trans: K^T, the exact adjoint).
+template <typename Args>
+__device__ __forceinline__ void factor_saved(const Args& a, Ctx& c, BProf& pf, int sc, bool trans) {
   const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, cs = c.cs, ncap = c.ncap;
   const cnd::EngineSoA<double>& E = a.soa;
-  const int ncs = E.nc, mode = E.mode;
-  const double* mu = E.mu ? E.mu + (size_t)sc * ncs : nullptr;
+  const double* mu = E.mu ? E.mu + (size_t)sc * E.nc : nullptr;
   const double* zh = a.zhat + (size_t)sc * n;
   const double* lamv = a.lam + (size_t)sc * a.P.m;
   const double* slk = a.slack + (size_t)sc * a.P.m;
@@ -1554,7 +1560,28 @@ __device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf&
     }
   for (int i = tid; i < e; i += NT) c.y[i] = a.nu[(size_t)sc * e + i];
   __syncthreads();
-  factor_kkt(c, pf, mode, mu, (a.flags & 1u) != 0);                         // :46
+  factor_kkt(c, pf, E.mode, mu, trans);                                     // :46
+}
+
+// Binds scene sc's contacts to c and finds its structure: 0 = ok, 1 = unsupported (too many contacts or the
+// topology), 2 = singular mass matrix.
+__device__ __forceinline__ int bind_scene(Ctx& c, const BPlan& P, const cnd::EngineSoA<double>& soa, const double* A,
+                                          int sc) {
+  const int ncs = soa.nc;
+  c.nc = soa.nc_s ? soa.nc_s[sc] : ncs;
+  c.b1 = soa.b1 + (soa.nc_s ? (size_t)sc * ncs : 0);
+  c.b2 = soa.b2 + (soa.nc_s ? (size_t)sc * ncs : 0);
+  c.A = P.e > 0 ? A + (size_t)sc * P.e * P.n : nullptr;
+  int rc = (c.nc < 0 || c.nc > P.ncap) ? 1 : 0;
+  if (rc == 0) { c.m = c.cs * c.nc; rc = build_structure(c, soa, sc); }
+  return rc;
+}
+
+// One factorisation at the saved solution, then one solve and chain rule per cotangent r in [r0, r1); each
+// round streams the factor blocks back from the L2 workspace.
+__device__ __forceinline__ void backward_scene(const BBwdArgs& a, Ctx& c, BProf& pf, int sc, int r0, int r1) {
+  const int tid = threadIdx.x, n = c.n;
+  factor_saved(a, c, pf, sc, (a.flags & 1u) != 0);
   for (int r = r0; r < r1; ++r) {
     const int so = r * a.B + sc;
     for (int i = tid; i < n; i += NT) c.rx[i] = a.g[(size_t)so * n + i];
@@ -1574,12 +1601,7 @@ __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_const
     const int sc = w / a.chunks, ch = w - sc * a.chunks;
     const int r0 = (int)((long long)a.R * ch / a.chunks), r1 = (int)((long long)a.R * (ch + 1) / a.chunks);
     const int ncs = a.soa.nc, n = P.n, nb = P.nb, e = P.e;
-    c.nc = a.soa.nc_s ? a.soa.nc_s[sc] : ncs;
-    c.b1 = a.soa.b1 + (a.soa.nc_s ? (size_t)sc * ncs : 0);
-    c.b2 = a.soa.b2 + (a.soa.nc_s ? (size_t)sc * ncs : 0);
-    c.A = e > 0 ? a.A + (size_t)sc * e * n : nullptr;
-    int rc = (c.nc < 0 || c.nc > P.ncap) ? 1 : 0;
-    if (rc == 0) { c.m = c.cs * c.nc; rc = build_structure(c, a.soa, sc); }
+    const int rc = bind_scene(c, P, a.soa, a.A, sc);
     pf.lap(BPH_STRUCT);
     if (rc != 0) {                                                          // the forward reported it: zero gradients
       const int tid = threadIdx.x;
@@ -1587,14 +1609,7 @@ __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_const
         const size_t so = (size_t)r * a.B + sc;
         for (int i = tid; i < n; i += NT) { if (a.dv) a.dv[so * n + i] = 0; if (a.dfext) a.dfext[so * n + i] = 0; }
         for (int i = tid; i < nb; i += NT) { if (a.dmass) a.dmass[so * nb + i] = 0; if (a.dinertia) a.dinertia[so * nb + i] = 0; }
-        for (int i = tid; i < ncs; i += NT) {
-          const size_t oc = so * ncs + i;
-          if (a.dnormal) { a.dnormal[oc * 2] = 0; a.dnormal[oc * 2 + 1] = 0; }
-          if (a.dp1) { a.dp1[oc * 2] = 0; a.dp1[oc * 2 + 1] = 0; }
-          if (a.dp2) { a.dp2[oc * 2] = 0; a.dp2[oc * 2 + 1] = 0; }
-          if (a.drest) a.drest[oc] = 0;
-          if (a.dmu) a.dmu[oc] = 0;
-        }
+        for (int i = tid; i < ncs; i += NT) zero_contact_grads(a, so * ncs + i);
         for (int i = tid; i < e; i += NT) if (a.db) a.db[so * e + i] = 0;
         if (a.dA) for (int i = tid; i < e * n; i += NT) a.dA[so * e * n + i] = 0;
       }
@@ -1608,119 +1623,33 @@ __global__ void __launch_bounds__(NT, 1) band_backward_kernel(const __grid_const
 // ------------------------------------------------------------------ Jacobian-vector products (DESIGN.md section 8)
 // Same system as lcp_condensed.cuh's cond_jvp_kernel: K [dx; ds; dz; dy] = -(r_x, 0, r_z, r_y) with the
 // non-transposed K factored once per (scene, chunk of tangents) at the saved iterate, d clamped as in the backward.
-// Rows live slot-major here (row r of contact k at r ncap + k); the gather of dG^T lam walks the per-body adjacency.
-__device__ __noinline__ void jvp_rhs(const BJvpArgs& a, const Ctx& c, int sc, int so) {
-  const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, ncap = c.ncap, nb = c.nb;
-  const cnd::EngineSoA<double>& E = a.soa;
-  const int ncs = E.nc, mode = E.mode;
-  const double* v = E.v + (size_t)sc * n;
-  const double* tv = a.t_v ? a.t_v + (size_t)so * n : nullptr;
-  const double* zh = c.x;
-  const double* lm = c.z;
-  auto tget = [](const double* t, size_t i) { return t ? t[i] : 0.0; };
-  for (int k = tid; k < nc; k += NT) {
-    const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
-    const int b1 = c.b1[k], b2 = c.b2[k];
-    const bool two = b2 < nb;
-    const double nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
-    const double p1x = E.p1[ic * 2], p1y = E.p1[ic * 2 + 1], p2x = E.p2[ic * 2], p2y = E.p2[ic * 2 + 1];
-    const double tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
-    const double t1x = tget(a.t_p1, oc * 2), t1y = tget(a.t_p1, oc * 2 + 1);
-    const double t2x = tget(a.t_p2, oc * 2), t2y = tget(a.t_p2, oc * 2 + 1);
-    double r1[3], r2[3], d1[3], d2[3];
-    cnd::contact_row<double>(p1x, p1y, p2x, p2y, nx, ny, r1, r2);
-    cnd::contact_row_tangent<double>(p1x, p1y, p2x, p2y, nx, ny, t1x, t1y, t2x, t2y, tnx, tny, d1, d2);
-    double jv = 0, tjv = 0, gz = 0;                                         // Jc v, d(Jc v), dJc zhat
-#pragma unroll
-    for (int q = 0; q < 3; ++q) {
-      const int j1 = 3 * b1 + q;
-      jv += r1[q] * v[j1];
-      tjv += d1[q] * v[j1] + (tv ? r1[q] * tv[j1] : 0.0);
-      gz += d1[q] * zh[j1];
-      if (two) {
-        const int j2 = 3 * b2 + q;
-        jv += r2[q] * v[j2];
-        tjv += d2[q] * v[j2] + (tv ? r2[q] * tv[j2] : 0.0);
-        gz += d2[q] * zh[j2];
-      }
-    }
-    const double rc = E.rest[ic], trc = tget(a.t_rest, oc);
-    if (mode == 0) {
-      c.rz[k] = gz - (trc * jv + rc * tjv);                                 // h_c = (Jc v) rest
-      cnd::contact_row_tangent<double>(p1x, p1y, p2x, p2y, ny, -nx, t1x, t1y, t2x, t2y, tny, -tnx, d1, d2);
-      double fz = 0;
-#pragma unroll
-      for (int q = 0; q < 3; ++q) { fz += d1[q] * zh[3 * b1 + q]; if (two) fz += d2[q] * zh[3 * b2 + q]; }
-      c.rz[ncap + k] = fz;
-      c.rz[2 * ncap + k] = -fz;
-      c.rz[3 * ncap + k] = -(tget(a.t_mu, oc) * lm[k]);                     // F[gamma_k][k] = mu_k
-    } else {
-      c.rz[k] = gz - (tjv * (1.0 - rc) - trc * jv);                         // h_c = (Jc v)(1 - rest)
-    }
-  }
-  for (int body = tid; body < nb; body += NT) {
+// The right-hand side is cnd::engine_jvp_rhs with this layout: rows slot-major (row q of contact k at q ncap + k),
+// and the contacts of a dof are those of its body's adjacency.
+struct BandRows {
+  const Ctx& c;
+  __device__ __forceinline__ double* x() const { return c.x; }
+  __device__ __forceinline__ double* z() const { return c.z; }
+  __device__ __forceinline__ double* y() const { return c.y; }
+  __device__ __forceinline__ double* rx() const { return c.rx; }
+  __device__ __forceinline__ double* rz() const { return c.rz; }
+  __device__ __forceinline__ double* ry() const { return c.ry; }
+  __device__ __forceinline__ int row(int q, int k) const { return q * c.ncap + k; }
+  template <typename F>
+  __device__ __forceinline__ void walk(int, int body, F f) const {
     const int s0 = c.start[body], s1 = c.start[body + 1];
-#pragma unroll
-    for (int comp = 0; comp < 3; ++comp) {
-      const int j = 3 * body + comp;
-      const double q = comp == 0 ? E.inertia[(size_t)sc * nb + body] : E.mass[(size_t)sc * nb + body];
-      const double tq = comp == 0 ? tget(a.t_inertia, (size_t)so * nb + body) : tget(a.t_mass, (size_t)so * nb + body);
-      double acc = tq * zh[j];
-      if (mode == 0) acc += tq * v[j] + q * (tv ? tv[j] : 0.0) + E.dt * tget(a.t_fext, (size_t)so * n + j);
-      for (int it = s0; it < s1; ++it) {                                    // the contacts that touch this body
-        const int ad = c.adj[it], k = ad >> 1, side = ad & 1;
-        const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
-        const double* pp = side ? E.p2 : E.p1;
-        const double* tp = side ? a.t_p2 : a.t_p1;
-        const double px = pp[ic * 2], py = pp[ic * 2 + 1], tpx = tget(tp, oc * 2), tpy = tget(tp, oc * 2 + 1);
-        const double nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
-        const double tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
-        auto drow = [&](double dx, double dy, double tdx, double tdy) {
-          return comp == 0 ? tpx * dy + px * tdy - tpy * dx - py * tdx : (comp == 1 ? tdx : tdy);
-        };
-        double g = drow(nx, ny, tnx, tny) * lm[k];
-        if (mode == 0) g += drow(ny, -nx, tny, -tnx) * (lm[ncap + k] - lm[2 * ncap + k]);
-        acc += side ? -g : g;
-      }
-      if (e > 0 && a.t_A) {
-        const double* tA = a.t_A + (size_t)so * e * n;
-        for (int i = 0; i < e; ++i) acc += tA[(size_t)i * n + j] * c.y[i];
-      }
-      c.rx[j] = acc;
-    }
+    for (int it = s0; it < s1; ++it) { const int ad = c.adj[it]; f(ad >> 1, ad & 1); }
   }
-  for (int i = tid; i < e; i += NT) {
-    double acc = -tget(a.t_b, (size_t)so * e + i);
-    if (a.t_A) {
-      const double* tA = a.t_A + (size_t)so * e * n + (size_t)i * n;
-      for (int j = 0; j < n; ++j) acc += tA[j] * zh[j];
-    }
-    c.ry[i] = acc;
-  }
-  __syncthreads();
+};
+
+// engine_jvp_rhs in the banded layout, kept out of line as in the condensed kernel.
+__device__ __noinline__ void jvp_rhs(const BJvpArgs& a, const Ctx& c, int sc, int so) {
+  cnd::engine_jvp_rhs<double>(a.soa, a.t, BandRows{c}, sc, so, c.n, c.e, c.nc);
 }
 
-// backward_scene's prologue (saved iterate, clamp, factorisation of K), kept separate so that the backward's code
-// is unchanged; then one right-hand side and one solve per tangent r in [r0, r1).
+// The saved solution and one factorisation of K, then one right-hand side and one solve per tangent r in [r0, r1).
 __device__ __forceinline__ void jvp_scene(const BJvpArgs& a, Ctx& c, BProf& pf, int sc, int r0, int r1) {
-  const int tid = threadIdx.x, n = c.n, e = c.e, nc = c.nc, cs = c.cs, ncap = c.ncap;
-  const cnd::EngineSoA<double>& E = a.soa;
-  const int ncs = E.nc, mode = E.mode;
-  const double* mu = E.mu ? E.mu + (size_t)sc * ncs : nullptr;
-  const double* zh = a.zhat + (size_t)sc * n;
-  const double* lamv = a.lam + (size_t)sc * a.P.m;
-  const double* slk = a.slack + (size_t)sc * a.P.m;
-  for (int i = tid; i < n; i += NT) c.x[i] = zh[i];
-  for (int r = 0; r < cs; ++r)
-    for (int k = tid; k < nc; k += NT) {
-      const int i = r * ncap + k, o = out_row(r, k, nc);
-      double d = lamv[o] / slk[o];
-      d = d > 1e10 ? 1e10 : (d < 1e-10 ? 1e-10 : d);
-      c.z[i] = lamv[o]; c.s[i] = slk[o]; c.d[i] = d; c.rs[i] = 0.0;
-    }
-  for (int i = tid; i < e; i += NT) c.y[i] = a.nu[(size_t)sc * e + i];
-  __syncthreads();
-  factor_kkt(c, pf, mode, mu, false);
+  const int tid = threadIdx.x, n = c.n, e = c.e;
+  factor_saved(a, c, pf, sc, false);
   for (int r = r0; r < r1; ++r) {
     const size_t so = (size_t)r * a.B + sc;
     jvp_rhs(a, c, sc, (int)so);
@@ -1740,17 +1669,11 @@ __global__ void __launch_bounds__(NT, 1) band_jvp_kernel(const __grid_constant__
   for (int w = blockIdx.x; w < a.B * a.chunks; w += gridDim.x) {
     const int sc = w / a.chunks, ch = w - sc * a.chunks;
     const int r0 = (int)((long long)a.R * ch / a.chunks), r1 = (int)((long long)a.R * (ch + 1) / a.chunks);
-    const int ncs = a.soa.nc, n = P.n, e = P.e;
-    c.nc = a.soa.nc_s ? a.soa.nc_s[sc] : ncs;
-    c.b1 = a.soa.b1 + (a.soa.nc_s ? (size_t)sc * ncs : 0);
-    c.b2 = a.soa.b2 + (a.soa.nc_s ? (size_t)sc * ncs : 0);
-    c.A = e > 0 ? a.A + (size_t)sc * e * n : nullptr;
-    int rc = (c.nc < 0 || c.nc > P.ncap) ? 1 : 0;
-    if (rc == 0) { c.m = c.cs * c.nc; rc = build_structure(c, a.soa, sc); }
+    const int rc = bind_scene(c, P, a.soa, a.A, sc);
     pf.lap(BPH_STRUCT);
     if (rc != 0) {                                                          // the forward reported it: zero tangents
       for (int r = r0; r < r1; ++r)
-        for (int i = threadIdx.x; i < n; i += NT) a.dz[((size_t)r * a.B + sc) * n + i] = 0.0;
+        for (int i = threadIdx.x; i < P.n; i += NT) a.dz[((size_t)r * a.B + sc) * P.n + i] = 0.0;
     } else {
       jvp_scene(a, c, pf, sc, r0, r1);
     }

@@ -1644,7 +1644,14 @@ __global__ void __launch_bounds__(NT, (NS <= 6) ? 2 : 1) cond_backward_kernel(co
 // derivative of the assembly (build_structure_soa), evaluated per contact and per dof, never as a dense matrix.
 // Every tangent is [R][B][...] like CBwdArgs' cotangents, nullptr = zero.
 // Dense inputs (soa.mass == nullptr): the structure comes from Q, G, A, F (or sload) as in cond_backward_kernel and
-// d(Q, p, G, h, F) are the dense tangents tQ ... tF; t_A, t_b serve both paths.
+// d(Q, p, G, h, F) are the dense tangents tQ ... tF.
+
+// Tangents of the engine's contact list, each [R][B][...] like the inputs it moves, nullptr = zero.
+template <typename T>
+struct EngineTangents {
+  const T *mass, *inertia, *v, *fext, *normal, *p1, *p2, *mu, *rest, *A, *b;
+};
+
 template <typename T>
 struct CJvpArgs {
   CPlan P;
@@ -1652,7 +1659,7 @@ struct CJvpArgs {
   const T *Q, *G, *A, *F;
   const T *zhat, *nu, *lam, *slack;
   EngineSoA<T> soa;
-  const T *t_mass, *t_inertia, *t_v, *t_fext, *t_normal, *t_p1, *t_p2, *t_mu, *t_rest, *t_A, *t_b;
+  EngineTangents<T> t;        // t.A, t.b serve both paths
   const T *tQ, *tp, *tG, *th, *tF;   // dense path: [R][B][...] or nullptr
   int* done;                  // dense path, as CBwdArgs
   const int* only;
@@ -1669,28 +1676,33 @@ __device__ __forceinline__ void contact_row_tangent(T p1x, T p1y, T p2x, T p2y, 
   r2[0] = -(t2x * dy + p2x * tdy - t2y * dx - p2y * tdx); r2[1] = -tdx; r2[2] = -tdy;
 }
 
-// Right-hand side (r_x, r_z, r_y) of tangent slot so into S.rx, S.rz, S.ry; the saved iterate is in S.x, S.z, S.y.
-template <typename T>
-__device__ __noinline__ void jvp_rhs(const CJvpArgs<T>& a, CSmem<T> S, Struct st, int sc, int so) {
-  const CPlan& P = a.P;
-  const EngineSoA<T>& E = a.soa;
-  const int n = P.n, e = P.e, tid = threadIdx.x, nb = E.nb, ncs = E.nc, nc = st.ncomp;
+// Right-hand side (r_x, r_z, r_y) of the engine JVP for tangent slot so of scene sc (nc contacts), shared by the
+// condensed and banded kernels. The layout L says where the two families keep things:
+//   L.x(), L.z(), L.y(): the saved iterate zhat, lam, nu;  L.rx(), L.rz(), L.ry(): where r_x, r_z, r_y go;
+//   L.row(q, k): the slot of row q of contact k (0: normal, 1 and 2: friction, 3: the gamma row of mode 0);
+//   L.walk(j, body, f): f(k, side) for every contact k touching dof j of `body`, side 1 when it is the contact's body2.
+// One thread per contact and one per dof; the walk's order is the summation order of dG^T lam (deterministic).
+template <typename T, typename L>
+__device__ __forceinline__ void engine_jvp_rhs(const EngineSoA<T>& E, const EngineTangents<T>& t, L lay, int sc, int so,
+                                            int n, int e, int nc) {
+  const int tid = threadIdx.x, nb = E.nb, ncs = E.nc;
   const int32_t* tb1 = E.b1 + (E.nc_s ? (size_t)sc * ncs : 0);
   const int32_t* tb2 = E.b2 + (E.nc_s ? (size_t)sc * ncs : 0);
   const T* v = E.v + (size_t)sc * n;
-  const T* tv = a.t_v ? a.t_v + (size_t)so * n : nullptr;
-  const T* zh = S.x(); const T* lm = S.z();
-  auto tget = [](const T* t, size_t i) { return t ? t[i] : T(0); };
-  // r_z, one thread per contact: rows {c, nc + 2c, nc + 2c + 1, 3nc + c} (mode 0) or {c} (mode 1)
-  for (int c = tid; c < nc; c += NT) {
-    const size_t ic = (size_t)sc * ncs + c, oc = (size_t)so * ncs + c;
-    const int b1 = tb1[c], b2 = tb2[c];
+  const T* tv = t.v ? t.v + (size_t)so * n : nullptr;
+  const T* zh = lay.x(); const T* lm = lay.z();
+  T* rz = lay.rz();
+  auto tget = [](const T* p, size_t i) { return p ? p[i] : T(0); };
+  // r_z, one thread per contact
+  for (int k = tid; k < nc; k += NT) {
+    const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
+    const int b1 = tb1[k], b2 = tb2[k];
     const bool two = b2 < nb;
     const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
     const T p1x = E.p1[ic * 2], p1y = E.p1[ic * 2 + 1], p2x = E.p2[ic * 2], p2y = E.p2[ic * 2 + 1];
-    const T tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
-    const T t1x = tget(a.t_p1, oc * 2), t1y = tget(a.t_p1, oc * 2 + 1);
-    const T t2x = tget(a.t_p2, oc * 2), t2y = tget(a.t_p2, oc * 2 + 1);
+    const T tnx = tget(t.normal, oc * 2), tny = tget(t.normal, oc * 2 + 1);
+    const T t1x = tget(t.p1, oc * 2), t1y = tget(t.p1, oc * 2 + 1);
+    const T t2x = tget(t.p2, oc * 2), t2y = tget(t.p2, oc * 2 + 1);
     T r1[3], r2[3], d1[3], d2[3];
     contact_row<T>(p1x, p1y, p2x, p2y, nx, ny, r1, r2);
     contact_row_tangent<T>(p1x, p1y, p2x, p2y, nx, ny, t1x, t1y, t2x, t2y, tnx, tny, d1, d2);
@@ -1708,62 +1720,82 @@ __device__ __noinline__ void jvp_rhs(const CJvpArgs<T>& a, CSmem<T> S, Struct st
         gz += d2[q] * zh[j2];
       }
     }
-    const T rc = E.rest[ic], trc = tget(a.t_rest, oc);
+    const T rc = E.rest[ic], trc = tget(t.rest, oc);
     if (E.mode == 0) {
-      S.rz()[c] = gz - (trc * jv + rc * tjv);                          // h_c = (Jc v) rest
-      contact_row<T>(p1x, p1y, p2x, p2y, ny, -nx, r1, r2);
+      rz[lay.row(0, k)] = gz - (trc * jv + rc * tjv);                 // h_c = (Jc v) rest
       contact_row_tangent<T>(p1x, p1y, p2x, p2y, ny, -nx, t1x, t1y, t2x, t2y, tny, -tnx, d1, d2);
       T fz = 0;                                                        // dJf zhat (row f2 = -row f1)
 #pragma unroll
       for (int q = 0; q < 3; ++q) { fz += d1[q] * zh[3 * b1 + q]; if (two) fz += d2[q] * zh[3 * b2 + q]; }
-      S.rz()[nc + 2 * c] = fz;
-      S.rz()[nc + 2 * c + 1] = -fz;
-      S.rz()[3 * nc + c] = -(tget(a.t_mu, oc) * lm[c]);              // F[gamma_c][c] = mu_c
+      rz[lay.row(1, k)] = fz;
+      rz[lay.row(2, k)] = -fz;
+      rz[lay.row(3, k)] = -(tget(t.mu, oc) * lm[k]);                  // F[gamma_k][k] = mu_k
     } else {
-      S.rz()[c] = gz - (tjv * (T(1) - rc) - trc * jv);                 // h_c = (Jc v)(1 - rest)
+      rz[lay.row(0, k)] = gz - (tjv * (T(1) - rc) - trc * jv);        // h_c = (Jc v)(1 - rest)
     }
   }
-  // r_x, one thread per dof; dG^T lam is gathered through the dof's contact list (ascending: deterministic)
+  // r_x, one thread per dof; dG^T lam is gathered through the contacts the layout's walk yields
   for (int j = tid; j < n; j += NT) {
     const int body = j / 3, comp = j - 3 * body;
     const T q = comp == 0 ? E.inertia[(size_t)sc * nb + body] : E.mass[(size_t)sc * nb + body];
-    const T tq = comp == 0 ? tget(a.t_inertia, (size_t)so * nb + body) : tget(a.t_mass, (size_t)so * nb + body);
+    const T tq = comp == 0 ? tget(t.inertia, (size_t)so * nb + body) : tget(t.mass, (size_t)so * nb + body);
     T acc = tq * zh[j];
-    if (E.mode == 0) acc += tq * v[j] + q * (tv ? tv[j] : T(0)) + E.dt * tget(a.t_fext, (size_t)so * n + j);
-    const int cnt = S.clcnt()[j];
-    for (int l = 0; l < cnt; ++l) {
-      const int c = S.clist()[l * n + j] >> 3;
-      const size_t ic = (size_t)sc * ncs + c, oc = (size_t)so * ncs + c;
-      const bool side1 = tb1[c] == body;
-      const T* pp = side1 ? E.p1 : E.p2;
-      const T* tp = side1 ? a.t_p1 : a.t_p2;
+    if (E.mode == 0) acc += tq * v[j] + q * (tv ? tv[j] : T(0)) + E.dt * tget(t.fext, (size_t)so * n + j);
+    lay.walk(j, body, [&](int k, int side) {
+      const size_t ic = (size_t)sc * ncs + k, oc = (size_t)so * ncs + k;
+      const T* pp = side ? E.p2 : E.p1;
+      const T* tp = side ? t.p2 : t.p1;
       const T px = pp[ic * 2], py = pp[ic * 2 + 1], tpx = tget(tp, oc * 2), tpy = tget(tp, oc * 2 + 1);
       const T nx = E.normal[ic * 2], ny = E.normal[ic * 2 + 1];
-      const T tnx = tget(a.t_normal, oc * 2), tny = tget(a.t_normal, oc * 2 + 1);
+      const T tnx = tget(t.normal, oc * 2), tny = tget(t.normal, oc * 2 + 1);
       // d(row entry) along direction (dx, dy): [p x d, d] of this body (negated for body2)
       auto drow = [&](T dx, T dy, T tdx, T tdy) {
         return comp == 0 ? tpx * dy + px * tdy - tpy * dx - py * tdx : (comp == 1 ? tdx : tdy);
       };
-      T g = drow(nx, ny, tnx, tny) * lm[c];
-      if (E.mode == 0) g += drow(ny, -nx, tny, -tnx) * (lm[nc + 2 * c] - lm[nc + 2 * c + 1]);
-      acc += side1 ? g : -g;
+      T g = drow(nx, ny, tnx, tny) * lm[k];
+      if (E.mode == 0) g += drow(ny, -nx, tny, -tnx) * (lm[lay.row(1, k)] - lm[lay.row(2, k)]);
+      acc += side ? -g : g;
+    });
+    if (e > 0 && t.A) {
+      const T* tA = t.A + (size_t)so * e * n;
+      for (int i = 0; i < e; ++i) acc += tA[(size_t)i * n + j] * lay.y()[i];
     }
-    if (e > 0 && a.t_A) {
-      const T* tA = a.t_A + (size_t)so * e * n;
-      for (int k = 0; k < e; ++k) acc += tA[(size_t)k * n + j] * S.y()[k];
-    }
-    S.rx()[j] = acc;
+    lay.rx()[j] = acc;
   }
-  for (int k = tid; k < e; k += NT) {
-    T acc = -tget(a.t_b, (size_t)so * e + k);
-    if (a.t_A) {
-      const T* tA = a.t_A + (size_t)so * e * n + (size_t)k * n;
+  for (int i = tid; i < e; i += NT) {
+    T acc = -tget(t.b, (size_t)so * e + i);
+    if (t.A) {
+      const T* tA = t.A + (size_t)so * e * n + (size_t)i * n;
       for (int j = 0; j < n; ++j) acc += tA[j] * zh[j];
     }
-    S.ry()[k] = acc;
+    lay.ry()[i] = acc;
   }
   __syncthreads();
 }
+
+// engine_jvp_rhs' layout in the condensed kernel: rows {k, nc + 2k, nc + 2k + 1, 3nc + k} of contact k, and the
+// dof's ascending contact list.
+template <typename T>
+struct CondRows {
+  CSmem<T> S;
+  int n, nc;
+  const int32_t* b1;
+  __device__ __forceinline__ T* x() const { return S.x(); }
+  __device__ __forceinline__ T* z() const { return S.z(); }
+  __device__ __forceinline__ T* y() const { return S.y(); }
+  __device__ __forceinline__ T* rx() const { return S.rx(); }
+  __device__ __forceinline__ T* rz() const { return S.rz(); }
+  __device__ __forceinline__ T* ry() const { return S.ry(); }
+  __device__ __forceinline__ int row(int q, int k) const { return q == 0 ? k : (q == 3 ? 3 * nc + k : nc + 2 * k + q - 1); }
+  template <typename F>
+  __device__ __forceinline__ void walk(int j, int body, F f) const {
+    const int cnt = S.clcnt()[j];
+    for (int l = 0; l < cnt; ++l) {
+      const int k = S.clist()[l * n + j] >> 3;
+      f(k, b1[k] == body ? 0 : 1);
+    }
+  }
+};
 
 // Right-hand side of tangent slot so for dense inputs (CJvpArgs::tQ ... tF): r_x by columns (thread j walks column j
 // of tG and tA: coalesced, no atomics), r_z and r_y by rows.
@@ -1775,7 +1807,7 @@ __device__ __noinline__ void jvp_rhs_dense(const CJvpArgs<T>& a, CSmem<T> S, Str
   const T* tQ = a.tQ ? a.tQ + (size_t)so * n * n : nullptr;
   const T* tG = a.tG ? a.tG + (size_t)so * m * n : nullptr;
   const T* tF = a.tF ? a.tF + (size_t)so * m * m : nullptr;
-  const T* tA = (a.t_A && e > 0) ? a.t_A + (size_t)so * e * n : nullptr;
+  const T* tA = (a.t.A && e > 0) ? a.t.A + (size_t)so * e * n : nullptr;
   for (int j = tid; j < n; j += NT) {
     T acc = a.tp ? a.tp[(size_t)so * n + j] : T(0);
     if (tQ) for (int i = 0; i < n; ++i) acc = fma(tQ[(size_t)j * n + i], zh[i], acc);
@@ -1790,15 +1822,25 @@ __device__ __noinline__ void jvp_rhs_dense(const CJvpArgs<T>& a, CSmem<T> S, Str
     S.rz()[i] = acc;
   }
   for (int k = tid; k < e; k += NT) {
-    T acc = a.t_b ? -a.t_b[(size_t)so * e + k] : T(0);
+    T acc = a.t.b ? -a.t.b[(size_t)so * e + k] : T(0);
     if (tA) for (int j = 0; j < n; ++j) acc = fma(tA[(size_t)k * n + j], zh[j], acc);
     S.ry()[k] = acc;
   }
   __syncthreads();
 }
 
+// engine_jvp_rhs in the condensed layout, kept out of line so that the JVP kernel's registers stay with the
+// factorisation and the solves.
+template <typename T>
+__device__ __noinline__ void jvp_rhs(const CJvpArgs<T>& a, CSmem<T> S, Struct st, int sc, int so) {
+  const EngineSoA<T>& E = a.soa;
+  engine_jvp_rhs<T>(E, a.t, CondRows<T>{S, a.P.n, st.ncomp, E.b1 + (E.nc_s ? (size_t)sc * E.nc : 0)}, sc, so, a.P.n,
+                    a.P.e, st.ncomp);
+}
+
 // One factorisation of K (not transposed) at the saved solution, then one right-hand side and one solve per
-// tangent r in [r0, r1). The prologue is backward_scene's, kept separate so that the backward's code is unchanged.
+// tangent r in [r0, r1). The prologue repeats backward_scene's: as one shared helper it moved ptxas' register
+// allocation of both kernels, and the backward ran measurably slower (DESIGN.md section 8).
 template <typename T, int NS, int CS, bool DENSE, typename PF>
 __device__ __forceinline__ void jvp_scene(const CJvpArgs<T>& a, CSmem<T>& S, const Struct& st, PF& pf, int sc,
                                           int r0, int r1) {

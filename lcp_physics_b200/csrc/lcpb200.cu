@@ -6,6 +6,7 @@
 #include <climits>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/lcpb200.h"
@@ -371,34 +372,85 @@ static int bwd_chunks(int R, int B, int target) {
   return std::max(1, std::min(R, (target + B - 1) / B));
 }
 
+// One launch of the condensed-KKT backward or JVP kernel at the handle's NS, and of the dual-form one at its
+// residency mode; the overload follows the args.
+template <typename T>
+static cudaError_t launch_cond(const lcpb200_handle_s* h, const cnd::CBwdArgs<T>& c, int grid, cudaStream_t st) {
+#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, grid, st)
+  return LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
+#undef CALL_BWD
+}
+
+template <typename T>
+static cudaError_t launch_cond(const lcpb200_handle_s* h, const cnd::CJvpArgs<T>& c, int grid, cudaStream_t st) {
+#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, grid, st)
+  return LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
+#undef CALL_JVP
+}
+
+template <typename T>
+static cudaError_t launch_dual(const lcpb200_handle_s* h, const BwdArgs<T>& a, int grid, cudaStream_t st) {
+  const int mode = h->plan.mode;
+  return mode == 0 ? launch_backward_t<T, 0>(a, grid, st)
+                   : mode == 1 ? launch_backward_t<T, 1>(a, grid, st) : launch_backward_t<T, 2>(a, grid, st);
+}
+
+template <typename T>
+static cudaError_t launch_dual(const lcpb200_handle_s* h, const JvpArgs<T>& a, int grid, cudaStream_t st) {
+  const int mode = h->plan.mode;
+  return mode == 0 ? launch_jvp_t<T, 0>(a, grid, st)
+                   : mode == 1 ? launch_jvp_t<T, 1>(a, grid, st) : launch_jvp_t<T, 2>(a, grid, st);
+}
+
 // Scene routing shared by the dense backward and JVP. fp32: condensed-KKT kernel first, the dual form only for the
 // scenes it flags as unstructured. fp64: the dual form first -- at the fp64 round-off floor (lambda, s ~ 1e-16,
 // d = lambda/s spanning 1e+-16) the condensed matrix loses dx (DESIGN.md "Parity") -- and the condensed kernel only
 // as a rescue for scenes on which the dual LU (pivoting restricted to its diagonal blocks) broke down (non-finite
 // dx). LCPB200_DUAL_BACKWARD=1 puts the dual form first for fp32 too.
-struct Route {
-  bool have_cond, cond_first;
-  int* flagbuf;              // [B]: the condensed kernel's done verdicts, or the dual form's bad flags
-  int cchunks, cgrid;        // condensed work items and grid
-  int dchunks, dgrid;        // dual-form work items and grid (the workspace is per CTA)
-};
-
-template <typename T>
-static int make_route(lcpb200_handle_s* h, int slot, int R, int B, cudaStream_t st, Route& r) {
-  r.have_cond = h->cplan.ok != 0;
-  r.cond_first = r.have_cond && sizeof(T) == 4 && !getenv("LCPB200_DUAL_BACKWARD");
-  r.flagbuf = nullptr;
-  if (r.have_cond) {
+// c (condensed) and a (dual form) come zeroed, with the fields of their direction set; this fills the fields the two
+// directions share and launches the kernels in route order.
+template <typename T, typename CArgs, typename DArgs>
+static int run_dense(lcpb200_handle_s* h, int slot, int R, int B, const void* Q, const void* G, const void* A,
+                     const void* F, const void* zhat, const void* nu, const void* lam, const void* slack,
+                     const void* Rsave, const unsigned char* sload, CArgs& c, DArgs& a, cudaStream_t st) {
+  const bool have_cond = h->cplan.ok != 0;
+  const bool cond_first = have_cond && sizeof(T) == 4 && !getenv("LCPB200_DUAL_BACKWARD");
+  int* flagbuf = nullptr;     // [B]: the condensed kernel's done verdicts, or the dual form's bad flags
+  if (have_cond) {
     CK(h->d_flag[slot].ensure(sizeof(int) * (size_t)B));
-    r.flagbuf = (int*)h->d_flag[slot].p;
+    flagbuf = (int*)h->d_flag[slot].p;
     // the dual form's bad flags are an OR over a scene's chunks and right-hand sides: start from 0
-    if (!r.cond_first) CK(cudaMemsetAsync(r.flagbuf, 0, sizeof(int) * (size_t)B, st));
+    if (!cond_first) CK(cudaMemsetAsync(flagbuf, 0, sizeof(int) * (size_t)B, st));
   }
-  r.cchunks = bwd_chunks(R, B, h->cond_grid);
-  r.cgrid = (int)std::min((long long)B * r.cchunks, (long long)std::max(h->cond_grid, 1));
-  r.dchunks = bwd_chunks(R, B, h->max_grid);
-  if (int rc = ensure_ws(h, B * r.dchunks)) return rc;
-  r.dgrid = (int)std::min((long long)B * r.dchunks, (long long)h->ws_ctas);
+  const int cchunks = bwd_chunks(R, B, h->cond_grid);
+  const int cgrid = (int)std::min((long long)B * cchunks, (long long)std::max(h->cond_grid, 1));
+  const int dchunks = bwd_chunks(R, B, h->max_grid);      // the dual form's workspace is per CTA
+  if (int rc = ensure_ws(h, B * dchunks)) return rc;
+  const int dgrid = (int)std::min((long long)B * dchunks, (long long)h->ws_ctas);
+  if (have_cond) {
+    c.P = h->cplan;
+    c.B = B;
+    c.R = R; c.chunks = cchunks;
+    c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
+    c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
+    c.done = cond_first ? flagbuf : nullptr;
+    c.only = cond_first ? nullptr : flagbuf;
+    c.sload = sload;
+    c.prof = h->cprof ? h->cprof + (size_t)slot * h->cond_grid * cnd::CPH_COUNT : nullptr;
+  }
+  if (cond_first) CK(launch_cond(h, c, cgrid, st));
+  a.P = h->plan;
+  a.B = B;
+  a.R = R; a.chunks = dchunks;
+  a.Q = (const T*)Q; a.G = (const T*)G; a.A = (const T*)A; a.F = (const T*)F;
+  a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
+  a.Rsave = have_cond ? nullptr : (const T*)Rsave;    // R is only formed when the forward ran on the dual form
+  a.skip = cond_first ? flagbuf : nullptr;
+  a.bad = (have_cond && !cond_first) ? flagbuf : nullptr;
+  a.ws = (T*)h->ws + (size_t)slot * h->plan.ws_per_cta * h->ws_ctas;
+  a.prof = h->prof ? h->prof + (size_t)slot * h->max_grid * PH_COUNT : nullptr;
+  CK(launch_dual(h, a, dgrid, st));
+  if (have_cond && !cond_first) CK(launch_cond(h, c, cgrid, st));
   return 0;
 }
 
@@ -407,57 +459,17 @@ static int launch_backward(lcpb200_handle_s* h, int slot, int R, int B, const vo
                            const void* F, const void* zhat, const void* nu, const void* lam, const void* slack,
                            const void* g, void* dQ, void* dp, void* dG, void* dh, void* dA, void* db, void* dF,
                            const void* Rsave, unsigned flags, cudaStream_t st, const unsigned char* sload = nullptr) {
-  Route rt;
-  if (int rc = make_route<T>(h, slot, R, B, st, rt)) return rc;
   cnd::CBwdArgs<T> c;
-  if (rt.have_cond) {
-    c.P = h->cplan;
-    c.B = B;
-    c.R = R; c.chunks = rt.cchunks;
-    c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
-    c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
-    c.g = (const T*)g;
-    c.dQ = (T*)dQ; c.dp = (T*)dp; c.dG = (T*)dG; c.dh = (T*)dh; c.dA = (T*)dA; c.db = (T*)db; c.dF = (T*)dF;
-    c.done = rt.cond_first ? rt.flagbuf : nullptr;
-    c.only = rt.cond_first ? nullptr : rt.flagbuf;
-    c.flags = flags;
-    c.sload = sload;
-    memset(&c.soa, 0, sizeof(c.soa));
-    c.dmass = c.dinertia = c.dv = c.dfext = c.dnormal = c.dp1 = c.dp2 = c.dmu = c.drest = nullptr;
-    c.prof = h->cprof ? h->cprof + (size_t)slot * h->cond_grid * cnd::CPH_COUNT : nullptr;
-  }
-  if (rt.cond_first) {
-#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, rt.cgrid, st)
-    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
-#undef CALL_BWD
-    CK(ce);
-  }
+  memset(&c, 0, sizeof(c));
+  c.g = (const T*)g;
+  c.dQ = (T*)dQ; c.dp = (T*)dp; c.dG = (T*)dG; c.dh = (T*)dh; c.dA = (T*)dA; c.db = (T*)db; c.dF = (T*)dF;
+  c.flags = flags;
   BwdArgs<T> a;
-  a.P = h->plan;
-  a.B = B;
-  a.R = R; a.chunks = rt.dchunks;
-  a.Q = (const T*)Q; a.G = (const T*)G; a.A = (const T*)A; a.F = (const T*)F;
-  a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
+  memset(&a, 0, sizeof(a));
   a.g = (const T*)g;
   a.dQ = (T*)dQ; a.dp = (T*)dp; a.dG = (T*)dG; a.dh = (T*)dh; a.dA = (T*)dA; a.db = (T*)db; a.dF = (T*)dF;
   a.flags = flags;
-  a.Rsave = rt.have_cond ? nullptr : (const T*)Rsave;    // R is only formed when the forward ran on the dual form
-  a.skip = rt.cond_first ? rt.flagbuf : nullptr;
-  a.bad = (rt.have_cond && !rt.cond_first) ? rt.flagbuf : nullptr;
-  a.ws = (T*)h->ws + (size_t)slot * h->plan.ws_per_cta * h->ws_ctas;
-  a.prof = h->prof ? h->prof + (size_t)slot * h->max_grid * PH_COUNT : nullptr;
-  const int mode = h->plan.mode;
-  const cudaError_t le = mode == 0   ? launch_backward_t<T, 0>(a, rt.dgrid, st)
-                         : mode == 1 ? launch_backward_t<T, 1>(a, rt.dgrid, st)
-                                     : launch_backward_t<T, 2>(a, rt.dgrid, st);
-  CK(le);
-  if (rt.have_cond && !rt.cond_first) {
-#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, rt.cgrid, st)
-    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
-#undef CALL_BWD
-    CK(ce);
-  }
-  return 0;
+  return run_dense<T>(h, slot, R, B, Q, G, A, F, zhat, nu, lam, slack, Rsave, sload, c, a, st);
 }
 
 // tg: tangents of (Q, p, G, h, A, b, F), each [R,B,...] or nullptr
@@ -465,56 +477,17 @@ template <typename T>
 static int launch_jvp(lcpb200_handle_s* h, int R, int B, const void* Q, const void* G, const void* A, const void* F,
                       const void* zhat, const void* nu, const void* lam, const void* slack, const void* const (&tg)[7],
                       void* dz, const void* Rsave, cudaStream_t st, const unsigned char* sload) {
-  Route rt;
-  if (int rc = make_route<T>(h, 0, R, B, st, rt)) return rc;
   cnd::CJvpArgs<T> c;
-  if (rt.have_cond) {
-    memset(&c, 0, sizeof(c));
-    c.P = h->cplan;
-    c.B = B;
-    c.R = R; c.chunks = rt.cchunks;
-    c.Q = (const T*)Q; c.G = (const T*)G; c.A = (const T*)A; c.F = (const T*)F;
-    c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
-    c.tQ = (const T*)tg[0]; c.tp = (const T*)tg[1]; c.tG = (const T*)tg[2]; c.th = (const T*)tg[3];
-    c.t_A = (const T*)tg[4]; c.t_b = (const T*)tg[5]; c.tF = (const T*)tg[6];
-    c.done = rt.cond_first ? rt.flagbuf : nullptr;
-    c.only = rt.cond_first ? nullptr : rt.flagbuf;
-    c.sload = sload;
-    c.dz = (T*)dz;
-    c.prof = h->cprof;
-  }
-  if (rt.cond_first) {
-#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, rt.cgrid, st)
-    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
-#undef CALL_JVP
-    CK(ce);
-  }
+  memset(&c, 0, sizeof(c));
+  c.tQ = (const T*)tg[0]; c.tp = (const T*)tg[1]; c.tG = (const T*)tg[2]; c.th = (const T*)tg[3];
+  c.t.A = (const T*)tg[4]; c.t.b = (const T*)tg[5]; c.tF = (const T*)tg[6];
+  c.dz = (T*)dz;
   JvpArgs<T> a;
-  a.P = h->plan;
-  a.B = B;
-  a.R = R; a.chunks = rt.dchunks;
-  a.Q = (const T*)Q; a.G = (const T*)G; a.A = (const T*)A; a.F = (const T*)F;
-  a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
+  memset(&a, 0, sizeof(a));
   a.tQ = (const T*)tg[0]; a.tp = (const T*)tg[1]; a.tG = (const T*)tg[2]; a.th = (const T*)tg[3];
   a.tA = (const T*)tg[4]; a.tb = (const T*)tg[5]; a.tF = (const T*)tg[6];
   a.dz = (T*)dz;
-  a.Rsave = rt.have_cond ? nullptr : (const T*)Rsave;
-  a.skip = rt.cond_first ? rt.flagbuf : nullptr;
-  a.bad = (rt.have_cond && !rt.cond_first) ? rt.flagbuf : nullptr;
-  a.ws = (T*)h->ws;
-  a.prof = h->prof;
-  const int mode = h->plan.mode;
-  const cudaError_t le = mode == 0   ? launch_jvp_t<T, 0>(a, rt.dgrid, st)
-                         : mode == 1 ? launch_jvp_t<T, 1>(a, rt.dgrid, st)
-                                     : launch_jvp_t<T, 2>(a, rt.dgrid, st);
-  CK(le);
-  if (rt.have_cond && !rt.cond_first) {
-#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, rt.cgrid, st)
-    const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
-#undef CALL_JVP
-    CK(ce);
-  }
-  return 0;
+  return run_dense<T>(h, 0, R, B, Q, G, A, F, zhat, nu, lam, slack, Rsave, sload, c, a, st);
 }
 
 static int check_fwd_args(lcpb200_handle_t h, int B, const void* Q, const void* p, const void* G, const void* hv,
@@ -812,16 +785,26 @@ extern "C" int lcpb200_backward_host(lcpb200_handle_t h, int B, const void* Q, c
 // structure-of-arrays the engine holds; no dense Q / G / F is written to or read from HBM, and the
 // backward returns the gradients w.r.t. the contact list (the chain rule through the assembly is
 // applied to the factored gradients inside the kernel).
+// The contact list an engine entry point receives, as the kernels' EngineSoA takes it.
+struct EngineIn {
+  int nb, nc, mode;
+  double dt;
+  const void *mass, *inertia, *v, *fext, *normal, *p1, *p2;
+  const int32_t *b1, *b2, *nc_s;
+  const void *mu, *rest;
+};
+
+// ph: the condensed kernels' buffer for every scene's p and h ([B][n] then [B][m], n the handle's n); nullptr for the
+// banded kernel, which keeps them in its workspace.
 template <typename T>
-static void fill_soa(cnd::EngineSoA<T>& s, lcpb200_handle_s* h, int B, int nb, int nc, int mode, double dt,
-                     const void* mass, const void* inertia, const void* v, const void* fext, const void* normal,
-                     const void* p1, const void* p2, const int32_t* b1, const int32_t* b2, const void* mu,
-                     const void* rest, const int32_t* nc_s = nullptr) {
-  s.mass = (const T*)mass; s.inertia = (const T*)inertia; s.v = (const T*)v; s.fext = (const T*)fext;
-  s.normal = (const T*)normal; s.p1 = (const T*)p1; s.p2 = (const T*)p2; s.mu = (const T*)mu; s.rest = (const T*)rest;
-  s.b1 = b1; s.b2 = b2; s.nc_s = nc_s; s.nb = nb; s.nc = nc; s.mode = mode; s.dt = (T)dt;
-  s.p_s = (T*)h->d_ph.p;
-  s.h_s = s.p_s + (size_t)B * h->n;
+static void fill_soa(cnd::EngineSoA<T>& s, const EngineIn& in, int B, int n, T* ph) {
+  memset(&s, 0, sizeof(s));
+  s.mass = (const T*)in.mass; s.inertia = (const T*)in.inertia; s.v = (const T*)in.v; s.fext = (const T*)in.fext;
+  s.normal = (const T*)in.normal; s.p1 = (const T*)in.p1; s.p2 = (const T*)in.p2; s.mu = (const T*)in.mu;
+  s.rest = (const T*)in.rest;
+  s.b1 = in.b1; s.b2 = in.b2; s.nc_s = in.nc_s; s.nb = in.nb; s.nc = in.nc; s.mode = in.mode; s.dt = (T)in.dt;
+  s.p_s = ph;
+  s.h_s = ph ? ph + (size_t)B * n : nullptr;
 }
 
 // Which kernel family serves the engine entry points of this handle: the condensed-KKT kernels (n + e <= 128,
@@ -869,19 +852,16 @@ static int check_engine(lcpb200_handle_t h, int B, int nb, int nc, int mode) {
 }
 
 template <typename T>
-static int engine_forward_t(lcpb200_handle_s* h, int B, int nb, int nc, int mode, double dt, const void* mass,
-                            const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
-                            const void* p2, const int32_t* b1, const int32_t* b2, const int32_t* ncs, const void* mu,
-                            const void* rest, const void* A, const void* b, double eps, int not_improved_lim, int max_iter, void* zhat,
-                            void* nu, void* lam, void* slack, int32_t* status, int32_t* iters, void* resid,
-                            cudaStream_t st) {
+static int engine_forward_t(lcpb200_handle_s* h, int B, const EngineIn& in, const void* A, const void* b, double eps,
+                            int not_improved_lim, int max_iter, void* zhat, void* nu, void* lam, void* slack,
+                            int32_t* status, int32_t* iters, void* resid, cudaStream_t st) {
   CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
   cnd::CFwdArgs<T> c;
   c.P = h->cplan;
   c.B = B;
   c.Q = nullptr; c.G = nullptr; c.F = nullptr;
   c.A = (const T*)A; c.b = (const T*)b;
-  fill_soa<T>(c.soa, h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, b1, b2, mu, rest, ncs);
+  fill_soa<T>(c.soa, in, B, h->n, (T*)h->d_ph.p);
   c.ssave = nullptr;
   c.p = c.soa.p_s; c.h = c.soa.h_s;
   c.zhat = (T*)zhat; c.nu = (T*)nu; c.lam = (T*)lam; c.slack = (T*)slack; c.resid = (T*)resid;
@@ -912,17 +892,13 @@ extern "C" int lcpb200_engine_forward(lcpb200_handle_t h, int B, int nb, int nc,
   DeviceGuard dg_;
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
+  const EngineIn in{nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2, contact_count, mu, restitution};
   if (use_banded(h)) {
     if (int rc = ensure_bplan(h, B, nb, nc, mode)) return rc;
     bnd::BArgs a;
     a.P = h->bplan;
     a.B = B;
-    memset(&a.soa, 0, sizeof(a.soa));
-    a.soa.mass = (const double*)mass; a.soa.inertia = (const double*)inertia; a.soa.v = (const double*)v;
-    a.soa.fext = (const double*)fext; a.soa.normal = (const double*)normal; a.soa.p1 = (const double*)p1;
-    a.soa.p2 = (const double*)p2; a.soa.mu = (const double*)mu; a.soa.rest = (const double*)restitution;
-    a.soa.b1 = body1; a.soa.b2 = body2; a.soa.nc_s = contact_count; a.soa.nb = nb; a.soa.nc = nc; a.soa.mode = mode;
-    a.soa.dt = dt;
+    fill_soa<double>(a.soa, in, B, h->n, nullptr);
     a.A = (const double*)A; a.b = (const double*)b;
     a.zhat = (double*)zhat; a.nu = (double*)nu; a.lam = (double*)lam; a.slack = (double*)slack; a.resid = (double*)resid;
     a.status = status; a.iters = iters;
@@ -933,41 +909,74 @@ extern "C" int lcpb200_engine_forward(lcpb200_handle_t h, int B, int nb, int nc,
     return 0;
   }
   return h->dtype == LCPB200_F32
-             ? engine_forward_t<float>(h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                       contact_count, mu, restitution, A, b, eps, not_improved_lim, max_iter, zhat, nu, lam, slack, status,
+             ? engine_forward_t<float>(h, B, in, A, b, eps, not_improved_lim, max_iter, zhat, nu, lam, slack, status,
                                        iters, resid, st)
-             : engine_forward_t<double>(h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                        contact_count, mu, restitution, A, b, eps, not_improved_lim, max_iter, zhat, nu, lam, slack, status,
+             : engine_forward_t<double>(h, B, in, A, b, eps, not_improved_lim, max_iter, zhat, nu, lam, slack, status,
                                         iters, resid, st);
 }
 
-template <typename T>
-static int engine_backward_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int mode, double dt, const void* mass,
-                             const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
-                             const void* p2, const int32_t* b1, const int32_t* b2, const int32_t* ncs, const void* mu,
-                             const void* rest, const void* A, const void* zhat, const void* nu, const void* lam, const void* slack,
-                             const void* g, void* dmass, void* dinertia, void* dv, void* dfext, void* dnormal,
-                             void* dp1, void* dp2, void* dmu, void* drest, void* dA, void* db, unsigned flags,
-                             cudaStream_t st) {
-  CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
-  cnd::CBwdArgs<T> c;
-  c.P = h->cplan;
-  c.B = B;
-  c.R = R; c.chunks = bwd_chunks(R, B, h->cond_grid);
-  c.Q = nullptr; c.G = nullptr; c.F = nullptr; c.A = (const T*)A;
-  c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack; c.g = (const T*)g;
-  c.dQ = c.dp = c.dG = c.dh = c.dF = nullptr;
-  c.dA = (T*)dA; c.db = (T*)db;
-  c.done = nullptr; c.only = nullptr; c.flags = flags; c.sload = nullptr;
-  c.prof = h->cprof;
-  fill_soa<T>(c.soa, h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, b1, b2, mu, rest, ncs);
-  c.dmass = (T*)dmass; c.dinertia = (T*)dinertia; c.dv = (T*)dv; c.dfext = (T*)dfext; c.dnormal = (T*)dnormal;
-  c.dp1 = (T*)dp1; c.dp2 = (T*)dp2; c.dmu = (T*)dmu; c.drest = (T*)drest;
-  const int cgrid = (int)std::min((long long)B * c.chunks, (long long)h->cond_grid);
-#define CALL_BWD(NSV) cnd::launch_cond_backward_t<T, NSV>(c, cgrid, st)
-  const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_BWD);
-#undef CALL_BWD
-  CK(ce);
+// Argument checks of the two engine derivative entries; name ("engine_backward", "engine_jvp") prefixes their
+// messages, rhs is the cotangent or the output the entry needs (rhs_name in the message).
+static int check_engine_deriv(lcpb200_handle_t h, const char* name, int R, int B, const EngineIn& in, const void* A,
+                              const void* zhat, const void* nu, const void* lam, const void* slack, const void* rhs,
+                              const char* rhs_name) {
+  if (int rc = check_engine(h, B, in.nb, in.nc, in.mode)) return rc;
+  const std::string nm(name);
+  if (R < 1) return fail(nm + "_batched: need R >= 1");
+  if ((long long)R * B > INT_MAX) return fail(nm + "_batched: R * B exceeds INT_MAX");
+  if (!in.mass || !in.inertia || !in.v || !in.normal || !in.p1 || !in.p2 || !in.b1 || !in.b2 || !in.rest)
+    return fail(nm + ": NULL input");
+  if (in.mode == 0 && !in.mu) return fail(nm + ": mu is needed for mode 0");
+  if (!zhat || !lam || !slack || !rhs) return fail(std::string("zhat, lam, slack, ") + rhs_name + " must be non-NULL");
+  if (h->e > 0 && (!A || !nu)) return fail("A and nu must be non-NULL when e > 0");
+  return 0;
+}
+
+// The fields an engine backward or JVP call fills alike, for the banded kernel (BBwdArgs, BJvpArgs) or the condensed
+// one (CBwdArgs, CJvpArgs): plan, work items and grid, contact list, saved solve. Zeroes the rest.
+template <typename T, typename Args>
+static int engine_deriv_args(lcpb200_handle_s* h, Args& a, int R, int B, const EngineIn& in, const void* A,
+                             const void* zhat, const void* nu, const void* lam, const void* slack, int* grid) {
+  memset(&a, 0, sizeof(a));
+  T* ph = nullptr;
+  int chunks;
+  if constexpr (std::is_same<decltype(a.P), bnd::BPlan>::value) {
+    chunks = bwd_chunks(R, B, h->num_sms);
+    const int items = B * chunks;
+    if (int rc = ensure_bplan(h, items, in.nb, in.nc, in.mode)) return rc;     // one L2 workspace per CTA of this grid
+    a.P = h->bplan;
+    a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
+    *grid = std::min(items, h->num_sms);
+  } else {
+    CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
+    ph = (T*)h->d_ph.p;
+    chunks = bwd_chunks(R, B, h->cond_grid);
+    a.P = h->cplan;
+    *grid = (int)std::min((long long)B * chunks, (long long)h->cond_grid);
+  }
+  a.B = B;
+  a.R = R; a.chunks = chunks;
+  fill_soa<T>(a.soa, in, B, h->n, ph);
+  a.A = (const T*)A;
+  a.zhat = (const T*)zhat; a.nu = (const T*)nu; a.lam = (const T*)lam; a.slack = (const T*)slack;
+  a.prof = h->cprof;
+  return 0;
+}
+
+// dg: the gradient outputs (dmass, dinertia, dv, dfext, dnormal, dp1, dp2, dmu, drest, dA, db), any may be nullptr
+template <typename T, typename Args>
+static int engine_backward_t(lcpb200_handle_s* h, int R, int B, const EngineIn& in, const void* A, const void* zhat,
+                             const void* nu, const void* lam, const void* slack, const void* g,
+                             void* const (&dg)[11], unsigned flags, cudaStream_t st) {
+  Args a;
+  int grid = 0;
+  if (int rc = engine_deriv_args<T>(h, a, R, B, in, A, zhat, nu, lam, slack, &grid)) return rc;
+  a.g = (const T*)g;
+  a.dmass = (T*)dg[0]; a.dinertia = (T*)dg[1]; a.dv = (T*)dg[2]; a.dfext = (T*)dg[3]; a.dnormal = (T*)dg[4];
+  a.dp1 = (T*)dg[5]; a.dp2 = (T*)dg[6]; a.dmu = (T*)dg[7]; a.drest = (T*)dg[8]; a.dA = (T*)dg[9]; a.db = (T*)dg[10];
+  a.flags = flags;
+  if constexpr (std::is_same<Args, bnd::BBwdArgs>::value) CK(bnd::launch_band_backward(a, grid, st));
+  else CK(launch_cond(h, a, grid, st));
   return 0;
 }
 
@@ -980,79 +989,37 @@ extern "C" int lcpb200_engine_backward_batched(lcpb200_handle_t h, int R, int B,
                                                void* dinertia, void* dv, void* dfext, void* dnormal, void* dp1, void* dp2,
                                                void* dmu, void* drestitution, void* dA, void* db, unsigned flags,
                                                void* stream) {
-  if (int rc = check_engine(h, B, nb, nc, mode)) return rc;
-  if (R < 1) return fail("engine_backward_batched: need R >= 1");
-  if ((long long)R * B > INT_MAX) return fail("engine_backward_batched: R * B exceeds INT_MAX");
-  if (!mass || !inertia || !v || !normal || !p1 || !p2 || !body1 || !body2 || !restitution) return fail("engine_backward: NULL input");
-  if (mode == 0 && !mu) return fail("engine_backward: mu is needed for mode 0");
-  if (!zhat || !lam || !slack || !dl_dzhat) return fail("zhat, lam, slack, dl_dzhat must be non-NULL");
-  if (h->e > 0 && (!A || !nu)) return fail("A and nu must be non-NULL when e > 0");
+  const EngineIn in{nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2, contact_count, mu, restitution};
+  if (int rc = check_engine_deriv(h, "engine_backward", R, B, in, A, zhat, nu, lam, slack, dl_dzhat, "dl_dzhat"))
+    return rc;
   if (flags != LCPB200_BWD_BUG_COMPATIBLE && flags != LCPB200_BWD_EXACT_ADJOINT)
     return fail("flags must be LCPB200_BWD_BUG_COMPATIBLE or LCPB200_BWD_EXACT_ADJOINT");
   if (B == 0) return 0;
   DeviceGuard dg_;
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_banded(h)) {
-    const int chunks = bwd_chunks(R, B, h->num_sms);
-    const int items = B * chunks;
-    if (int rc = ensure_bplan(h, items, nb, nc, mode)) return rc;     // one L2 workspace per CTA of this grid
-    bnd::BBwdArgs a;
-    a.P = h->bplan;
-    a.B = B;
-    a.R = R; a.chunks = chunks;
-    memset(&a.soa, 0, sizeof(a.soa));
-    a.soa.mass = (const double*)mass; a.soa.inertia = (const double*)inertia; a.soa.v = (const double*)v;
-    a.soa.fext = (const double*)fext; a.soa.normal = (const double*)normal; a.soa.p1 = (const double*)p1;
-    a.soa.p2 = (const double*)p2; a.soa.mu = (const double*)mu; a.soa.rest = (const double*)restitution;
-    a.soa.b1 = body1; a.soa.b2 = body2; a.soa.nc_s = contact_count; a.soa.nb = nb; a.soa.nc = nc; a.soa.mode = mode;
-    a.soa.dt = dt;
-    a.A = (const double*)A;
-    a.zhat = (const double*)zhat; a.nu = (const double*)nu; a.lam = (const double*)lam; a.slack = (const double*)slack;
-    a.g = (const double*)dl_dzhat;
-    a.dmass = (double*)dmass; a.dinertia = (double*)dinertia; a.dv = (double*)dv; a.dfext = (double*)dfext;
-    a.dnormal = (double*)dnormal; a.dp1 = (double*)dp1; a.dp2 = (double*)dp2; a.dmu = (double*)dmu;
-    a.drest = (double*)drestitution; a.dA = (double*)dA; a.db = (double*)db;
-    a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
-    a.prof = h->cprof;
-    a.flags = flags;
-    CK(bnd::launch_band_backward(a, std::min(items, h->num_sms), st));
-    return 0;
-  }
+  void* const dg[11] = {dmass, dinertia, dv, dfext, dnormal, dp1, dp2, dmu, drestitution, dA, db};
+  if (use_banded(h))
+    return engine_backward_t<double, bnd::BBwdArgs>(h, R, B, in, A, zhat, nu, lam, slack, dl_dzhat, dg, flags, st);
   return h->dtype == LCPB200_F32
-             ? engine_backward_t<float>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                        contact_count, mu, restitution, A, zhat, nu, lam, slack, dl_dzhat, dmass, dinertia, dv, dfext,
-                                        dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, st)
-             : engine_backward_t<double>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                         contact_count, mu, restitution, A, zhat, nu, lam, slack, dl_dzhat, dmass, dinertia, dv, dfext,
-                                         dnormal, dp1, dp2, dmu, drestitution, dA, db, flags, st);
+             ? engine_backward_t<float, cnd::CBwdArgs<float>>(h, R, B, in, A, zhat, nu, lam, slack, dl_dzhat, dg, flags, st)
+             : engine_backward_t<double, cnd::CBwdArgs<double>>(h, R, B, in, A, zhat, nu, lam, slack, dl_dzhat, dg, flags,
+                                                                st);
 }
 
-template <typename T>
-static int engine_jvp_t(lcpb200_handle_s* h, int R, int B, int nb, int nc, int mode, double dt, const void* mass,
-                        const void* inertia, const void* v, const void* fext, const void* normal, const void* p1,
-                        const void* p2, const int32_t* b1, const int32_t* b2, const int32_t* ncs, const void* mu,
-                        const void* rest, const void* A, const void* zhat, const void* nu, const void* lam,
-                        const void* slack, const void* const (&tg)[11], void* dz, cudaStream_t st) {
-  CK(h->d_ph.ensure(sizeof(T) * (size_t)B * (h->n + h->m)));
-  cnd::CJvpArgs<T> c;
-  memset(&c, 0, sizeof(c));              // the dense-path fields (Q, G, F, tQ ... tF, done, only, sload) stay NULL
-  c.P = h->cplan;
-  c.B = B;
-  c.R = R; c.chunks = bwd_chunks(R, B, h->cond_grid);
-  c.A = (const T*)A;
-  c.zhat = (const T*)zhat; c.nu = (const T*)nu; c.lam = (const T*)lam; c.slack = (const T*)slack;
-  fill_soa<T>(c.soa, h, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, b1, b2, mu, rest, ncs);
-  c.t_mass = (const T*)tg[0]; c.t_inertia = (const T*)tg[1]; c.t_v = (const T*)tg[2]; c.t_fext = (const T*)tg[3];
-  c.t_normal = (const T*)tg[4]; c.t_p1 = (const T*)tg[5]; c.t_p2 = (const T*)tg[6]; c.t_mu = (const T*)tg[7];
-  c.t_rest = (const T*)tg[8]; c.t_A = (const T*)tg[9]; c.t_b = (const T*)tg[10];
-  c.dz = (T*)dz;
-  c.prof = h->cprof;
-  const int cgrid = (int)std::min((long long)B * c.chunks, (long long)h->cond_grid);
-#define CALL_JVP(NSV) cnd::launch_cond_jvp_t<T, NSV>(c, cgrid, st)
-  const cudaError_t ce = LCPB200_NS_DISPATCH(h->cplan.NS, CALL_JVP);
-#undef CALL_JVP
-  CK(ce);
+// tg: the tangents (t_mass, t_inertia, t_v, t_fext, t_normal, t_p1, t_p2, t_mu, t_rest, t_A, t_b), nullptr = zero
+template <typename T, typename Args>
+static int engine_jvp_t(lcpb200_handle_s* h, int R, int B, const EngineIn& in, const void* A, const void* zhat,
+                        const void* nu, const void* lam, const void* slack, const void* const (&tg)[11], void* dz,
+                        cudaStream_t st) {
+  Args a;
+  int grid = 0;
+  if (int rc = engine_deriv_args<T>(h, a, R, B, in, A, zhat, nu, lam, slack, &grid)) return rc;
+  a.t = {(const T*)tg[0], (const T*)tg[1], (const T*)tg[2], (const T*)tg[3], (const T*)tg[4], (const T*)tg[5],
+         (const T*)tg[6], (const T*)tg[7], (const T*)tg[8], (const T*)tg[9], (const T*)tg[10]};
+  a.dz = (T*)dz;
+  if constexpr (std::is_same<Args, bnd::BJvpArgs>::value) CK(bnd::launch_band_jvp(a, grid, st));
+  else CK(launch_cond(h, a, grid, st));
   return 0;
 }
 
@@ -1066,50 +1033,18 @@ extern "C" int lcpb200_engine_jvp_batched(lcpb200_handle_t h, int R, int B, int 
                                           const void* t_normal, const void* t_p1, const void* t_p2, const void* t_mu,
                                           const void* t_restitution, const void* t_A, const void* t_b, void* dz,
                                           void* stream) {
-  if (int rc = check_engine(h, B, nb, nc, mode)) return rc;
-  if (R < 1) return fail("engine_jvp_batched: need R >= 1");
-  if ((long long)R * B > INT_MAX) return fail("engine_jvp_batched: R * B exceeds INT_MAX");
-  if (!mass || !inertia || !v || !normal || !p1 || !p2 || !body1 || !body2 || !restitution) return fail("engine_jvp: NULL input");
-  if (mode == 0 && !mu) return fail("engine_jvp: mu is needed for mode 0");
-  if (!zhat || !lam || !slack || !dz) return fail("zhat, lam, slack, dz must be non-NULL");
-  if (h->e > 0 && (!A || !nu)) return fail("A and nu must be non-NULL when e > 0");
+  const EngineIn in{nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2, contact_count, mu, restitution};
+  if (int rc = check_engine_deriv(h, "engine_jvp", R, B, in, A, zhat, nu, lam, slack, dz, "dz")) return rc;
   if (B == 0) return 0;
   const void* const tg[11] = {t_mass, t_inertia, t_v, t_fext, t_normal, t_p1, t_p2, mode == 0 ? t_mu : nullptr,
                               t_restitution, h->e > 0 ? t_A : nullptr, h->e > 0 ? t_b : nullptr};
   DeviceGuard dg_;
   CK(dg_.set(h->device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_banded(h)) {
-    const int chunks = bwd_chunks(R, B, h->num_sms);
-    const int items = B * chunks;
-    if (int rc = ensure_bplan(h, items, nb, nc, mode)) return rc;     // one L2 workspace per CTA of this grid
-    bnd::BJvpArgs a;
-    a.P = h->bplan;
-    a.B = B;
-    a.R = R; a.chunks = chunks;
-    memset(&a.soa, 0, sizeof(a.soa));
-    a.soa.mass = (const double*)mass; a.soa.inertia = (const double*)inertia; a.soa.v = (const double*)v;
-    a.soa.fext = (const double*)fext; a.soa.normal = (const double*)normal; a.soa.p1 = (const double*)p1;
-    a.soa.p2 = (const double*)p2; a.soa.mu = (const double*)mu; a.soa.rest = (const double*)restitution;
-    a.soa.b1 = body1; a.soa.b2 = body2; a.soa.nc_s = contact_count; a.soa.nb = nb; a.soa.nc = nc; a.soa.mode = mode;
-    a.soa.dt = dt;
-    a.A = (const double*)A;
-    a.zhat = (const double*)zhat; a.nu = (const double*)nu; a.lam = (const double*)lam; a.slack = (const double*)slack;
-    a.t_mass = (const double*)tg[0]; a.t_inertia = (const double*)tg[1]; a.t_v = (const double*)tg[2];
-    a.t_fext = (const double*)tg[3]; a.t_normal = (const double*)tg[4]; a.t_p1 = (const double*)tg[5];
-    a.t_p2 = (const double*)tg[6]; a.t_mu = (const double*)tg[7]; a.t_rest = (const double*)tg[8];
-    a.t_A = (const double*)tg[9]; a.t_b = (const double*)tg[10];
-    a.dz = (double*)dz;
-    a.wsd = (double*)h->d_bwsd.p; a.wsi = (int*)h->d_bwsi.p;
-    a.prof = h->cprof;
-    CK(bnd::launch_band_jvp(a, std::min(items, h->num_sms), st));
-    return 0;
-  }
+  if (use_banded(h)) return engine_jvp_t<double, bnd::BJvpArgs>(h, R, B, in, A, zhat, nu, lam, slack, tg, dz, st);
   return h->dtype == LCPB200_F32
-             ? engine_jvp_t<float>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                   contact_count, mu, restitution, A, zhat, nu, lam, slack, tg, dz, st)
-             : engine_jvp_t<double>(h, R, B, nb, nc, mode, dt, mass, inertia, v, fext, normal, p1, p2, body1, body2,
-                                    contact_count, mu, restitution, A, zhat, nu, lam, slack, tg, dz, st);
+             ? engine_jvp_t<float, cnd::CJvpArgs<float>>(h, R, B, in, A, zhat, nu, lam, slack, tg, dz, st)
+             : engine_jvp_t<double, cnd::CJvpArgs<double>>(h, R, B, in, A, zhat, nu, lam, slack, tg, dz, st);
 }
 
 extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc, int mode, double dt,
