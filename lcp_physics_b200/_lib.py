@@ -92,6 +92,11 @@ def ptr(t):
     return ctypes.c_void_p(t.data_ptr())
 
 
+def stream_ptr(device):
+    """The current CUDA stream of `device`, as the `stream` argument of the entry points."""
+    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
 class Handle:
     """Owns one lcpb200 handle (solver plan + workspace) for (dtype, n, m, e, device)."""
 

@@ -20,12 +20,10 @@ Reads from `world` exactly what the reference engine reads (engines.py:27-77):
 and per-body `fric_coeff`, `restitution`; `world.fric_dirs` must be 2
 (world.py:191-192 hard-codes dir2 = -dir1).
 """
-import ctypes
-import math
-
 import torch
 
 from . import _lib
+from ._derivatives import JvpFn, Solve, VjpFn, flatten_directions
 from .lcp import LCPFunction
 
 
@@ -34,10 +32,6 @@ class Engine:
 
     def solve_dynamics(self, world, dt):
         raise NotImplementedError
-
-
-def _stream_ptr(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 class _AssembleFn(torch.autograd.Function):
@@ -59,7 +53,7 @@ class _AssembleFn(torch.autograd.Function):
             _lib.check(lib.lcpb200_assemble(
                 _lib.dtype_code(dt_), B, nb, nc, float(dt),
                 *[_lib.ptr(t) for t in ins], _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(mu_c), _lib.ptr(rest_c),
-                *[_lib.ptr(t) for t in (Q, p, G, h, F)], _stream_ptr(dev)))
+                *[_lib.ptr(t) for t in (Q, p, G, h, F)], _lib.stream_ptr(dev)))
         ctx.save_for_backward(*ins[:3], *ins[4:], mu_c, rest_c, body1, body2)
         ctx.dt = float(dt)
         ctx.dims = (B, nb, nc)
@@ -82,7 +76,7 @@ class _AssembleFn(torch.autograd.Function):
                 _lib.dtype_code(dt_), B, nb, nc, ctx.dt,
                 *[_lib.ptr(t) for t in (mass, inertia, v, normal, p1, p2)], _lib.ptr(body1), _lib.ptr(body2),
                 _lib.ptr(mu), _lib.ptr(rest), *[_lib.ptr(t) for t in up], *[_lib.ptr(t) for t in outs],
-                _stream_ptr(dev)))
+                _lib.stream_ptr(dev)))
         dmass, dinertia, dv, dfext, dnormal, dp1, dp2, dmu, drest = outs
         return dmass, dinertia, dv, dfext, dnormal, dp1, dp2, dmu, drest, None, None, None
 
@@ -94,125 +88,65 @@ def assemble_contacts(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, b
     return _AssembleFn.apply(mass, inertia, v, fext, normal, p1, p2, mu, rest, body1, body2, dt)
 
 
+def _engine_args(meta, saved):
+    """The handle for the current stream and the argument block both engine derivative entries
+    (lcpb200_engine_backward_batched, lcpb200_engine_jvp_batched) take after R: B, nb, nc, mode, dt, the seven
+    inputs, body1, body2, counts, mu, rest, A and the saved zhat, nu, lam, slack. Returns (handle, args, held):
+    the pointers in args point into held, which must outlive the call."""
+    (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = saved
+    dt, mode, _exact, B, nb, nc, e = meta
+    held = [None if t is None else t.contiguous()
+            for t in (mass, inertia, v, fext, normal, p1, p2, body1, body2, counts, mu, rest, A, zhat, nu, lam, slack)]
+    hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, mass.device.index,
+                         torch.cuda.current_stream(mass.device).cuda_stream)
+    return hd, [B, nb, nc, mode, dt] + [_lib.ptr(t) for t in held], held
+
+
 def _engine_backward(dzhat, meta, saved):
     """lcpb200_engine_backward_batched: dzhat [..., B, n] -> the 11 gradients (mass ... rest, A, b), each with
     dzhat's leading dims in front. The leading dims are the R cotangents of one call: each scene's KKT matrix is
     factored once for all of them."""
-    lib = _lib.load()
-    (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = saved
-    dt, mode, exact, B, nb, nc, e = meta
+    _dt, _mode, exact, B, nb, _nc, e = meta
+    mass = saved[0]
     dev = mass.device
-    lead = tuple(dzhat.shape[:-2])
-    g = dzhat.reshape(-1, B, 3 * nb).contiguous()
-    R = g.shape[0]
-    z = lambda t: torch.zeros((R,) + tuple(t.shape), dtype=t.dtype, device=dev)
-    outs = [z(mass), z(inertia), z(v), z(fext), z(normal), z(p1), z(p2), z(mu), z(rest)]
-    dA = z(A) if e > 0 else None
-    db = torch.zeros(R, B, e, dtype=mass.dtype, device=dev) if e > 0 else None
-    ins = [t.contiguous() for t in (mass, inertia, v, fext, normal, p1, p2)]
-    hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, dev.index,
-                         torch.cuda.current_stream(dev).cuda_stream)
+    lead, R, (g,) = flatten_directions([dzhat], [(B, 3 * nb)], mass.dtype, dev)
+    # saved[:10]: mass, inertia, v, fext, normal, p1, p2, mu, rest, A (None when e == 0)
+    outs = [None if t is None else torch.zeros((R,) + tuple(t.shape), dtype=t.dtype, device=dev) for t in saved[:10]]
+    outs.append(torch.zeros(R, B, e, dtype=mass.dtype, device=dev) if e > 0 else None)
+    hd, args, held = _engine_args(meta, saved)
     with torch.cuda.device(dev):
-        _lib.check(lib.lcpb200_engine_backward_batched(
-            hd.raw, R, B, nb, nc, mode, dt, *[_lib.ptr(t) for t in ins],
-            _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu.contiguous()), _lib.ptr(rest.contiguous()),
-            _lib.ptr(A.contiguous() if e > 0 else None), *[_lib.ptr(t) for t in (zhat, nu, lam, slack, g)],
-            *[_lib.ptr(t) for t in outs], _lib.ptr(dA), _lib.ptr(db), 1 if exact else 0, _stream_ptr(dev)))
-    return tuple(None if t is None else t.reshape(lead + tuple(t.shape[1:])) for t in (*outs, dA, db))
-
-
-class _EngineVjpFn(torch.autograd.Function):
-    """The vector-Jacobian product of engine_solve: dl/dzhat and the saved solve in, gradients w.r.t. the contact
-    list out. Under torch.func.vmap (vmap of a torch.func.vjp, jacrev) the cotangents of every vmapped call
-    arrive together and go to ONE batched kernel call, which factors each scene's KKT matrix once for all of them."""
-
-    @staticmethod
-    def forward(dzhat, meta, *saved):
-        return _engine_backward(dzhat, meta, saved)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        pass
-
-    @staticmethod
-    def backward(ctx, *grads):
-        raise NotImplementedError("engine_solve: second derivatives are not implemented")
-
-    @staticmethod
-    def vmap(info, in_dims, dzhat, meta, *saved):
-        if any(d is not None for d in in_dims[2:]):
-            raise NotImplementedError(
-                "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
-                "instead (vmap of the vector-Jacobian product -- torch.func.vjp, jacrev -- is supported)")
-        # one more leading cotangent dim; apply (not forward) so that an enclosing vmap level batches it again
-        outs = _EngineVjpFn.apply(dzhat.movedim(in_dims[0], 0), meta, *saved)
-        return outs, tuple(None if t is None else 0 for t in outs)
-
-
-_TANGENT_INPUTS = 11      # mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b: the inputs a tangent may move
+        _lib.check(_lib.load().lcpb200_engine_backward_batched(
+            hd.raw, R, *args, _lib.ptr(g), *[_lib.ptr(t) for t in outs], 1 if exact else 0, _lib.stream_ptr(dev)))
+    return tuple(None if t is None else t.reshape(lead + tuple(t.shape[1:])) for t in outs)
 
 
 def _engine_jvp(tangents, meta, saved):
     """lcpb200_engine_jvp_batched: tangents of (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, b), each
     [..., *input shape] or None (zero), -> the tangent of zhat [..., B, n]. The leading dims, the same for every
     tangent, are the R directions of one call: each scene's KKT matrix is factored once for all of them."""
-    lib = _lib.load()
-    (mass, inertia, v, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = saved
-    dt, mode, _exact, B, nb, nc, e = meta
+    _dt, _mode, _exact, B, nb, _nc, e = meta
+    mass = saved[0]
     dev = mass.device
-    shapes = [t.shape for t in (mass, inertia, v, fext, normal, p1, p2, mu, rest)]
-    shapes += [A.shape, (B, e)] if e > 0 else [None, None]
-    lead = next((tuple(t.shape[:t.dim() - len(s)]) for t, s in zip(tangents, shapes) if t is not None and s is not None),
-                ())
-    R = math.prod(lead)
-    ts = [None if (t is None or s is None) else t.to(mass.dtype).reshape((R,) + tuple(s)).contiguous()
-          for t, s in zip(tangents, shapes)]
+    if e == 0:
+        tangents = list(tangents[:9]) + [None, None]
+    shapes = [t.shape for t in saved[:9]] + [(B, e, 3 * nb), (B, e)]
+    lead, R, ts = flatten_directions(tangents, shapes, mass.dtype, dev)
     dz = torch.zeros((R, B, 3 * nb), dtype=mass.dtype, device=dev)
     if any(t is not None for t in ts) and R > 0:
-        ins = [t.contiguous() for t in (mass, inertia, v, fext, normal, p1, p2)]
-        hd = _lib.get_handle(mass.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, dev.index,
-                             torch.cuda.current_stream(dev).cuda_stream)
+        hd, args, held = _engine_args(meta, saved)
         with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_engine_jvp_batched(
-                hd.raw, R, B, nb, nc, mode, dt, *[_lib.ptr(t) for t in ins],
-                _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu.contiguous()), _lib.ptr(rest.contiguous()),
-                _lib.ptr(A.contiguous() if e > 0 else None), *[_lib.ptr(t) for t in (zhat, nu, lam, slack)],
-                *[_lib.ptr(t) for t in ts], _lib.ptr(dz), _stream_ptr(dev)))
+            _lib.check(_lib.load().lcpb200_engine_jvp_batched(
+                hd.raw, R, *args, *[_lib.ptr(t) for t in ts], _lib.ptr(dz), _lib.stream_ptr(dev)))
     return dz.reshape(lead + (B, 3 * nb))
 
 
-class _EngineJvpFn(torch.autograd.Function):
-    """The Jacobian-vector product of engine_solve: tangents of the contact list and the saved solve in, the tangent
-    of zhat out. Under torch.func.vmap (jacfwd, vmap of a torch.func.jvp) the tangents of every vmapped call arrive
-    together and go to ONE batched kernel call, which factors each scene's KKT matrix once for all of them."""
-
-    @staticmethod
-    def forward(meta, *args):
-        return _engine_jvp(args[:_TANGENT_INPUTS], meta, args[_TANGENT_INPUTS:])
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        pass
-
-    @staticmethod
-    def backward(ctx, *grads):
-        raise NotImplementedError("engine_solve: second derivatives are not implemented")
-
-    @staticmethod
-    def jvp(ctx, *tangents):
-        raise NotImplementedError("engine_solve: second derivatives are not implemented")
-
-    @staticmethod
-    def vmap(info, in_dims, meta, *args):
-        if any(d is not None for d in in_dims[1 + _TANGENT_INPUTS:]):
-            raise NotImplementedError(
-                "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
-                "instead (vmap of the Jacobian-vector product -- torch.func.jvp, jacfwd -- is supported)")
-        # one more leading tangent dim; a tangent this level does not batch is the same for every direction
-        ts = [None if t is None else (t.movedim(d, 0) if d is not None else t.expand((info.batch_size,) + t.shape))
-              for t, d in zip(args[:_TANGENT_INPUTS], in_dims[1:1 + _TANGENT_INPUTS])]
-        out = _EngineJvpFn.apply(meta, *ts, *args[_TANGENT_INPUTS:])
-        return out, 0
+# VjpFn's and JvpFn's meta: _EngineSolveFn's ctx.meta; saved: its saved tensors
+_ENGINE = Solve(
+    _engine_backward, _engine_jvp, 11, "engine_solve: second derivatives are not implemented",
+    "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 instead (vmap of the "
+    "vector-Jacobian product -- torch.func.vjp, jacrev -- is supported)",
+    "engine_solve: vmap over the inputs of the solve is not supported; batch scenes along dim 0 instead (vmap of the "
+    "Jacobian-vector product -- torch.func.jvp, jacfwd -- is supported)")
 
 
 class _EngineSolveFn(torch.autograd.Function):
@@ -243,7 +177,7 @@ class _EngineSolveFn(torch.autograd.Function):
             _lib.check(lib.lcpb200_engine_forward(
                 hd.raw, B, nb, nc, int(mode), float(dt), *[_lib.ptr(t) for t in ins], _lib.ptr(body1), _lib.ptr(body2),
                 _lib.ptr(counts), _lib.ptr(mu_c), _lib.ptr(rest_c), _lib.ptr(A_c), _lib.ptr(b_c), 1e-12, 3, int(max_iter),
-                *[_lib.ptr(t) for t in (zhat, nu, lam, slack, status, iters, resid)], _stream_ptr(dev)))
+                *[_lib.ptr(t) for t in (zhat, nu, lam, slack, status, iters, resid)], _lib.stream_ptr(dev)))
         _last_info.update(iters=iters, resid=resid, status=status, lam=lam, slack=slack, nu=nu)
         return zhat, status, nu, lam, slack
 
@@ -254,22 +188,22 @@ class _EngineSolveFn(torch.autograd.Function):
         zhat, status, nu, lam, slack = output
         B, nb = mass.shape
         e = A.shape[1] if (A is not None and A.dim() > 1) else 0
-        ctx.save_for_backward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2,
-                              zhat, nu, lam, slack, counts)
-        ctx.save_for_forward(mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2,
-                             zhat, nu, lam, slack, counts)
+        saved = (mass, inertia, v, fext, normal, p1, p2, mu, rest, A if e > 0 else None, body1, body2, zhat, nu, lam,
+                 slack, counts)
+        ctx.save_for_backward(*saved)
+        ctx.save_for_forward(*saved)
         ctx.meta = (float(dt), int(mode), bool(exact), B, nb, normal.shape[1], e)
         ctx.mark_non_differentiable(*[t for t in (status, nu, lam, slack) if t is not None])
 
     @staticmethod
     def backward(ctx, dzhat, *_):
-        grads = _EngineVjpFn.apply(dzhat, ctx.meta, *ctx.saved_tensors)
+        grads = VjpFn.apply(dzhat, _ENGINE, ctx.meta, *ctx.saved_tensors)
         return (*grads, None, None, None, None, None, None, None)
 
     @staticmethod
     def jvp(ctx, *tangents):
         # the true derivative whatever exact_adjoint says: K is factored as the forward factors it
-        dzhat = _EngineJvpFn.apply(ctx.meta, *tangents[:_TANGENT_INPUTS], *ctx.saved_tensors)
+        dzhat = JvpFn.apply(_ENGINE, ctx.meta, *tangents[:_ENGINE.n_tangents], *ctx.saved_tensors)
         return dzhat, None, None, None, None
 
     @staticmethod

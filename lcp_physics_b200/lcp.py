@@ -14,11 +14,10 @@ include/lcpb200.h. CUDA tensors are solved in place on the current stream; CPU
 tensors (what the reference's `World` produces) go through the host-buffer entry
 points, which copy in, solve and copy back. There is no CPU fallback.
 """
-import ctypes
-
 import torch
 
 from . import _lib
+from ._derivatives import JvpFn, Solve, VjpFn, flatten_directions
 
 SINGULAR_Q_MSG = """
 lcp Error: Cannot perform LU factorization on Q.
@@ -54,10 +53,6 @@ def _sizes(Q, p, G, h, A, b, F):
         raise ValueError("A/b have shapes %s/%s, expected %s/%s"
                          % (tuple(A.shape), tuple(b.shape), (B, e, n), (B, e)))
     return B, n, m, e
-
-
-def _stream_ptr(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def solve_forward(Q, p, G, h, A, b, F, eps=1e-12, not_improved_lim=3, max_iter=10, out=None, save=None):
@@ -100,7 +95,7 @@ def solve_forward(Q, p, G, h, A, b, F, eps=1e-12, not_improved_lim=3, max_iter=1
     else:
         hd.fwd_generation += 1
         with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_forward(*args, None, _stream_ptr(dev)))
+            _lib.check(lib.lcpb200_forward(*args, None, _lib.stream_ptr(dev)))
         if save is not None:
             # the library keeps the block structure it found for these inputs; a backward for the SAME inputs
             # may reuse it as long as no other forward ran on this handle in between (LCPB200_BWD_REUSE_STRUCTURE)
@@ -116,17 +111,17 @@ def solve_backward(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need=(True,) * 7,
     the device; CUDA path: a token that lets the backward reuse the block structure the forward found).
     `exact_adjoint`: False = the reference's behaviour (it re-uses the UN-transposed KKT
     factorisation, which is the true adjoint only when F == 0 -- SURVEY.md F6); True = the
-    transposed system (F^T in place of F inside the KKT solve), the exact gradient."""
+    transposed system (F^T in place of F inside the KKT solve), the exact gradient.
+    CUDA inputs take solve_backward_batched with one cotangent; CPU inputs the host-buffer path."""
+    if G.device.type == "cuda":
+        return solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need, saved=saved,
+                                      exact_adjoint=exact_adjoint, out=out)
     _lib.require_cuda()
     lib = _lib.load()
     B, m, n = G.shape
     e = A.shape[1] if (A is not None and A.dim() > 1) else 0
-    dtype, dev = G.dtype, G.device
-    on_host = dev.type != "cuda"
-    dev_index = torch.cuda.current_device() if on_host else dev.index
-    hd = _lib.get_handle(dtype, n, m, e, dev_index,
-                         "host" if on_host else torch.cuda.current_stream(dev).cuda_stream)
-    mk = lambda *shape: torch.empty(*shape, dtype=dtype, device=dev)
+    dtype = G.dtype
+    hd = _lib.get_handle(dtype, n, m, e, torch.cuda.current_device(), "host")
     shapes = [(B, n, n), (B, n), (B, m, n), (B, m), (B, e, n), (B, e), (B, m, m)]
     outs = []
     for k, shp in enumerate(shapes):
@@ -134,32 +129,32 @@ def solve_backward(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need=(True,) * 7,
         if out is not None:
             outs.append(out[k] if want else None)
         else:
-            outs.append(mk(*shp) if want else None)
+            outs.append(torch.empty(*shp, dtype=dtype, device=G.device) if want else None)
     if B == 0:
         return tuple(outs)
     ins = [Q.contiguous(), G.contiguous(), A.contiguous() if e > 0 else None, F.contiguous(),
            zhat.contiguous(), nu.contiguous() if e > 0 else None, lam.contiguous(), slack.contiguous(),
            dl_dzhat.contiguous().to(dtype)]
-    if on_host:
-        tok = saved.get("token") if saved else None
-        if tok is not None and tok[0] is hd and tok[1] == hd.host_generation and tok[2] == B:
-            in_ptrs = [None] * 8 + [_lib.ptr(ins[8])]          # reuse what forward_host left on the device
-        else:
-            in_ptrs = [_lib.ptr(t) for t in ins]
-        hd.host_generation += 1
-        _lib.check(lib.lcpb200_backward_host(hd.raw, B, *in_ptrs, *[_lib.ptr(t) for t in outs], 1 if exact_adjoint else 0))
+    if _reuses(saved, "token", hd, hd.host_generation, B):
+        in_ptrs = [None] * 8 + [_lib.ptr(ins[8])]          # reuse what forward_host left on the device
     else:
-        tok = saved.get("struct") if saved else None
-        reuse = tok is not None and tok[0] is hd and tok[1] == hd.fwd_generation and tok[2] == B
-        flags = (1 if exact_adjoint else 0) | (2 if reuse else 0)
-        args = [hd.raw, B] + [_lib.ptr(t) for t in ins] + [_lib.ptr(t) for t in outs] + [None, flags]
-        with torch.cuda.device(dev):
-            _lib.check(lib.lcpb200_backward(*args, _stream_ptr(dev)))
+        in_ptrs = [_lib.ptr(t) for t in ins]
+    hd.host_generation += 1
+    _lib.check(lib.lcpb200_backward_host(hd.raw, B, *in_ptrs, *[_lib.ptr(t) for t in outs], 1 if exact_adjoint else 0))
     return tuple(outs)
 
 
-def _to_device(ts, dev):
-    return [None if t is None else t.to(dev) for t in ts]
+def _reuses(saved, kind, hd, generation, B):
+    """True when `saved`, filled by solve_forward(save=...), holds the token of the last forward on handle hd
+    (generation) for B scenes: "struct" for the block structure of the device path, "token" for the state the host
+    path retained."""
+    return bool(saved) and saved.get(kind) == (hd, generation, B)
+
+
+def _saved_on(run, home, e, Q, G, A, F, zhat, nu, lam, slack):
+    """The saved solve as the batched dense entries take it: contiguous, on the device the call runs on."""
+    return [None if t is None else (t.contiguous() if home == run else t.to(run).contiguous())
+            for t in (Q, G, A if e > 0 else None, F, zhat, nu if e > 0 else None, lam, slack)]
 
 
 def _device_call(dev):
@@ -169,40 +164,35 @@ def _device_call(dev):
     return torch.device("cuda", torch.cuda.current_device()), dev
 
 
-def _reuse_flag(saved, hd, B):
-    tok = saved.get("struct") if saved else None
-    return 2 if (tok is not None and tok[0] is hd and tok[1] == hd.fwd_generation and tok[2] == B) else 0
-
-
 def solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dl_dzhat, need=(True,) * 7, saved=None,
-                           exact_adjoint=False):
+                           exact_adjoint=False, out=None):
     """lcpb200_backward_batched: dl_dzhat [..., B, n] -> (dQ, dp, dG, dh, dA, db, dF), each with dl_dzhat's leading
     dims in front; entries not needed (or dA/db when e == 0) are None. The leading dims are the R cotangents of one
     call: each scene's KKT matrix is factored once for all of them. Slot r equals solve_backward(dl_dzhat[r]).
-    CPU inputs are copied to the current CUDA device and the gradients copied back."""
+    CPU inputs are copied to the current CUDA device and the gradients copied back. `out`: preallocated results,
+    shaped as returned, written in place (for CPU inputs, after the copy back)."""
     _lib.require_cuda()
     lib = _lib.load()
     B, m, n = G.shape
     e = A.shape[1] if (A is not None and A.dim() > 1) else 0
     dtype = G.dtype
     run, home = _device_call(G.device)
-    lead = tuple(dl_dzhat.shape[:-2])
-    R = 1
-    for d in lead:
-        R *= d
+    lead, R, (g,) = flatten_directions([dl_dzhat], [(B, n)], dtype, run)
     shapes = [(n, n), (n,), (m, n), (m,), (e, n), (e,), (m, m)]
-    outs = [torch.empty((R, B) + s, dtype=dtype, device=run) if (need[k] and not (k in (4, 5) and e == 0)) else None
-            for k, s in enumerate(shapes)]
+    into = out is not None and home == run
+    outs = [(out[k] if into else torch.empty(*lead, B, *s, dtype=dtype, device=run))
+            if (need[k] and not (k in (4, 5) and e == 0)) else None for k, s in enumerate(shapes)]
     if R > 0 and B > 0:
-        ins = _to_device([Q, G, A if e > 0 else None, F, zhat, nu if e > 0 else None, lam, slack], run)
-        ins = [None if t is None else t.contiguous() for t in ins]
-        g = dl_dzhat.to(device=run, dtype=dtype).reshape(R, B, n).contiguous()
+        ins = _saved_on(run, home, e, Q, G, A, F, zhat, nu, lam, slack)
         hd = _lib.get_handle(dtype, n, m, e, run.index, torch.cuda.current_stream(run).cuda_stream)
-        flags = (1 if exact_adjoint else 0) | (_reuse_flag(saved, hd, B) if home.type == "cuda" else 0)
+        reuse = home == run and _reuses(saved, "struct", hd, hd.fwd_generation, B)
+        flags = (1 if exact_adjoint else 0) | (2 if reuse else 0)
         with torch.cuda.device(run):
             _lib.check(lib.lcpb200_backward_batched(hd.raw, R, B, *[_lib.ptr(t) for t in ins], _lib.ptr(g),
-                                                    *[_lib.ptr(t) for t in outs], None, flags, _stream_ptr(run)))
-    return tuple(None if t is None else t.to(home).reshape(lead + tuple(t.shape[1:])) for t in outs)
+                                                    *[_lib.ptr(t) for t in outs], None, flags, _lib.stream_ptr(run)))
+    if home != run:
+        outs = [None if t is None else (t.to(home) if out is None else out[k].copy_(t)) for k, t in enumerate(outs)]
+    return tuple(outs)
 
 
 def solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, tangents, saved=None):
@@ -216,92 +206,39 @@ def solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, tangents, saved=None):
     e = A.shape[1] if (A is not None and A.dim() > 1) else 0
     dtype = G.dtype
     run, home = _device_call(G.device)
-    shapes = [(B, n, n), (B, n), (B, m, n), (B, m), (B, e, n), (B, e), (B, m, m)]
     if e == 0:
         tangents = list(tangents[:4]) + [None, None] + [tangents[6]]
-    lead = next((tuple(t.shape[:t.dim() - len(s)]) for t, s in zip(tangents, shapes) if t is not None), ())
-    R = 1
-    for d in lead:
-        R *= d
-    ts = [None if t is None else t.to(device=run, dtype=dtype).reshape((R,) + s).contiguous()
-          for t, s in zip(tangents, shapes)]
+    lead, R, ts = flatten_directions(tangents, [(B, n, n), (B, n), (B, m, n), (B, m), (B, e, n), (B, e), (B, m, m)],
+                                     dtype, run)
     dz = torch.zeros((R, B, n), dtype=dtype, device=run)
     if R > 0 and B > 0 and any(t is not None for t in ts):
-        ins = _to_device([Q, G, A if e > 0 else None, F, zhat, nu if e > 0 else None, lam, slack], run)
-        ins = [None if t is None else t.contiguous() for t in ins]
+        ins = _saved_on(run, home, e, Q, G, A, F, zhat, nu, lam, slack)
         hd = _lib.get_handle(dtype, n, m, e, run.index, torch.cuda.current_stream(run).cuda_stream)
-        flags = _reuse_flag(saved, hd, B) if home.type == "cuda" else 0
+        flags = 2 if home == run and _reuses(saved, "struct", hd, hd.fwd_generation, B) else 0
         with torch.cuda.device(run):
             _lib.check(lib.lcpb200_jvp_batched(hd.raw, R, B, *[_lib.ptr(t) for t in ins], *[_lib.ptr(t) for t in ts],
-                                               _lib.ptr(dz), None, flags, _stream_ptr(run)))
+                                               _lib.ptr(dz), None, flags, _lib.stream_ptr(run)))
     return dz.to(home).reshape(lead + (B, n))
 
 
-_SECOND = "LCPFunction: second derivatives are not implemented"
+def _lcp_vjp(dzhat, meta, saved):
+    need, state, exact = meta
+    zhat, Q, G, A, F, nu, lam, slack = saved
+    if dzhat.dim() == 2:        # LCPFunction's backward: CPU inputs keep the host path and its retained state
+        return solve_backward(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
+    return solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
+
+
+def _lcp_jvp(tangents, state, saved):
+    zhat, Q, G, A, F, nu, lam, slack = saved
+    return solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, tangents, saved=state)
+
+
 _BATCHED_PRIMAL = ("LCPFunction: vmap over the inputs of the solve is not supported; batch scenes along dim 0 "
                    "instead (vmap of its vector-Jacobian and Jacobian-vector products -- jacrev, jacfwd -- is supported)")
-
-
-class _LCPVjpFn(torch.autograd.Function):
-    """The vector-Jacobian product of LCPFunction: dl/dzhat and the saved solve in, the seven gradients out. One
-    cotangent [B, n] is today's backward (solve_backward); under torch.func.vmap (vmap of a torch.func.vjp, jacrev)
-    the cotangents of every vmapped call arrive together and go to ONE lcpb200_backward_batched call."""
-
-    @staticmethod
-    def forward(dzhat, meta, *saved):
-        need, state, exact = meta
-        zhat, Q, G, A, F, nu, lam, slack = saved
-        if dzhat.dim() == 2:
-            return solve_backward(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
-        return solve_backward_batched(Q, G, A, F, zhat, nu, lam, slack, dzhat, need, saved=state, exact_adjoint=exact)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        pass
-
-    @staticmethod
-    def backward(ctx, *grads):
-        raise NotImplementedError(_SECOND)
-
-    @staticmethod
-    def vmap(info, in_dims, dzhat, meta, *saved):
-        if any(d is not None for d in in_dims[2:]):
-            raise NotImplementedError(_BATCHED_PRIMAL)
-        # one more leading cotangent dim; apply (not forward) so that an enclosing vmap level batches it again
-        outs = _LCPVjpFn.apply(dzhat.movedim(in_dims[0], 0), meta, *saved)
-        return outs, tuple(None if t is None else 0 for t in outs)
-
-
-class _LCPJvpFn(torch.autograd.Function):
-    """The Jacobian-vector product of LCPFunction: tangents of (Q, p, G, h, A, b, F) and the saved solve in, the
-    tangent of zhat out. Under torch.func.vmap (jacfwd, vmap of a torch.func.jvp) the tangents of every vmapped call
-    arrive together and go to ONE lcpb200_jvp_batched call."""
-
-    @staticmethod
-    def forward(state, *args):
-        zhat, Q, G, A, F, nu, lam, slack = args[7:]
-        return solve_jvp_batched(Q, G, A, F, zhat, nu, lam, slack, args[:7], saved=state)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        pass
-
-    @staticmethod
-    def backward(ctx, *grads):
-        raise NotImplementedError(_SECOND)
-
-    @staticmethod
-    def jvp(ctx, *tangents):
-        raise NotImplementedError(_SECOND)
-
-    @staticmethod
-    def vmap(info, in_dims, state, *args):
-        if any(d is not None for d in in_dims[8:]):
-            raise NotImplementedError(_BATCHED_PRIMAL)
-        # one more leading tangent dim; a tangent this level does not batch is the same for every direction
-        ts = [None if t is None else (t.movedim(d, 0) if d is not None else t.expand((info.batch_size,) + t.shape))
-              for t, d in zip(args[:7], in_dims[1:8])]
-        return _LCPJvpFn.apply(state, *ts, *args[7:]), 0
+# VjpFn's meta: (need, forward's save dict, exact_adjoint); JvpFn's: the save dict. saved: _LCPFn.setup_context's.
+_LCP = Solve(_lcp_vjp, _lcp_jvp, 7, "LCPFunction: second derivatives are not implemented", _BATCHED_PRIMAL,
+             _BATCHED_PRIMAL)
 
 
 class _LCPFn(torch.autograd.Function):
@@ -338,13 +275,13 @@ class _LCPFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dl_dzhat, *_):
         need = tuple(ctx.needs_input_grad[:7])
-        grads = _LCPVjpFn.apply(dl_dzhat, (need, ctx.state, ctx.exact_adjoint), *ctx.saved_tensors)
+        grads = VjpFn.apply(dl_dzhat, _LCP, (need, ctx.state, ctx.exact_adjoint), *ctx.saved_tensors)
         return (*grads, None)
 
     @staticmethod
     def jvp(ctx, tQ, tp, tG, th, tA, tb, tF, _):
         # the true derivative whatever exact_adjoint says: K is factored as the forward factors it
-        dz = _LCPJvpFn.apply(ctx.state, tQ, tp, tG, th, tA, tb, tF, *ctx.saved_tensors)
+        dz = JvpFn.apply(_LCP, ctx.state, tQ, tp, tG, th, tA, tb, tF, *ctx.saved_tensors)
         return dz, None, None, None
 
     @staticmethod

@@ -34,7 +34,6 @@ Everything is differentiable through torch autograd (the LCP through lcpb200_eng
 42 dynamic bodies (3 (nb + npoly) + 3 n_static <= 128) use the condensed-KKT kernels (fp32 / fp64); larger scenes
 (BASELINE config 4: a 512-ball pile) the banded large-scene kernels (csrc/lcp_banded.cuh), float64.
 """
-import ctypes
 import math
 
 import torch
@@ -507,8 +506,7 @@ class BatchedWorld:
                 _lib.check(lib.lcpb200_contacts(
                     _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps,
                     *[_lib.ptr(t) for t in ins[:-1]], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat),
-                    *[_lib.ptr(t) for t in geo], _lib.ptr(ins[-1]),
-                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                    *[_lib.ptr(t) for t in geo], _lib.ptr(ins[-1]), _lib.stream_ptr(dev)))
             # tensors only: _DetectFn marks every output non-differentiable
             return tuple(t for t in (b1, b2, counts, feat, *geo) if t is not None)
         # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the

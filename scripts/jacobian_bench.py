@@ -12,7 +12,6 @@ its power limit.
     python scripts/jacobian_bench.py [--rounds 3] [--batch 1024]
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -22,7 +21,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from lcp_physics_b200 import _lib  # noqa: E402
-from lcp_physics_b200.engines import engine_solve  # noqa: E402
+from lcp_physics_b200.engines import _engine_args, engine_solve  # noqa: E402
 from lcp_physics_b200.scenes import make_ball_pile  # noqa: E402
 from lcp_physics_b200.world import BatchedWorld  # noqa: E402
 from scripts.joint_bench import chain_world  # noqa: E402
@@ -47,36 +46,32 @@ def timed(fn):
 
 
 def kernel_legs(w, R):
-    """The two legs of (a) on the saved solve of w's current contact list: callables and a result check."""
+    """The two legs of (a) on the saved solve of w's current contact list: callables, and the tensors their
+    arguments point into (kept alive by the caller while the legs run)."""
     lib = _lib.load()
     v = w.v.detach().clone().requires_grad_(True)
     b = w.v.new_zeros(w.B, w.ne) if w.ne else None
-    z, _ = engine_solve(w.mass, w.inertia, v, w.fext, w.c_normal, w.c_p1, w.c_p2, w.c_mu, w.c_rest, w.c_b1, w.c_b2, w.dt,
-                        A=w.A, b=b, mode=0, max_iter=w.max_iter, exact_adjoint=w.exact_adjoint, counts=w.counts)
-    ctx = z.grad_fn
-    (mass, inertia, vv, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = ctx.saved_tensors
-    dt, mode, exact, B, nb, nc, e = ctx.meta
-    G = torch.randn(R, B, 3 * nb, dtype=z.dtype, device=z.device, generator=torch.Generator("cuda").manual_seed(0))
+    inputs = (w.mass, w.inertia, v, w.fext, w.c_normal, w.c_p1, w.c_p2, w.c_mu, w.c_rest)
+    z, _ = engine_solve(*inputs, w.c_b1, w.c_b2, w.dt, A=w.A, b=b, mode=0, max_iter=w.max_iter,
+                        exact_adjoint=w.exact_adjoint, counts=w.counts)
+    hd, args, held = _engine_args(z.grad_fn.meta, z.grad_fn.saved_tensors)
+    gen = torch.Generator("cuda").manual_seed(0)
+    G = torch.randn((R,) + tuple(z.shape), dtype=z.dtype, device=z.device, generator=gen)
     o = lambda t: torch.zeros((R,) + tuple(t.shape), dtype=t.dtype, device=t.device)
-    outs = [o(t) for t in (mass, inertia, vv, fext, normal, p1, p2, mu, rest)]
-    outs += [o(A), torch.zeros(R, B, e, dtype=z.dtype, device=z.device)] if e else [None, None]
-    hd = _lib.get_handle(z.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, z.device.index,
-                         torch.cuda.current_stream().cuda_stream)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    ins = [_lib.ptr(t) for t in (mass, inertia, vv, fext, normal, p1, p2)] + [
-        _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu), _lib.ptr(rest), _lib.ptr(A),
-        _lib.ptr(zhat), _lib.ptr(nu), _lib.ptr(lam), _lib.ptr(slack)]
-    flags = 1 if exact else 0
+    outs = [o(t) for t in inputs]
+    outs += [o(w.A), torch.zeros(R, w.B, w.ne, dtype=z.dtype, device=z.device)] if w.ne else [None, None]
+    st = _lib.stream_ptr(z.device)
+    flags = 1 if w.exact_adjoint else 0
 
     def batched():
-        _lib.check(lib.lcpb200_engine_backward_batched(hd.raw, R, B, nb, nc, mode, dt, *ins, _lib.ptr(G),
-                                                       *[_lib.ptr(t) for t in outs], flags, st))
+        _lib.check(lib.lcpb200_engine_backward_batched(hd.raw, R, *args, _lib.ptr(G), *[_lib.ptr(t) for t in outs],
+                                                       flags, st))
 
     def sequential():
         for r in range(R):
-            _lib.check(lib.lcpb200_engine_backward(hd.raw, B, nb, nc, mode, dt, *ins, _lib.ptr(G[r]),
+            _lib.check(lib.lcpb200_engine_backward(hd.raw, *args, _lib.ptr(G[r]),
                                                    *[_lib.ptr(None if t is None else t[r]) for t in outs], flags, st))
-    return batched, sequential
+    return batched, sequential, held
 
 
 def autograd_rows(w):
@@ -130,7 +125,7 @@ def main():
         R = 2 * w.n
         extra = {"B": w.B, "n": w.n, "R": R, "mean_contacts_per_world": float(w.counts.float().mean()),
                  "banded_kernel": w.large}
-        batched, sequential = kernel_legs(w, R)
+        batched, sequential, held = kernel_legs(w, R)
         batched()
         sequential()                                           # warm-up of both legs
         torch.cuda.synchronize()

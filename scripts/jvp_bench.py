@@ -14,7 +14,6 @@ max) of every leg, peak memory where measured, the card and its power limit.
     python scripts/jvp_bench.py [--rounds 5] [--batch 1024] [--steps 30]
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -24,7 +23,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from lcp_physics_b200 import _lib  # noqa: E402
-from lcp_physics_b200.engines import engine_solve  # noqa: E402
+from lcp_physics_b200.engines import _engine_args, engine_solve  # noqa: E402
 from lcp_physics_b200.scenes import make_ball_pile  # noqa: E402
 from lcp_physics_b200.world import BatchedWorld  # noqa: E402
 from scripts.obstacle_bench import card  # noqa: E402
@@ -65,44 +64,38 @@ def peak(fn):
 
 
 def kernel_legs(w, R):
-    """(a) on the saved solve of w's current contact list: batched JVP, R single-tangent JVPs, batched VJP."""
+    """(a) on the saved solve of w's current contact list: batched JVP, R single-tangent JVPs, batched VJP; and the
+    tensors their arguments point into (kept alive by the caller while the legs run)."""
     lib = _lib.load()
     v = w.v.detach().clone().requires_grad_(True)
     b = w.v.new_zeros(w.B, w.ne) if w.ne else None
-    z, _ = engine_solve(w.mass, w.inertia, v, w.fext, w.c_normal, w.c_p1, w.c_p2, w.c_mu, w.c_rest, w.c_b1, w.c_b2, w.dt,
-                        A=w.A, b=b, mode=0, max_iter=w.max_iter, exact_adjoint=True, counts=w.counts)
-    ctx = z.grad_fn
-    (mass, inertia, vv, fext, normal, p1, p2, mu, rest, A, body1, body2, zhat, nu, lam, slack, counts) = ctx.saved_tensors
-    dt, mode, exact, B, nb, nc, e = ctx.meta
+    inputs = (w.mass, w.inertia, v, w.fext, w.c_normal, w.c_p1, w.c_p2, w.c_mu, w.c_rest)
+    z, _ = engine_solve(*inputs, w.c_b1, w.c_b2, w.dt, A=w.A, b=b, mode=0, max_iter=w.max_iter, exact_adjoint=True,
+                        counts=w.counts)
+    hd, args, held = _engine_args(z.grad_fn.meta, z.grad_fn.saved_tensors)
     gen = torch.Generator("cuda").manual_seed(0)
     rnd = lambda t: torch.randn((R,) + tuple(t.shape), dtype=t.dtype, device=t.device, generator=gen)
-    tg = [rnd(t) for t in (mass, inertia, vv, fext, normal, p1, p2, mu, rest)] + ([rnd(A), rnd(nu)] if e else [None] * 2)
-    dz = torch.zeros(R, B, 3 * nb, dtype=z.dtype, device=z.device)
-    G = rnd(zhat)
+    tg = [rnd(t) for t in inputs] + ([rnd(w.A), rnd(b)] if w.ne else [None] * 2)
+    dz = torch.zeros((R,) + tuple(z.shape), dtype=z.dtype, device=z.device)
+    G = rnd(z)
     o = lambda t: torch.zeros((R,) + tuple(t.shape), dtype=t.dtype, device=t.device)
-    outs = [o(t) for t in (mass, inertia, vv, fext, normal, p1, p2, mu, rest)] + ([o(A), o(nu)] if e else [None] * 2)
-    hd = _lib.get_handle(z.dtype, 3 * nb, (4 if mode == 0 else 1) * nc, e, z.device.index,
-                         torch.cuda.current_stream().cuda_stream)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    ins = [_lib.ptr(t) for t in (mass, inertia, vv, fext, normal, p1, p2)] + [
-        _lib.ptr(body1), _lib.ptr(body2), _lib.ptr(counts), _lib.ptr(mu), _lib.ptr(rest), _lib.ptr(A),
-        _lib.ptr(zhat), _lib.ptr(nu), _lib.ptr(lam), _lib.ptr(slack)]
+    outs = [o(t) for t in inputs] + ([o(w.A), o(b)] if w.ne else [None] * 2)
+    st = _lib.stream_ptr(z.device)
 
     def jvp_batched():
-        _lib.check(lib.lcpb200_engine_jvp_batched(hd.raw, R, B, nb, nc, mode, dt, *ins, *[_lib.ptr(t) for t in tg],
-                                                  _lib.ptr(dz), st))
+        _lib.check(lib.lcpb200_engine_jvp_batched(hd.raw, R, *args, *[_lib.ptr(t) for t in tg], _lib.ptr(dz), st))
 
     def jvp_sequential():
         for r in range(R):
-            _lib.check(lib.lcpb200_engine_jvp_batched(hd.raw, 1, B, nb, nc, mode, dt, *ins,
+            _lib.check(lib.lcpb200_engine_jvp_batched(hd.raw, 1, *args,
                                                       *[_lib.ptr(None if t is None else t[r]) for t in tg],
                                                       _lib.ptr(dz[r]), st))
 
     def vjp_batched():
-        _lib.check(lib.lcpb200_engine_backward_batched(hd.raw, R, B, nb, nc, mode, dt, *ins, _lib.ptr(G),
-                                                       *[_lib.ptr(t) for t in outs], 1, st))
+        _lib.check(lib.lcpb200_engine_backward_batched(hd.raw, R, *args, _lib.ptr(G), *[_lib.ptr(t) for t in outs], 1,
+                                                       st))
     return {"jvp_batched_one_call": jvp_batched, "jvp_R_single_calls": jvp_sequential,
-            "vjp_batched_one_call": vjp_batched}
+            "vjp_batched_one_call": vjp_batched}, held
 
 
 def rollout_legs(B, nballs, cols, seed, steps):
@@ -152,7 +145,7 @@ def main():
     w.step()
     torch.cuda.synchronize()
     for R in (3, w.n):
-        legs = kernel_legs(w, R)
+        legs, held = kernel_legs(w, R)
         for fn in legs.values():
             fn()                                                   # warm-up
         torch.cuda.synchronize()
