@@ -252,6 +252,28 @@ int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, 
                      void* p1, void* p2, void* penetration, void* mu, void* restitution_c,
                      const uint32_t* no_contact, void* stream);
 
+/* lcpb200_contacts for a batch whose scenes hold different bodies: scene s takes part with the bodies whose bit is set
+ * in active[s] and walks the pairs of those bodies only, so its contact list is that of the world holding just its
+ * active bodies (same rules, same lexicographic order, body indices of the full list) and its walk costs its own
+ * pairs. The arguments are those of lcpb200_contacts, plus:
+ *   no_contact                                        NULL, or per-scene pair masks in the layout of lcpb200_contacts:
+ *                                                     scene s reads the mask at no_contact + s * no_contact_stride
+ *                                                     (in uint32 words; stride 0: one mask shared by the batch), with
+ *                                                     the bit of the pair's body indices
+ *   active[B, ceil(nt / 32)] uint32                   NULL (every body active), or bit k % 32 of word k / 32 of row s
+ *                                                     set iff body k of [circles, polygons, obstacles] is active in
+ *                                                     scene s; bits at k >= nt are ignored
+ * feat is required; nt = nb + np + no <= 8192 (the active list of a scene is kept in shared memory), else an error.
+ * Padding pairs and feat of unused slots are those of lcpb200_contacts. With every body active and a shared mask the
+ * outputs equal lcpb200_contacts'. */
+int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
+                            const void* rad, const void* fric, const void* rest, const void* pverts, const void* pcen,
+                            const void* pfric, const void* prest, const void* overts, const void* oref,
+                            const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
+                            int32_t* feat, void* normal, void* p1, void* p2, void* penetration, void* mu,
+                            void* restitution_c, const uint32_t* no_contact, long long no_contact_stride,
+                            const uint32_t* active, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

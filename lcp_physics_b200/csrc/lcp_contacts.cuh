@@ -24,6 +24,9 @@
 // obstacles, np == 0), one contact per pair at most. MASK == true (lcpb200_contacts with no_contact) reads a
 // pair-exclusion bitmask shared by the batch and skips an excluded pair before
 // any rule is evaluated, as the reference's `if geom1 in geom2.no_contact: return` (contacts.py:60, add_no_contact).
+// ACTIVE == true (lcpb200_contacts_active) walks each scene over its own active bodies: the CTA first compacts the
+// scene's active body indices into shared memory, then walks the pairs of that sub-list, so a scene pays for its own
+// pairs only and its contacts come in the order of the world that holds just its active bodies.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,6 +37,7 @@ namespace cts {
 constexpr int NT = 256;
 constexpr int ITEMS = 4;            // consecutive pairs per thread and chunk
 constexpr int MAX_NV = 256;         // vertices per polygon (feat packs edge indices in 8 bits)
+constexpr int MAX_ACTIVE_NT = 8192; // bodies of a world walked with per-scene activity (uint16 list, 16 KB of smem)
 
 // number of pairs (i', j') with i' < i, i.e. index of pair (i, i + 1), in a list of nt bodies
 __host__ __device__ __forceinline__ long long pairs_before(long long i, long long nt) { return i * (2 * nt - i - 1) / 2; }
@@ -280,69 +284,116 @@ __host__ __device__ int hull_hull(const T* __restrict__ P1, const T* __restrict_
 // feat [B, cap] (HULLS only, may be nullptr): the hull-hull features, -1 for every other contact.
 // no_contact (MASK only): bit i * nt + j (i < j, nt = nb + np + no) set iff the pair (i, j) never makes contact; an
 // excluded pair sets no hit bit, so the compaction keeps the order of the remaining pairs.
-template <typename T, bool HULLS, bool MASK = false>
+// ACTIVE (with HULLS and MASK; nt <= MAX_ACTIVE_NT): active [B, ceil(nt / 32)] (nullptr: every body active), bit k of
+// scene s set iff body k takes part in scene s. The scene's active bodies are listed in index order (dynamic bodies
+// first, then obstacles, as in the body list); the pairs are enumerated over that list's counts (nd_s, nt_s) and
+// mapped back to body indices, which everything after the decode uses (the mask, the rule dispatch, the outputs).
+// no_contact may be nullptr; otherwise scene s reads its mask at no_contact + s * nc_stride (stride 0: one mask for
+// the batch).
+template <typename T, bool HULLS, bool MASK = false, bool ACTIVE = false>
 __global__ void __launch_bounds__(NT) find_contacts_kernel(Bodies<T> bd, int B, int cap, T eps,
                                                            int32_t* __restrict__ body1, int32_t* __restrict__ body2,
                                                            int32_t* __restrict__ feat, int32_t* __restrict__ counts,
-                                                           const uint32_t* __restrict__ no_contact = nullptr) {
+                                                           const uint32_t* __restrict__ no_contact = nullptr,
+                                                           const uint32_t* __restrict__ active = nullptr,
+                                                           long long nc_stride = 0) {
+  static_assert(!ACTIVE || (HULLS && MASK), "the active walk is the polygon walk with a per-scene mask");
   __shared__ int warp_tot[NT / 32];
+  __shared__ uint16_t act[ACTIVE ? MAX_ACTIVE_NT : 1];           // ACTIVE: the scene's active bodies, in index order
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nb = bd.nb, nv = bd.nv;
   const int nd = nb + (HULLS ? bd.np : 0);                       // dynamic bodies: the rows of the pair list
   const int nt = nd + bd.no;                                     // bodies in the pair list
-  const long long npairs = pairs_before(nd, nt);                 // rows i < nd; circles only: nb (nb - 1) / 2
-  const int imax = nd - 1 < nt - 2 ? nd - 1 : nt - 2;            // last row with a pair
+  long long npairs = pairs_before(nd, nt);                       // rows i < nd; circles only: nb (nb - 1) / 2
+  int imax = nd - 1 < nt - 2 ? nd - 1 : nt - 2;                  // last row with a pair
+  int ntw = nt;                                                  // length of the list the pairs are decoded over
   for (int sc = blockIdx.x; sc < B; sc += gridDim.x) {
     const T* P = bd.pos + (size_t)sc * nb * 2;
     const T* R = bd.rad + (size_t)sc * nb;
     int32_t* o1 = body1 + (size_t)sc * cap;
     int32_t* o2 = body2 + (size_t)sc * cap;
+    const uint32_t* mask = no_contact;
+    if constexpr (ACTIVE) {
+      // compaction of the scene's active bodies: one 32-body word per thread (nt <= 8192 = 32 NT), a block-wide
+      // exclusive scan of (active bodies | active dynamic bodies << 16) per word
+      if (mask) mask += (size_t)sc * nc_stride;
+      const int words = (nt + 31) >> 5;
+      uint32_t w = 0;
+      if (tid < words) {
+        w = active ? __ldg(active + (size_t)sc * words + tid) : 0xffffffffu;
+        const int left = nt - 32 * tid;                          // bodies in this word
+        if (left < 32) w &= (1u << left) - 1u;
+      }
+      const int dleft = nd - 32 * tid;                           // dynamic bodies in this word
+      const uint32_t wd = dleft >= 32 ? w : dleft <= 0 ? 0u : w & ((1u << dleft) - 1u);
+      const int mine = __popc(w) | __popc(wd) << 16;
+      int incl = mine;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+      __syncthreads();                                           // the previous scene is done with act and warp_tot
+      if (lane == 31) warp_tot[warp] = incl;
+      __syncthreads();
+      int before = 0, total = 0;
+#pragma unroll
+      for (int w8 = 0; w8 < NT / 32; ++w8) { const int v = warp_tot[w8]; if (w8 < warp) before += v; total += v; }
+      int at = (before + incl - mine) & 0xffff;
+      for (uint32_t r = w; r; r &= r - 1u) act[at++] = (uint16_t)(32 * tid + __ffs(r) - 1);
+      __syncthreads();                                           // act complete; warp_tot is rewritten by the walk
+      const int nd_s = total >> 16;
+      ntw = total & 0xffff;
+      npairs = pairs_before(nd_s, ntw);
+      imax = nd_s - 1 < ntw - 2 ? nd_s - 1 : ntw - 2;
+    }
     int base = 0;                                                // contacts found in the previous chunks
     for (long long q0 = 0; q0 < npairs; q0 += (long long)NT * ITEMS) {
       const long long q = q0 + (long long)tid * ITEMS;
       int i = 0, j = 0;
       if (q < npairs) {                                          // (i, j) of pair q: closed form + exact fix-up
-        const double t = 2.0 * nt - 1.0;
+        const double t = 2.0 * ntw - 1.0;
         long long ii = (long long)floor((t - sqrt(t * t - 8.0 * (double)q)) * 0.5);
         if (ii < 0) ii = 0;
         if (ii > imax) ii = imax;
-        while (ii + 1 <= imax && pairs_before(ii + 1, nt) <= q) ++ii;
-        while (ii > 0 && pairs_before(ii, nt) > q) --ii;
+        while (ii + 1 <= imax && pairs_before(ii + 1, ntw) <= q) ++ii;
+        while (ii > 0 && pairs_before(ii, ntw) > q) --ii;
         i = (int)ii;
-        j = (int)(q - pairs_before(ii, nt)) + i + 1;
+        j = (int)(q - pairs_before(ii, ntw)) + i + 1;
       }
       unsigned hit = 0;                                          // HULLS: 2 bits per pair, its contact count
       int pi[ITEMS], pj[ITEMS];
       int f[HULLS ? 2 * ITEMS : 1];
 #pragma unroll
       for (int u = 0; u < ITEMS; ++u) {
-        pi[u] = i; pj[u] = j;
+        int bi = i, bj = j;                                      // body indices of list positions (i, j)
+        if constexpr (ACTIVE) {
+          if (q + u < npairs) { bi = act[i]; bj = act[j]; }
+        }
+        pi[u] = bi; pj[u] = bj;
         if (q + u < npairs) {
           bool skip = false;
           if constexpr (MASK) {
-            const long long bit = (long long)i * nt + j;
-            skip = (__ldg(no_contact + (bit >> 5)) >> (bit & 31)) & 1u;
+            const long long bit = (long long)bi * nt + bj;
+            if (!ACTIVE || mask) skip = (__ldg(mask + (bit >> 5)) >> (bit & 31)) & 1u;
           }
           if (skip) {
             if constexpr (HULLS) f[2 * u] = -1;
-          } else if (j < nb) {
-            const T dx = P[2 * i] - P[2 * j], dy = P[2 * i + 1] - P[2 * j + 1];
+          } else if (bj < nb) {
+            const T dx = P[2 * bi] - P[2 * bj], dy = P[2 * bi + 1] - P[2 * bj + 1];
             const T dist = sqrt(dx * dx + dy * dy);
-            const T pen = R[i] + R[j] - dist;                    // contacts.py:70-73
+            const T pen = R[bi] + R[bj] - dist;                  // contacts.py:70-73
             if (!(pen < -eps)) hit |= 1u << (HULLS ? 2 * u : u); // `if penetration < -eps: return`
             if constexpr (HULLS) f[2 * u] = -1;
-          } else if (!HULLS || i < nb) {
-            const T* V = HULLS ? bd.verts(sc, j) : bd.overts + ((size_t)sc * bd.no + (j - nb)) * nv * 2;
-            const PolyHit<T> h = circle_polygon<T>(V, nv, P[2 * i], P[2 * i + 1]);
+          } else if (!HULLS || bi < nb) {
+            const T* V = HULLS ? bd.verts(sc, bj) : bd.overts + ((size_t)sc * bd.no + (bj - nb)) * nv * 2;
+            const PolyHit<T> h = circle_polygon<T>(V, nv, P[2 * bi], P[2 * bi + 1]);
             // outside: `if best_dist > eps: return` (contacts.py:110-112); inside: sep - rad < 0 <= eps always
-            if (h.inside || !(sqrt(h.d2) - R[i] > eps)) hit |= 1u << (HULLS ? 2 * u : u);
+            if (h.inside || !(sqrt(h.d2) - R[bi] > eps)) hit |= 1u << (HULLS ? 2 * u : u);
             if constexpr (HULLS) f[2 * u] = -1;
           } else if constexpr (HULLS) {
-            const int n = hull_hull<T>(bd.verts(sc, i), bd.centre(sc, i), bd.verts(sc, j), bd.centre(sc, j), nv, eps,
-                                       &f[2 * u]);
+            const int n = hull_hull<T>(bd.verts(sc, bi), bd.centre(sc, bi), bd.verts(sc, bj), bd.centre(sc, bj), nv,
+                                       eps, &f[2 * u]);
             hit |= (unsigned)n << (2 * u);
           }
-          if (++j == nt) { ++i; j = i + 1; }
+          if (++j == ntw) { ++i; j = i + 1; }
         }
       }
       int mine;
@@ -485,6 +536,16 @@ static void launch_find_contacts(const Bodies<T>& bd, int B, int cap, T eps, int
                                  const uint32_t* no_contact = nullptr) {
   const int grid = B < 8 * num_sms ? B : 8 * num_sms;
   find_contacts_kernel<T, HULLS, MASK><<<grid, NT, 0, st>>>(bd, B, cap, eps, body1, body2, feat, counts, no_contact);
+}
+
+// the walk over each scene's active bodies (nt <= MAX_ACTIVE_NT); active / no_contact may be nullptr
+template <typename T>
+static void launch_find_contacts_active(const Bodies<T>& bd, int B, int cap, T eps, int32_t* body1, int32_t* body2,
+                                        int32_t* feat, int32_t* counts, int num_sms, cudaStream_t st,
+                                        const uint32_t* no_contact, long long nc_stride, const uint32_t* active) {
+  const int grid = B < 8 * num_sms ? B : 8 * num_sms;
+  find_contacts_kernel<T, true, true, true><<<grid, NT, 0, st>>>(bd, B, cap, eps, body1, body2, feat, counts,
+                                                                 no_contact, active, nc_stride);
 }
 
 }  // namespace cts

@@ -1061,21 +1061,25 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
 }
 
 // ------------------------------------------------------------------ contact detection
-// One body of lcpb200_contacts per dtype. The instantiation is chosen here and only here: the mask walk when the
-// caller passes no_contact, the polygon walk (HULLS) when it passes feat, the circle walk otherwise; the geometry
-// kernel follows the walk's HULLS.
+// One body of lcpb200_contacts and lcpb200_contacts_active per dtype. The instantiation is chosen here and only here:
+// the active walk for lcpb200_contacts_active; else the mask walk when the caller passes no_contact, the polygon walk
+// (HULLS) when it passes feat, the circle walk otherwise; the geometry kernel follows the walk's HULLS.
 template <typename T>
 static void contacts_t(int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos, const void* rad,
                        const void* fric, const void* rest, const void* pverts, const void* pcen, const void* pfric,
                        const void* prest, const void* overts, const void* oref, const void* ofric, const void* orest,
                        int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2,
-                       void* pen, void* mu, void* rest_c, const uint32_t* no_contact, int sms, cudaStream_t st) {
+                       void* pen, void* mu, void* rest_c, const uint32_t* no_contact, bool per_scene,
+                       const uint32_t* active, long long nc_stride, int sms, cudaStream_t st) {
   cts::Bodies<T> bd;
   bd.nb = nb; bd.np = np; bd.no = no; bd.nv = nv;
   bd.pos = (const T*)pos; bd.rad = (const T*)rad; bd.fric = (const T*)fric; bd.rest = (const T*)rest;
   bd.pverts = (const T*)pverts; bd.pcen = (const T*)pcen; bd.pfric = (const T*)pfric; bd.prest = (const T*)prest;
   bd.overts = (const T*)overts; bd.oref = (const T*)oref; bd.ofric = (const T*)ofric; bd.orest = (const T*)orest;
-  if (no_contact)
+  if (per_scene)
+    cts::launch_find_contacts_active<T>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st, no_contact, nc_stride,
+                                        active);
+  else if (no_contact)
     cts::launch_find_contacts<T, true, true>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st, no_contact);
   else if (feat)
     cts::launch_find_contacts<T, true, false>(bd, B, cap, (T)eps, body1, body2, feat, counts, sms, st);
@@ -1090,12 +1094,13 @@ static void contacts_t(int B, int nb, int np, int no, int nv, int cap, double ep
                                            (T*)pen, (T*)mu, (T*)rest_c, sms, st);
 }
 
-extern "C" int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
-                                const void* rad, const void* fric, const void* rest, const void* pverts,
-                                const void* pcen, const void* pfric, const void* prest, const void* overts,
-                                const void* oref, const void* ofric, const void* orest, int32_t* body1,
-                                int32_t* body2, int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2,
-                                void* pen, void* mu, void* rest_c, const uint32_t* no_contact, void* stream) {
+// Argument checks and launch shared by both entry points; per_scene selects the active walk.
+static int contacts_entry(bool per_scene, int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                          const void* pos, const void* rad, const void* fric, const void* rest, const void* pverts,
+                          const void* pcen, const void* pfric, const void* prest, const void* overts, const void* oref,
+                          const void* ofric, const void* orest, int32_t* body1, int32_t* body2, int32_t* counts,
+                          int32_t* feat, void* normal, void* p1, void* p2, void* pen, void* mu, void* rest_c,
+                          const uint32_t* no_contact, const uint32_t* active, long long nc_stride, void* stream) {
   if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
   if (B < 0 || nb < 0 || np < 0 || no < 0 || cap <= 0 || nb + np <= 0)
     return fail("contacts: need B >= 0, nb, np, no >= 0, nb + np > 0, cap > 0");
@@ -1104,7 +1109,14 @@ extern "C" int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv
   if ((nb > 0 && (!pos || !rad)) || (np > 0 && (!pverts || !pcen)) || (no > 0 && (!overts || !oref)) || !body1 ||
       !body2 || !counts)
     return fail("contacts: NULL argument");
-  if ((np > 0 || no_contact) && !feat) return fail("contacts: polygons and no_contact need feat");
+  if (per_scene) {
+    if ((long long)nb + np + no > cts::MAX_ACTIVE_NT)
+      return fail("contacts_active: at most 8192 bodies (nb + np + no)");
+    if (nc_stride < 0) return fail("contacts_active: need no_contact_stride >= 0");
+    if (!feat) return fail("contacts_active: need feat");
+  } else if ((np > 0 || no_contact) && !feat) {
+    return fail("contacts: polygons and no_contact need feat");
+  }
   const int ngeo = (normal != nullptr) + (p1 != nullptr) + (p2 != nullptr) + (pen != nullptr) + (mu != nullptr) +
                    (rest_c != nullptr);
   if (ngeo != 0 && ngeo != 6) return fail("contacts: the geometry outputs are all NULL or all non-NULL");
@@ -1116,9 +1128,34 @@ extern "C" int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   (dtype == LCPB200_F32 ? contacts_t<float> : contacts_t<double>)(
       B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest, overts, oref, ofric, orest, body1,
-      body2, counts, feat, normal, p1, p2, pen, mu, rest_c, no_contact, sms, (cudaStream_t)stream);
+      body2, counts, feat, normal, p1, p2, pen, mu, rest_c, no_contact, per_scene, active, nc_stride, sms,
+      (cudaStream_t)stream);
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int lcpb200_contacts(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps, const void* pos,
+                                const void* rad, const void* fric, const void* rest, const void* pverts,
+                                const void* pcen, const void* pfric, const void* prest, const void* overts,
+                                const void* oref, const void* ofric, const void* orest, int32_t* body1,
+                                int32_t* body2, int32_t* counts, int32_t* feat, void* normal, void* p1, void* p2,
+                                void* pen, void* mu, void* rest_c, const uint32_t* no_contact, void* stream) {
+  return contacts_entry(false, dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest,
+                        overts, oref, ofric, orest, body1, body2, counts, feat, normal, p1, p2, pen, mu, rest_c,
+                        no_contact, nullptr, 0, stream);
+}
+
+extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no, int nv, int cap, double eps,
+                                       const void* pos, const void* rad, const void* fric, const void* rest,
+                                       const void* pverts, const void* pcen, const void* pfric, const void* prest,
+                                       const void* overts, const void* oref, const void* ofric, const void* orest,
+                                       int32_t* body1, int32_t* body2, int32_t* counts, int32_t* feat, void* normal,
+                                       void* p1, void* p2, void* pen, void* mu, void* rest_c,
+                                       const uint32_t* no_contact, long long no_contact_stride,
+                                       const uint32_t* active, void* stream) {
+  return contacts_entry(true, dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest,
+                        overts, oref, ofric, orest, body1, body2, counts, feat, normal, p1, p2, pen, mu, rest_c,
+                        no_contact, active, no_contact_stride, stream);
 }
 
 // ------------------------------------------------------------------ assembly

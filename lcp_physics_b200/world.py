@@ -36,6 +36,7 @@ Everything is differentiable through torch autograd (the LCP through lcpb200_eng
 """
 import math
 
+import numpy as np
 import torch
 import torch.autograd.forward_ad as fwAD
 
@@ -233,6 +234,91 @@ def _has_tangent(t):
     return t is not None and fwAD.unpack_dual(t).tangent is not None
 
 
+MAX_ACTIVE_BODIES = 8192        # bodies of a world walked per scene (the kernel's shared-memory list of active bodies)
+
+
+def check_active(active, B, nt):
+    """Validates a per-scene activity mask, bool [B, nt] or broadcastable to it; returns it as a contiguous [B, nt]."""
+    a = torch.as_tensor(active)
+    if a.dtype != torch.bool:
+        raise ValueError("active: need a bool mask [B, nb + npoly + no] = [%d, %d], got dtype %s" % (B, nt, a.dtype))
+    try:
+        a = a.expand(B, nt)
+    except RuntimeError:
+        raise ValueError("active: need a bool mask [B, nb + npoly + no] = [%d, %d] (or broadcastable), got %s"
+                         % (B, nt, tuple(a.shape))) from None
+    return a.contiguous()
+
+
+def check_constraint_activity(cons, active):
+    """A constraint takes part in scene s iff all its bodies are active there; raises ValueError, naming the scene and
+    the constraint, when a constraint has both active and inactive bodies in some scene."""
+    for ci, c in enumerate(cons):
+        a = active[:, list(c.bodies())]
+        mixed = (a.any(1) & ~a.all(1)).nonzero()
+        if mixed.numel():
+            raise ValueError("constraints: constraint %d (%s of bodies %s) has active and inactive bodies in scene %d; "
+                             "a constraint takes part in a scene only with all its bodies active"
+                             % (ci, type(c).__name__, c.bodies(), int(mixed[0, 0])))
+
+
+def _no_contact_words(pairs, nt, where):
+    """Bitmask [ceil(nt * nt / 32)] int32 of one pair list: bit i * nt + j (i < j) per excluded pair. Built from the
+    pair list alone (nt * nt / 8 bytes: the layout the contact walk reads)."""
+    prs = np.asarray([tuple(int(x) for x in pr) for pr in pairs], dtype=np.int64).reshape(-1, 2)
+    bad = ~((prs >= 0) & (prs < nt)).all(1)
+    if bad.any():
+        raise ValueError("no_contact: body index out of range in %r%s (%d bodies)"
+                         % (tuple(int(x) for x in prs[bad][0]), where, nt))
+    same = prs[:, 0] == prs[:, 1]
+    if same.any():
+        a = int(prs[same][0, 0])
+        raise ValueError("no_contact: the pair (%d, %d)%s names one body twice" % (a, a, where))
+    bits = prs.min(1) * nt + prs.max(1)
+    words = np.zeros((nt * nt + 31) // 32, dtype=np.uint32)
+    np.bitwise_or.at(words, bits >> 5, (np.uint32(1) << (bits & 31).astype(np.uint32)))
+    return torch.from_numpy(words.view(np.int32).copy())
+
+
+def mask_bits(words, nt, i, j):
+    """Bit i * nt + j of no_contact words ([W] or [B, W]) for the pairs (i, j) (long tensors, same device): True where
+    the pair is excluded; [len(i)] or [B, len(i)]."""
+    bit = i * nt + j
+    return ((words[..., bit >> 5] >> (bit & 31).to(torch.int32)) & 1).bool()
+
+
+def per_scene_pairs(pairs):
+    """True when a `no_contact` argument is a list of pair lists, one per scene: its items are sequences of pairs,
+    where a shared list's items are pairs of indices."""
+    seq = lambda x: isinstance(x, (list, tuple))
+    items = list(pairs)
+    return bool(items) and all(seq(ps) and all(seq(pr) for pr in ps) for ps in items)
+
+
+def no_contact_masks(pairs, B, nt):
+    """The no_contact bitmask of lcpb200_contacts / lcpb200_contacts_active: for one pair list shared by the batch,
+    words [ceil(nt * nt / 32)] int32; for a length-B list of pair lists (its items are sequences of pairs, where a
+    shared list's items are pairs of indices), one row per scene, [B, ceil(nt * nt / 32)]: nt * nt / 8 bytes per
+    scene (8 MB at the 8192-body bound), so per-scene lists suit worlds of up to a few hundred bodies."""
+    items = list(pairs)
+    if not per_scene_pairs(items):
+        return _no_contact_words(items, nt, "")
+    if len(items) != B:
+        raise ValueError("no_contact: a per-scene list needs one pair list per scene (B = %d), got %d"
+                         % (B, len(items)))
+    return torch.stack([_no_contact_words(ps, nt, " of scene %d" % s) for s, ps in enumerate(items)])
+
+
+def pack_bits(mask):
+    """bool [B, nt] -> int32 [B, ceil(nt / 32)]: bit k % 32 of word k / 32 set iff mask[:, k]."""
+    B, nt = mask.shape
+    W = (nt + 31) // 32
+    m = torch.zeros(B, 32 * W, dtype=torch.int64, device=mask.device)
+    m[:, :nt] = mask.to(torch.int64)
+    w = (m.reshape(B, W, 32) << torch.arange(32, device=mask.device)).sum(2)
+    return torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32).contiguous()
+
+
 def _pad_vertices(v, V):
     """[B, n, V0, 2] -> [B, n, V, 2] (V >= V0) by repeating the last vertex: a zero-length edge, skipped by every rule."""
     if v.shape[2] == V:
@@ -246,7 +332,7 @@ class BatchedWorld:
                  strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False,
                  obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5, polygons=None, poly_rot=0.0, poly_vel=None,
                  poly_mass=1.0, poly_fric=0.9, poly_rest=0.5, constraints=None, no_contact=None,
-                 external_force=None):
+                 external_force=None, active=None):
         """pos [B,nb,2] (nb may be 0), rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass /
         restitution / fric_coeff [B,nb] (or broadcastable).
         `polygons`: dynamic convex polygons, the reference's `Rect` / `Hull` bodies (bodies.py:154-301): world-frame
@@ -269,9 +355,17 @@ class BatchedWorld:
         `constraints`: `Joint` / `FixedJoint` / `XConstraint` / `YConstraint` / `RotConstraint` specs naming dynamic
         bodies by index (topology shared by the batch); their equality rows follow the `static` pins' rows, in list
         order. `no_contact`: pairs (a, b) of indices in [circles, polygons, obstacles] that never make contact
-        (Body.add_no_contact), shared by the batch; joints do not imply it. `external_force`: f(t) -> [B, nd, 3]
+        (Body.add_no_contact), shared by the batch, or a length-B list of such pair lists, one per scene; joints do not
+        imply it. `external_force`: f(t) -> [B, nd, 3]
         (rot, x, y) given the per-scene time t [B], evaluated once per step at its start and added to gravity
-        (ExternalForce); gradients reach whatever f closes over."""
+        (ExternalForce); gradients reach whatever f closes over.
+        `active`: bool [B, nb + npoly + no] (or broadcastable), which bodies of [circles, polygons, obstacles] take
+        part in each scene, so that the scenes of one batch can hold different bodies (None: all of them). An inactive
+        body is frozen: it gets no gravity and no external force, its p and v are carried through every step
+        unchanged, and it makes no contact (the contact walk of each scene visits its active bodies only). A
+        constraint belongs to the scenes in which all its bodies are active; one with active and inactive bodies in
+        the same scene raises ValueError (list, e.g., a 4-link and a 7-link chain and activate one of them per scene).
+        At most 8192 bodies in all (nb + npoly + no) with `active` or per-scene `no_contact`."""
         _lib.require_cuda()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         pos = torch.as_tensor(pos)
@@ -344,13 +438,22 @@ class BatchedWorld:
             if self.no:
                 self.ov = _pad_vertices(self.ov, self.nv)
         nt = nd + self.no
+        # the walk over each scene's own bodies (lcpb200_contacts_active) when scenes differ in bodies or masks
+        self.per_scene = active is not None or (no_contact is not None and per_scene_pairs(no_contact))
+        if self.per_scene and nt > MAX_ACTIVE_BODIES:
+            raise ValueError("BatchedWorld: with `active` or per-scene `no_contact` a world holds at most %d bodies "
+                             "(nb + npoly + no), got %d" % (MAX_ACTIVE_BODIES, nt))
         ii, jj = torch.triu_indices(nt, nt, 1)
         if self.no:
             keep = ii < nd                                                          # obstacles never pair up
             ii, jj = ii[keep], jj[keep]
         self.pi, self.pj = ii.to(self.device), jj.to(self.device)                   # pair (i, j), i < j, lexicographic
+        self.active, self.active_words = None, None          # active_words None: every body active in the walk
+        if active is not None:
+            self._init_active(active, nt)
+            self.fext = torch.where(self.dof_active, self.fext, torch.zeros_like(self.fext))   # frozen: no gravity
         self._init_constraints(to)
-        self.nc_mask = None
+        self.nc_mask, self.nc_stride = None, 0
         if no_contact is not None:
             self._init_no_contact(no_contact, nt)
         if self.np:
@@ -415,6 +518,16 @@ class BatchedWorld:
             self.ne += c.num_constraints
         if self.cons:
             self.A = self._equality_rows()
+        if self.active is not None:
+            check_constraint_activity(self.cons, self.active)
+
+    def _init_active(self, active, nt):
+        """Per-scene body activity: self.active [B, nt] bool, body_active [B, nd, 1] / dof_active [B, n] for the
+        freezing, and the bitmask of lcpb200_contacts_active, active_words [B, ceil(nt / 32)] (bit k of word k / 32)."""
+        self.active = check_active(active, self.B, nt).to(self.device)
+        self.body_active = self.active[:, :self.nd].unsqueeze(2)
+        self.dof_active = self.body_active.expand(-1, -1, 3).reshape(self.B, self.n)
+        self.active_words = pack_bits(self.active)
 
     def _equality_rows(self):
         """World.Je() (world.py:156-170) for every scene, [B, ne, n]: the `static` pins' identity rows, then each
@@ -455,25 +568,21 @@ class BatchedWorld:
                 continue
             rot1 = r0 + vel[:, 3 * c.i] * dts
             pos1 = _polar_to_cart(st[0], rot1)
-            st[1:] = [rot1, pos1, self.p[:, c.i, 1:] + pos1]
+            pos = self.p[:, c.i, 1:] + pos1
+            if self.active is not None:
+                # a joint of frozen bodies keeps its state, as its bodies keep theirs
+                on = self.active[:, c.i]
+                rot1, pos1 = torch.where(on, rot1, st[1]), torch.where(on.unsqueeze(1), pos1, st[2])
+                pos = torch.where(on.unsqueeze(1), pos, st[3])
+            st[1:] = [rot1, pos1, pos]
 
     def _init_no_contact(self, pairs, nt):
-        """Pair-exclusion bitmask (no_contact of lcpb200_contacts): bit i * nt + j (i < j) per excluded pair."""
-        words = [0] * ((nt * nt + 31) // 32)
-        ex = torch.zeros(nt, nt, dtype=torch.bool)
-        for pr in pairs:
-            a, b = (int(x) for x in pr)
-            if not (0 <= a < nt and 0 <= b < nt):
-                raise ValueError("no_contact: body index out of range in %r (%d bodies)" % (tuple(pr), nt))
-            if a == b:
-                raise ValueError("no_contact: the pair (%d, %d) names one body twice" % (a, b))
-            a, b = min(a, b), max(a, b)
-            bit = a * nt + b
-            words[bit >> 5] |= 1 << (bit & 31)
-            ex[a, b] = True
-        words = [w - (1 << 32) if w >= 1 << 31 else w for w in words]            # the same 32 bits as int32
-        self.nc_mask = torch.tensor(words, dtype=torch.int32, device=self.device)
-        self.nc_pair_excluded = ex.to(self.device)[self.pi, self.pj]              # per pair of self.pi / self.pj
+        """Pair-exclusion bitmask (no_contact of lcpb200_contacts): bit i * nt + j (i < j) per excluded pair. A
+        length-B list of pair lists gives one mask per scene ([B, words], nc_stride = words)."""
+        words = no_contact_masks(pairs, self.B, nt)
+        self.nc_mask = words.to(self.device)
+        self.nc_stride = int(words.shape[1]) if words.dim() == 2 else 0
+        self.nc_pair_excluded = mask_bits(self.nc_mask, nt, self.pi, self.pj)      # per pair of self.pi / self.pj
 
     # ------------------------------------------------------------------ contacts.py:60-292, batched
     def find_contacts(self):
@@ -491,9 +600,10 @@ class BatchedWorld:
         tracked = (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst
         needs_graph = (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tracked)) or any(
             _has_tangent(t) for t in tracked)
-        # feat selects the polygon walk, which worlds with polygons or no_contact pairs need; the others keep the
-        # circle walk
-        with_feat = self.np > 0 or self.nc_mask is not None
+        # feat selects the polygon walk, which worlds with polygons, no_contact pairs or per-scene bodies need; the
+        # others keep the circle walk
+        with_feat = self.np > 0 or self.nc_mask is not None or self.per_scene
+        masks = (self.nc_mask, self.active_words) if self.per_scene else (self.nc_mask,)
         d = lambda t: t.detach().contiguous() if t is not None else None
 
         def walk(*ins):
@@ -502,11 +612,17 @@ class BatchedWorld:
             feat = i32(B, cap) if with_feat else None
             new = lambda *s_: torch.empty(B, cap, *s_, dtype=self.dtype, device=dev)
             geo = [None] * 6 if needs_graph else [new(2), new(2), new(2), new(), new(), new()]
+            bodies = [_lib.ptr(t) for t in ins[:-len(masks)]]
+            outs = [_lib.ptr(t) for t in (b1, b2, counts, feat, *geo)]
             with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_contacts(
-                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps,
-                    *[_lib.ptr(t) for t in ins[:-1]], _lib.ptr(b1), _lib.ptr(b2), _lib.ptr(counts), _lib.ptr(feat),
-                    *[_lib.ptr(t) for t in geo], _lib.ptr(ins[-1]), _lib.stream_ptr(dev)))
+                if self.per_scene:
+                    _lib.check(lib.lcpb200_contacts_active(
+                        _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps, *bodies, *outs,
+                        _lib.ptr(ins[-2]), self.nc_stride, _lib.ptr(ins[-1]), _lib.stream_ptr(dev)))
+                else:
+                    _lib.check(lib.lcpb200_contacts(
+                        _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, cap, self.eps, *bodies, *outs,
+                        _lib.ptr(ins[-1]), _lib.stream_ptr(dev)))
             # tensors only: _DetectFn marks every output non-differentiable
             return tuple(t for t in (b1, b2, counts, feat, *geo) if t is not None)
         # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the
@@ -514,7 +630,7 @@ class BatchedWorld:
         pcen = self.p[:, nb:, 1:] if self.np else None
         ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
                + obst]
-        out = _detect(walk, *ins, self.nc_mask)
+        out = _detect(walk, *ins, *masks)
         b1, b2, counts = out[:3]
         feat = out[3] if with_feat else None
         if int(counts.max()) > cap:
@@ -684,7 +800,8 @@ class BatchedWorld:
     def find_contacts_torch(self):
         """The same contact list with torch ops only (O(nb^2) tensors, a stable sort for the compaction): the
         independent implementation tests/test_gpu_world.py and tests/test_gpu_obstacles.py check lcpb200_contacts'
-        circle walk against. Returns (counts, b1, b2). Not available for worlds with
+        circle walk against; pairs excluded per scene and pairs with an inactive body make no contact. Returns
+        (counts, b1, b2). Not available for worlds with
         dynamic polygons: their hull-hull rule is checked against the CPU oracle (oracle/polygon_oracle.py)."""
         if self.np:
             raise NotImplementedError("find_contacts_torch: worlds with dynamic polygons (see oracle/polygon_oracle.py)")
@@ -702,6 +819,8 @@ class BatchedWorld:
             active = torch.where(cc, pen >= -self.eps, hit_o)
             if self.nc_mask is not None:
                 active = active & ~self.nc_pair_excluded                                  # contacts.py:60
+            if self.active is not None:
+                active = active & self.active[:, self.pi] & self.active[:, self.pj]
             counts = active.sum(1)
             order = torch.sort((~active).to(torch.int8), dim=1, stable=True)[1][:, :self.cap]
             return counts.to(torch.int32), self.pi[order].to(torch.int32), self.pj[order].to(torch.int32)
@@ -710,6 +829,8 @@ class BatchedWorld:
         active = pen >= -self.eps                                                  # `if penetration < -eps: return`
         if self.nc_mask is not None:
             active = active & ~self.nc_pair_excluded                                      # contacts.py:60
+        if self.active is not None:
+            active = active & self.active[:, self.pi] & self.active[:, self.pj]
         counts = active.sum(1)
         order = torch.sort((~active).to(torch.int8), dim=1, stable=True)[1][:, :self.cap]   # active pairs first, in pair order
         return counts.to(torch.int32), self.pi[order].to(torch.int32), self.pj[order].to(torch.int32)
@@ -719,7 +840,13 @@ class BatchedWorld:
 
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
-        z, status = engine_solve(self.mass, self.inertia, self.v, self.fext if fext is None else fext, self.c_normal,
+        mass, inertia, v = self.mass, self.inertia, self.v
+        if self.active is not None:
+            # frozen bodies are isolated blocks of K whose results step_dt discards: no gradient through them
+            keep = lambda t, m: torch.where(m, t, t.detach())
+            mass, inertia = keep(mass, self.body_active[..., 0]), keep(inertia, self.body_active[..., 0])
+            v = keep(v, self.dof_active)
+        z, status = engine_solve(mass, inertia, v, self.fext if fext is None else fext, self.c_normal,
                                  self.c_p1, self.c_p2, self.c_mu, self.c_rest, self.c_b1, self.c_b2, dt, A=self.A, b=b,
                                  mode=mode,
                                  max_iter=self.max_iter if mode == 0 else 10, exact_adjoint=self.exact_adjoint,
@@ -743,7 +870,10 @@ class BatchedWorld:
             if tuple(f.shape) != (self.B, self.nd, 3):
                 raise ValueError("external_force: f(t) must return [B, nd, 3] = %s, got %s"
                                  % ((self.B, self.nd, 3), tuple(f.shape)))
-            fext = self.fext + f.reshape(self.B, self.n)
+            f = f.reshape(self.B, self.n)
+            if self.active is not None:
+                f = torch.where(self.dof_active, f, torch.zeros_like(f))
+            fext = self.fext + f
         return -self._lcp(0, dt, b, fext)
 
     def post_stabilization(self):
@@ -760,11 +890,16 @@ class BatchedWorld:
     def step_dt(self, dt):
         start_p = self.p.clone()
         start_rot = [st[1] if st is not None else None for st in self._jstate]      # world.py:85
+        start_v = self.v
         self.v = self.solve_dynamics(dt)
+        if self.active is not None:
+            self.v = torch.where(self.dof_active, self.v, start_v)                 # frozen bodies keep p and v
         dts = self.v.new_full((self.B,), float(dt))
         done = torch.zeros(self.B, dtype=torch.bool, device=self.device)
         while True:
             moved = start_p + self.v.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)      # body.move(dt)
+            if self.active is not None:
+                moved = torch.where(self.body_active, moved, start_p)
             self.p = torch.where(done.reshape(self.B, 1, 1), self.p, moved)
             self.find_contacts()
             ok = self.max_penetration() <= self.tol
@@ -780,6 +915,8 @@ class BatchedWorld:
         if self.post_stab:
             tmp_v = self.v
             dp = self.post_stabilization() / 2                                     # world.py:111-112
+            if self.active is not None:
+                dp = torch.where(self.dof_active, dp, torch.zeros_like(dp))
             self.p = self.p + dp.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)
             if self.cons:
                 self._move_joints([st[1] if st is not None else None for st in self._jstate], dp, dts)   # :117-118
