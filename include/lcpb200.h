@@ -274,6 +274,39 @@ int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no, int nv, in
                             void* restitution_c, const uint32_t* no_contact, long long no_contact_stride,
                             const uint32_t* active, void* stream);
 
+/* Ray casts against the bodies of B scenes (the body groups of lcpb200_contacts): R rays per scene, each an origin and a
+ * UNIT direction (not normalised here), cast against the body list [circles 0..nb-1, polygons nb..nb+np-1, obstacles
+ * nb+np..nb+np+no-1] at their current pose. A ray hits a body only where it ENTERS it at some 0 <= t <= max_dist:
+ *   circle (c, r)                 w = o - c, b = u . w, k = |w|^2 - r^2: a miss if k < 0 (the origin is inside),
+ *                                 b >= 0 or disc = b^2 - k < 0, else t = k / (-b + sqrt(disc)); feat -1, normal
+ *                                 (o + t u - c) / r
+ *   polygon / obstacle            convex, either orientation; Cyrus-Beck clipping against every edge of non-zero length
+ *                                 (outward unit normal n_e, start vertex v_e, num = n_e . (v_e - o), den = n_e . u):
+ *                                 den == 0 a miss if num < 0, else the edge is ignored; den < 0 an entering edge at
+ *                                 t = num / den, the largest wins (the first edge on a tie); den > 0 a leaving edge,
+ *                                 the smallest t kept. A hit iff an entering edge exists and 0 <= t_enter <= t_leave,
+ *                                 t_enter <= max_dist; feat = the entering edge, normal = its n_e. An origin inside the
+ *                                 polygon gives t_enter < 0: no hit.
+ * The nearest hit wins; an exact tie goes to the lower body index. A ray that hits nothing gets body -1, feat -1,
+ * t = max_dist and a zero normal; so does a direction of zero length or with a non-finite component, or a non-finite
+ * origin. Deterministic (no atomics); results do not depend on how the rays are split into CTAs.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb]                             circles (NULL when nb == 0)
+ *   pverts[B,np,nv,2] overts[B,no,nv,2]               polygons and obstacles: world-frame vertices (NULL when the
+ *                                                     group is empty); a vertex repeated to pad to nv is skipped
+ *   origin[B,R,2] dir[B,R,2]                          the rays; dir of unit length
+ *   active_words[B, ceil(nt / 32)] int32              NULL (every body visible), or the layout of lcpb200_contacts_active:
+ *                                                     bit k % 32 of word k / 32 of row s set iff body k is active in
+ *                                                     scene s; inactive bodies are invisible (nt <= 8192)
+ *   t[B,R] body[B,R] feat[B,R] int32                  OUT: distance, body index (-1: no hit), entering edge (-1: a
+ *                                                     circle or no hit)
+ *   normal[B,R,2]                                     OUT or NULL: the surface normal at the hit
+ * Returns non-zero without launching on B <= 0, R <= 0, nb + np + no == 0, nv > 256 (or nv < 3 with polygons),
+ * max_dist < 0 or non-finite (in the dtype), a NULL required pointer, active_words with nt > 8192, or B * R > 2^31 - 1. */
+int lcpb200_raycast(int dtype, int B, int nb, int np, int no, int nv, int R, double max_dist, const void* pos,
+                    const void* rad, const void* pverts, const void* overts, const void* origin, const void* dir,
+                    const int32_t* active_words, void* t, int32_t* body, int32_t* feat, void* normal, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

@@ -44,6 +44,7 @@ _SIGS = {
     "lcpb200_contacts": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 24),
     "lcpb200_contacts_active": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 23 +
                                 [ctypes.c_longlong, _vp, _vp]),
+    "lcpb200_raycast": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 12),
     "lcpb200_assemble": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 17),
     "lcpb200_assemble_backward": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 25),
 }

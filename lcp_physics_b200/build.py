@@ -26,7 +26,9 @@ NVCC_FLAGS = ARCH + [
 DUAL_DEPS = ["lcp_kernels.cu", "lcp_launch.h", "lcp_device.cuh", "lcp_lu.cuh", "lcp_solver.cuh"]
 COND_DEPS = ["lcp_cond_kernels.cu", "lcp_cond_launch.h", "lcp_device.cuh", "lcp_condensed.cuh"]
 BAND_DEPS = ["lcp_band_kernels.cu", "lcp_band_launch.h", "lcp_device.cuh", "lcp_condensed.cuh", "lcp_banded.cuh"]
-API_DEPS = ["lcpb200.cu", "lcp_assemble.cuh", "lcp_contacts.cuh", "../../include/lcpb200.h"] + DUAL_DEPS[1:] + COND_DEPS[1:] + BAND_DEPS[1:]
+RAY_DEPS = ["lcp_ray_kernels.cu", "lcp_ray_launch.h", "lcp_raycast.cuh", "lcp_contacts.cuh"]
+API_DEPS = (["lcpb200.cu", "lcp_assemble.cuh", "lcp_contacts.cuh", "lcp_ray_launch.h", "../../include/lcpb200.h"] +
+            DUAL_DEPS[1:] + COND_DEPS[1:] + BAND_DEPS[1:])
 
 # dual-form kernels: one TU per (dtype, residency mode); condensed kernels: one per (dtype, NS)
 DUAL_VARIANTS = [(t, m) for t in ("float", "double") for m in (0, 1, 2)]
@@ -41,6 +43,7 @@ def _jobs():
         jobs.append(("cond_%s_%d.o" % (t, ns), "lcp_cond_kernels.cu", ["-DLCP_T=%s" % t, "-DLCP_NS=%d" % ns], COND_DEPS))
     # LCPB200_BAND_DEFS: extra -D flags for the banded kernel (debug builds, e.g. -DLCP_BAND_LUPROF)
     jobs.append(("band.o", "lcp_band_kernels.cu", os.environ.get("LCPB200_BAND_DEFS", "").split(), BAND_DEPS))
+    jobs.append(("ray.o", "lcp_ray_kernels.cu", [], RAY_DEPS))
     jobs.append(("api.o", "lcpb200.cu", [], API_DEPS))
     return jobs
 

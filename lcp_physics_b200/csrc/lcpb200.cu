@@ -3,7 +3,9 @@
 #include <stdio.h>
 #include <string.h>
 #include <algorithm>
+#include <cfloat>
 #include <climits>
+#include <cmath>
 #include <new>
 #include <string>
 #include <type_traits>
@@ -15,6 +17,7 @@
 #include "lcp_cond_launch.h"
 #include "lcp_band_launch.h"
 #include "lcp_contacts.cuh"
+#include "lcp_ray_launch.h"
 
 using namespace lcpb200;
 using cnd::CPlan;
@@ -1156,6 +1159,50 @@ extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no,
   return contacts_entry(true, dtype, B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest,
                         overts, oref, ofric, orest, body1, body2, counts, feat, normal, p1, p2, pen, mu, rest_c,
                         no_contact, active, no_contact_stride, stream);
+}
+
+// ------------------------------------------------------------------ ray casts
+extern "C" int lcpb200_raycast(int dtype, int B, int nb, int np, int no, int nv, int R, double max_dist,
+                               const void* pos, const void* rad, const void* pverts, const void* overts,
+                               const void* origin, const void* dir, const int32_t* active_words, void* t,
+                               int32_t* body, int32_t* feat, void* normal, void* stream) {
+  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
+  if (B <= 0 || R <= 0 || nb < 0 || np < 0 || no < 0) return fail("raycast: need B, R > 0 and nb, np, no >= 0");
+  const long long nt = (long long)nb + np + no;
+  if (nt == 0) return fail("raycast: no body (nb + np + no == 0)");
+  if (nt > 0x7fffffffLL) return fail("raycast: too many bodies");
+  if (nv > cts::MAX_NV || (np + no > 0 && nv < 3)) return fail("raycast: polygons need 3 <= nv <= 256 vertices");
+  if (!std::isfinite(max_dist) || max_dist < 0 || (dtype == LCPB200_F32 && max_dist > FLT_MAX))
+    return fail("raycast: need a finite max_dist >= 0");
+  if ((nb > 0 && (!pos || !rad)) || (np > 0 && !pverts) || (no > 0 && !overts) || !origin || !dir || !t || !body ||
+      !feat)
+    return fail("raycast: NULL argument");
+  if (active_words && nt > cts::MAX_ACTIVE_NT) return fail("raycast: at most 8192 bodies (nb + np + no) with active");
+  if ((long long)B * R > 0x7fffffffLL) return fail("raycast: B * R rays exceed int32 indexing");
+  int dev = 0, sms = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == LCPB200_F32) {
+    ray::RayArgs<float> a{};
+    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
+    a.bd.pos = (const float*)pos; a.bd.rad = (const float*)rad;
+    a.bd.pverts = (const float*)pverts; a.bd.overts = (const float*)overts;
+    a.B = B; a.R = R; a.max_dist = (float)max_dist;
+    a.origin = (const float*)origin; a.dir = (const float*)dir; a.active = (const uint32_t*)active_words;
+    a.t = (float*)t; a.body = body; a.feat = feat; a.normal = (float*)normal;
+    CK(ray::launch_raycast<float>(a, sms, st));
+  } else {
+    ray::RayArgs<double> a{};
+    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
+    a.bd.pos = (const double*)pos; a.bd.rad = (const double*)rad;
+    a.bd.pverts = (const double*)pverts; a.bd.overts = (const double*)overts;
+    a.B = B; a.R = R; a.max_dist = max_dist;
+    a.origin = (const double*)origin; a.dir = (const double*)dir; a.active = (const uint32_t*)active_words;
+    a.t = (double*)t; a.body = body; a.feat = feat; a.normal = (double*)normal;
+    CK(ray::launch_raycast<double>(a, sms, st));
+  }
+  return 0;
 }
 
 // ------------------------------------------------------------------ assembly

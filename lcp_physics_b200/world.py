@@ -838,6 +838,127 @@ class BatchedWorld:
     def max_penetration(self):
         return self.c_pen.max(dim=1)[0]
 
+    # ------------------------------------------------------------------ ray casts
+    def _ray_arg(self, x, name):
+        """A ray argument [B, R, 2] or [R, 2] (shared by the batch) as a [B, R, 2] tensor of the world's dtype / device."""
+        if isinstance(x, torch.Tensor):
+            if not x.is_floating_point():
+                raise ValueError("%s: need a floating-point tensor, got dtype %s" % (name, x.dtype))
+            x = x.to(device=self.device, dtype=self.dtype)
+        else:
+            x = torch.as_tensor(x, dtype=self.dtype, device=self.device)
+        if x.dim() == 2:
+            x = x.unsqueeze(0).expand(self.B, -1, -1)
+        if x.dim() != 3 or x.shape[0] != self.B or x.shape[2] != 2 or x.shape[1] == 0:
+            raise ValueError("%s: need [B, R, 2] or [R, 2] with R >= 1 (B = %d), got %s"
+                             % (name, self.B, tuple(x.shape)))
+        return x
+
+    def raycast(self, origin, direction, max_dist):
+        """Casts rays against every scene's bodies at the current state (lcpb200_raycast): origin / direction
+        [B, R, 2] or [R, 2] (shared by the batch); direction is normalised here. A ray hits a body only where it enters
+        it within max_dist: an origin inside a body does not see that body. Returns (dist [B, R], body [B, R] int64
+        indexing [circles, polygons, obstacles], -1 for no hit, normal [B, R, 2] at the hit); a ray that hits nothing
+        reads max_dist with zero gradient and a zero normal, as does a zero or non-finite direction. Inactive bodies
+        (`active`) are invisible.
+        The kernel makes every discrete choice (which body, which edge). When a gradient or tangent is needed, dist and
+        normal are rebuilt from those choices with torch ops, so that gradients reach the origins, the directions, p,
+        the radii, the polygons' initial vertices and the obstacles' vertices (and forward_ad / torch.func work)."""
+        o = self._ray_arg(origin, "origin")
+        d = self._ray_arg(direction, "direction")
+        if o.shape[1] != d.shape[1]:
+            raise ValueError("direction: need as many rays as origin (%d), got %d" % (o.shape[1], d.shape[1]))
+        md = float(max_dist)
+        if not math.isfinite(md) or md < 0:
+            raise ValueError("max_dist: need a finite distance >= 0, got %r" % (max_dist,))
+        nrm = d.norm(dim=2, keepdim=True)
+        u = d / torch.where(nrm > 0, nrm, torch.ones_like(nrm))      # a zero direction stays zero: it hits nothing
+        lib = _lib.load()
+        B, R, nb, dev = self.B, int(o.shape[1]), self.nb, self.device
+        pverts = self.polygon_vertices() if self.np else None
+        tracked = (o, u, self.p, self.rad) + ((self.plocal,) if self.np else ()) + ((self.ov,) if self.no else ())
+        needs_graph = (torch.is_grad_enabled() and any(t.requires_grad for t in tracked)) or any(
+            _has_tangent(t) for t in tracked)
+        dc = lambda t: t.detach().contiguous() if t is not None else None
+
+        def cast(pos, rad, pv, ov, oo, uu, aw):
+            t = torch.empty(B, R, dtype=self.dtype, device=dev)
+            body = torch.empty(B, R, dtype=torch.int32, device=dev)
+            feat = torch.empty(B, R, dtype=torch.int32, device=dev)
+            normal = None if needs_graph else torch.empty(B, R, 2, dtype=self.dtype, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.lcpb200_raycast(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, R, md, _lib.ptr(pos), _lib.ptr(rad),
+                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(oo), _lib.ptr(uu), _lib.ptr(aw), _lib.ptr(t), _lib.ptr(body),
+                    _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
+            # tensors only: _DetectFn marks every output non-differentiable
+            return tuple(x for x in (t, body, feat, normal) if x is not None)
+        out = _detect(cast, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), dc(o),
+                      dc(u), self.active_words)
+        body = out[1].long()
+        if not needs_graph:
+            return out[0], body, out[3]
+        dist, normal = self._ray_torch(o, u, body, out[2].long(), md, pverts)
+        return dist, body, normal
+
+    def _ray_torch(self, o, u, body, feat, max_dist, pverts):
+        """Torch mirror of csrc/lcp_raycast.cuh, REBUILT FROM THE KERNEL'S CHOICES body / feat [B, R]: the circle's
+        entry t = k / (-b + sqrt(b^2 - k)) and normal (w + t u) / r, or the entering edge's t = n_e . (v_e - o) /
+        n_e . u and normal n_e; max_dist (a constant) and a zero normal where nothing is hit."""
+        nb, V = self.nb, self.nv
+        B, R = body.shape
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+        zero = torch.zeros_like(o)
+        is_c = (body >= 0) & (body < nb)
+        is_p = body >= nb
+        dist = torch.full((B, R), max_dist, dtype=o.dtype, device=o.device)
+        normal = zero
+        if nb:
+            ci = torch.where(is_c, body, 0)
+            w = o - take2(self.p[:, :nb, 1:], ci)
+            r = torch.gather(self.rad, 1, ci)
+            b = (u * w).sum(2)
+            k = (w * w).sum(2) - r * r
+            disc = torch.where(is_c, b * b - k, torch.ones_like(b))
+            den = torch.where(is_c, -b + disc.sqrt(), torch.ones_like(b))
+            t_c = k / den
+            n_c = (w + t_c.unsqueeze(2) * u) / torch.where(is_c, r, torch.ones_like(r)).unsqueeze(2)
+            dist = torch.where(is_c, t_c, dist)
+            normal = torch.where(is_c.unsqueeze(2), n_c, normal)
+        if self.np or self.no:
+            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            W = torch.roll(polys, -1, dims=2)
+            area = (polys[..., 0] * W[..., 1] - polys[..., 1] * W[..., 0]).sum(2)
+            orient = torch.where(area > 0, 1.0, -1.0).to(o.dtype)                                       # [B, P]
+            k = torch.where(is_p, body - nb, 0)
+            e = torch.where(is_p, feat, 0)
+            flat = polys.reshape(B, -1, 2)
+            ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
+            E = vf - ve
+            ln = E.norm(dim=2)
+            ln1 = torch.where(is_p, ln, torch.ones_like(ln))
+            sg = torch.gather(orient, 1, k)
+            n = torch.stack([sg * E[..., 1] / ln1, -sg * E[..., 0] / ln1], 2)
+            den = (n * u).sum(2)
+            t_p = (n * (ve - o)).sum(2) / torch.where(is_p, den, -torch.ones_like(den))
+            dist = torch.where(is_p, t_p, dist)
+            normal = torch.where(is_p.unsqueeze(2), n, normal)
+        return dist, normal
+
+    def lidar(self, body, n_rays, max_dist, fov=2 * math.pi, start=0.0):
+        """n_rays rays from the centre of dynamic body `body` (the same body in every scene), ray k at the angle
+        p[:, body, 0] + start + k fov / n_rays: a lidar turning with its body. The mounting body, whose centre lies
+        inside it, never appears in the readings. Returns what `raycast` returns."""
+        if isinstance(body, bool) or not isinstance(body, int) or not 0 <= body < self.nd:
+            raise ValueError("body: need the index of a dynamic body in [0, %d), got %r" % (self.nd, body))
+        if isinstance(n_rays, bool) or not isinstance(n_rays, int) or n_rays < 1:
+            raise ValueError("n_rays: need an int >= 1, got %r" % (n_rays,))
+        k = torch.arange(n_rays, dtype=self.dtype, device=self.device)
+        ang = self.p[:, body, 0:1] + start + k * float(fov) / n_rays                           # [B, n_rays]
+        direction = torch.stack([torch.cos(ang), torch.sin(ang)], 2)
+        origin = self.p[:, body, 1:].unsqueeze(1).expand(-1, n_rays, -1)
+        return self.raycast(origin, direction, max_dist)
+
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
         mass, inertia, v = self.mass, self.inertia, self.v
