@@ -307,6 +307,40 @@ int lcpb200_raycast(int dtype, int B, int nb, int np, int no, int nv, int R, dou
                     const void* rad, const void* pverts, const void* overts, const void* origin, const void* dir,
                     const int32_t* active_words, void* t, int32_t* body, int32_t* feat, void* normal, void* stream);
 
+/* Signed distances from query points to the bodies of B scenes (the body groups of lcpb200_contacts): Q points per
+ * scene (or Q points shared by every scene), each tested against the body list [circles 0..nb-1, polygons
+ * nb..nb+np-1, obstacles nb+np..nb+np+no-1] at their current pose; inactive bodies are skipped.
+ *   circle (c, r)                 sdf = |x - c| - r, feat -1, normal (x - c) / |x - c|; (0, 0) when x == c
+ *   polygon / obstacle            convex, either orientation; every edge of non-zero length e (start vertex v_e, end
+ *                                 vertex v_f, E = v_f - v_e, outward unit normal n_e) gives s_e = n_e . (x - v_e).
+ *                                 Inside (every s_e <= 0): sdf = max_e s_e, feat = 256 + e of the largest (the first
+ *                                 edge on a tie), normal n_e. Outside: t = clamp((x - v_e) . E / |E|^2, 0, 1), closest
+ *                                 point q_e = v_e if t <= 0, v_f (the vertex itself, not v_e + E) if t >= 1, else
+ *                                 v_e + t E; sdf = min_e |x - q_e| (the first edge on a tie: the two edges meeting at a
+ *                                 vertex tie exactly in its region), feat = e, normal (x - q) / |x - q|.
+ * The smallest sdf wins; an exact tie goes to the lower body index (from best = max_dist, body -1, a body replaces the
+ * best iff body < 0 ? sdf <= best : sdf < best). A point with no body at sdf <= max_dist, or a non-finite point, gets
+ * body -1, feat -1, sdf = max_dist and a zero normal. This is the exact Euclidean signed distance of one circle or
+ * convex polygon; for overlapping bodies it is the min of theirs, exact outside every body and a bound inside.
+ * Deterministic (no atomics); results do not depend on how the points are split into CTAs.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb]                             circles (NULL when nb == 0)
+ *   pverts[B,np,nv,2] overts[B,no,nv,2]               polygons and obstacles: world-frame vertices (NULL when the
+ *                                                     group is empty); a vertex repeated to pad to nv is skipped
+ *   points[B,Q,2], or [Q,2] with shared_points = 1    the query points; shared_points = 1: every scene reads the same Q
+ *   active_words[B, ceil(nt / 32)] int32              NULL (every body present), or the layout of
+ *                                                     lcpb200_contacts_active (nt <= 8192); inactive bodies are skipped
+ *   sdf[B,Q] body[B,Q] feat[B,Q] int32                OUT: signed distance, body index (-1: none within max_dist),
+ *                                                     feature (-1: a circle or none; e: outside, nearest edge e;
+ *                                                     256 + e: inside, nearest face e)
+ *   normal[B,Q,2]                                     OUT or NULL: the unit direction of increasing distance
+ * Returns non-zero without launching on B <= 0, Q <= 0, nb + np + no == 0, nv > 256 (or nv < 3 with polygons),
+ * max_dist < 0 or non-finite (in the dtype), a NULL required pointer, active_words with nt > 8192, or B * Q > 2^31 - 1. */
+int lcpb200_signed_distance(int dtype, int B, int nb, int np, int no, int nv, int Q, double max_dist, const void* pos,
+                            const void* rad, const void* pverts, const void* overts, const void* points,
+                            int shared_points, const int32_t* active_words, void* sdf, int32_t* body, int32_t* feat,
+                            void* normal, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

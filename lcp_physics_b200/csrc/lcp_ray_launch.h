@@ -1,4 +1,5 @@
-// lcp_ray_launch.h -- host-side launch interface of the batched ray cast (lcp_ray_kernels.cu, lcp_raycast.cuh).
+// lcp_ray_launch.h -- host-side launch interface of the batched ray cast and signed distance (lcp_ray_kernels.cu,
+// lcp_raycast.cuh, lcp_sdf.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,6 +27,26 @@ struct RayArgs {
 
 template <typename T>
 cudaError_t launch_raycast(const RayArgs<T>& a, int num_sms, cudaStream_t st);
+
+// One batch of query points against the bodies of lcpb200_signed_distance, bd as in RayArgs. points [B,Q,2], or [Q,2]
+// read by every scene when shared_points != 0; active as in RayArgs; outputs sdf / body / feat [B,Q], normal [B,Q,2]
+// or nullptr.
+template <typename T>
+struct SdfArgs {
+  cts::Bodies<T> bd;
+  int B, Q;
+  T max_dist;
+  const T* points;
+  int shared_points;
+  const uint32_t* active;
+  T* sdf;
+  int32_t* body;
+  int32_t* feat;
+  T* normal;
+};
+
+template <typename T>
+cudaError_t launch_sdf(const SdfArgs<T>& a, int num_sms, cudaStream_t st);
 
 }  // namespace ray
 }  // namespace lcpb200

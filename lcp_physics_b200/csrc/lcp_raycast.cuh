@@ -31,6 +31,59 @@ constexpr int TC = 256;       // circles per tile
 constexpr int TV = 1024;      // polygon vertices per tile (>= 4 polygons at nv = 256)
 constexpr int TP = 256;       // polygons per tile
 
+// Tile staging shared by raycast_kernel and sdf_kernel (lcp_sdf.cuh). Every thread of the CTA calls these with the same
+// arguments, between a barrier that frees the shared memory and one that publishes the tile.
+//
+// nb, nv are bd.nb, bd.nv and tid, nth threadIdx.x, blockDim.x, passed in from the kernel's registers.
+//
+// Circles c0 .. c0 + n - 1 of scene sc: centre, radius and active flag (aw: the scene's active words, or nullptr).
+template <typename T>
+__device__ __forceinline__ void stage_circles(const cts::Bodies<T>& bd, int nb, int sc, int c0, int n,
+                                              const uint32_t* aw, T* s_cx, T* s_cy, T* s_cr, unsigned char* s_con,
+                                              int tid, int nth) {
+  for (int k = tid; k < n; k += nth) {
+    const size_t g = (size_t)sc * nb + c0 + k;
+    const int b = c0 + k;
+    s_cx[k] = bd.pos[2 * g]; s_cy[k] = bd.pos[2 * g + 1]; s_cr[k] = bd.rad[g];
+    s_con[k] = aw ? (unsigned char)((__ldg(aw + (b >> 5)) >> (b & 31)) & 1u) : (unsigned char)1;
+  }
+}
+
+// Polygons q0 .. q0 + n - 1 of scene sc (bodies nb + q0 + k, dynamic polygons then obstacles): the vertices (polygon q
+// at s_pv[2 q nv]), the orientation s_po[q] (+-1 from poly_orient; 0: inactive), and per edge e the flag s_eok[q nv + e]
+// (edge_ok) and the outward unit normal s_pn[2 (q nv + e)] (zero for a zero-length edge). Holds two barriers of its own.
+template <typename T>
+__device__ __forceinline__ void stage_polygons(const cts::Bodies<T>& bd, int nb, int nv, int sc, int q0, int n,
+                                               const uint32_t* aw, T* s_pv, T* s_pn, unsigned char* s_eok,
+                                               signed char* s_po, int tid, int nth) {
+  for (int k = tid; k < n * nv; k += nth) {
+    const int q = k / nv, v = k - q * nv;
+    const T* P = bd.verts(sc, nb + q0 + q);
+    s_pv[2 * k] = P[2 * v]; s_pv[2 * k + 1] = P[2 * v + 1];
+  }
+  __syncthreads();
+  for (int q = tid; q < n; q += nth) {
+    const int b = nb + q0 + q;
+    const bool on = !aw || ((__ldg(aw + (b >> 5)) >> (b & 31)) & 1u);
+    s_po[q] = on ? (signed char)cts::poly_orient(&s_pv[2 * q * nv], nv) : (signed char)0;
+  }
+  __syncthreads();
+  for (int k = tid; k < n * nv; k += nth) {
+    const int q = k / nv, e = k - q * nv, f = e + 1 == nv ? 0 : e + 1;
+    const T* P = &s_pv[2 * q * nv];
+    const bool ok = cts::edge_ok(P, nv, e);
+    const T ex = P[2 * f] - P[2 * e], ey = P[2 * f + 1] - P[2 * e + 1];
+    const T len = sqrt(ex * ex + ey * ey);
+    const T o = T(s_po[q]);
+    s_eok[k] = ok;
+    s_pn[2 * k] = ok ? o * ey / len : T(0);
+    s_pn[2 * k + 1] = ok ? -o * ex / len : T(0);
+  }
+}
+
+// the polygons of one tile: as many as fit TV vertices, at most TP
+__host__ __device__ __forceinline__ int poly_tile(int npo, int nv) { return npo > 0 ? (TV / nv < TP ? TV / nv : TP) : 1; }
+
 template <typename T>
 __global__ void __launch_bounds__(NT) raycast_kernel(RayArgs<T> a, int chunks) {
   __shared__ T s_cx[TC], s_cy[TC], s_cr[TC];
@@ -43,7 +96,7 @@ __global__ void __launch_bounds__(NT) raycast_kernel(RayArgs<T> a, int chunks) {
   const cts::Bodies<T>& bd = a.bd;
   const int nb = bd.nb, npo = bd.np + bd.no, nv = bd.nv;
   const int nt = nb + npo, words = (nt + 31) >> 5;
-  const int ptile = npo > 0 ? (TV / nv < TP ? TV / nv : TP) : 1;
+  const int ptile = poly_tile(npo, nv);
   const T maxd = a.max_dist;
   const long long items = (long long)a.B * chunks;
   for (long long it = blockIdx.x; it < items; it += gridDim.x) {
@@ -51,7 +104,7 @@ __global__ void __launch_bounds__(NT) raycast_kernel(RayArgs<T> a, int chunks) {
     const int r = (int)(it - (long long)sc * chunks) * nth + tid;
     const bool live = r < a.R;
     const size_t ri = (size_t)sc * a.R + (live ? r : 0);
-    T ox = T(0), oy = T(0), ux = T(0), uy = T(0);
+    T ux = T(0), oy = T(0), ox = T(0), uy = T(0);       // this order keeps the SASS of before the staging helpers
     if (live) {
       ox = a.origin[2 * ri]; oy = a.origin[2 * ri + 1];
       ux = a.dir[2 * ri]; uy = a.dir[2 * ri + 1];
@@ -64,12 +117,7 @@ __global__ void __launch_bounds__(NT) raycast_kernel(RayArgs<T> a, int chunks) {
     for (int c0 = 0; c0 < nb; c0 += TC) {
       const int n = nb - c0 < TC ? nb - c0 : TC;
       __syncthreads();                                   // the previous tile (or work item) is done with the smem
-      for (int k = tid; k < n; k += nth) {
-        const size_t g = (size_t)sc * nb + c0 + k;
-        const int b = c0 + k;
-        s_cx[k] = bd.pos[2 * g]; s_cy[k] = bd.pos[2 * g + 1]; s_cr[k] = bd.rad[g];
-        s_con[k] = aw ? (unsigned char)((__ldg(aw + (b >> 5)) >> (b & 31)) & 1u) : (unsigned char)1;
-      }
+      stage_circles(bd, nb, sc, c0, n, aw, s_cx, s_cy, s_cr, s_con, tid, nth);
       __syncthreads();
       if (valid) {
         for (int k = 0; k < n; ++k) {
@@ -92,29 +140,7 @@ __global__ void __launch_bounds__(NT) raycast_kernel(RayArgs<T> a, int chunks) {
     for (int q0 = 0; q0 < npo; q0 += ptile) {
       const int n = npo - q0 < ptile ? npo - q0 : ptile;
       __syncthreads();
-      for (int k = tid; k < n * nv; k += nth) {
-        const int q = k / nv, v = k - q * nv;
-        const T* P = bd.verts(sc, nb + q0 + q);
-        s_pv[2 * k] = P[2 * v]; s_pv[2 * k + 1] = P[2 * v + 1];
-      }
-      __syncthreads();
-      for (int q = tid; q < n; q += nth) {
-        const int b = nb + q0 + q;
-        const bool on = !aw || ((__ldg(aw + (b >> 5)) >> (b & 31)) & 1u);
-        s_po[q] = on ? (signed char)cts::poly_orient(&s_pv[2 * q * nv], nv) : (signed char)0;
-      }
-      __syncthreads();
-      for (int k = tid; k < n * nv; k += nth) {
-        const int q = k / nv, e = k - q * nv, f = e + 1 == nv ? 0 : e + 1;
-        const T* P = &s_pv[2 * q * nv];
-        const bool ok = cts::edge_ok(P, nv, e);
-        const T ex = P[2 * f] - P[2 * e], ey = P[2 * f + 1] - P[2 * e + 1];
-        const T len = sqrt(ex * ex + ey * ey);
-        const T o = T(s_po[q]);
-        s_eok[k] = ok;
-        s_pn[2 * k] = ok ? o * ey / len : T(0);
-        s_pn[2 * k + 1] = ok ? -o * ex / len : T(0);
-      }
+      stage_polygons(bd, nb, nv, sc, q0, n, aw, s_pv, s_pn, s_eok, s_po, tid, nth);
       __syncthreads();
       if (valid) {
         for (int q = 0; q < n; ++q) {

@@ -1,0 +1,131 @@
+// lcp_sdf.cuh -- batched signed distances to the bodies of BatchedWorld scenes (lcpb200_signed_distance).
+//
+// A query point x is tested against the body list [circles, dynamic polygons, obstacles] of its scene, inactive bodies
+// skipped:
+//   circle (c, r):    sdf = |x - c| - r, feat -1, normal (x - c) / |x - c| ((0, 0) when x == c).
+//   convex polygon:   either orientation (poly_orient), zero-length padding edges skipped (edge_ok). Edge e runs from
+//                     v_e to v_f, E = v_f - v_e, outward unit normal n_e, s_e = n_e . (x - v_e).
+//                     inside (every s_e <= 0): sdf = max_e s_e, feat 256 + e of the largest (the first on a tie),
+//                     normal n_e.
+//                     outside: t = clamp((x - v_e) . E / |E|^2, 0, 1), q_e = v_e if t <= 0, v_f (the loaded vertex)
+//                     if t >= 1, else v_e + t E; sdf = min_e |x - q_e| (compared as |x - q_e|^2; the first edge wins a
+//                     tie, so the two edges meeting at a vertex tie exactly in its region and the lower one is
+//                     reported), feat e, normal (x - q) / |x - q|.
+// The smallest sdf wins, an exact tie goes to the lower body index: starting from best = max_dist, body -1, a body
+// replaces the best iff (body < 0 ? sdf <= best : sdf < best). Nothing within max_dist, or a non-finite point: body -1,
+// feat -1, sdf = max_dist, normal (0, 0). This is the exact Euclidean signed distance of one circle or convex polygon;
+// over overlapping bodies it is the min of their distances, exact outside every body and a bound inside.
+//
+// Layout: one CTA per (scene, chunk of blockDim.x points) work item, one point per thread, the best (sdf, body, feat,
+// normal) in registers; the bodies are staged through shared memory in the tiles of raycast_kernel (stage_circles,
+// stage_polygons). Every thread visits the bodies in index order, so the result depends neither on the chunking nor on
+// the tile sizes. No atomics.
+#pragma once
+#include "lcp_raycast.cuh"
+
+namespace lcpb200 {
+namespace ray {
+
+template <typename T>
+__global__ void __launch_bounds__(NT) sdf_kernel(SdfArgs<T> a, int chunks) {
+  __shared__ T s_cx[TC], s_cy[TC], s_cr[TC];
+  __shared__ unsigned char s_con[TC];
+  __shared__ T s_pv[2 * TV];
+  __shared__ T s_pn[2 * TV];
+  __shared__ unsigned char s_eok[TV];
+  __shared__ signed char s_po[TP];
+  const int tid = threadIdx.x, nth = blockDim.x;
+  const cts::Bodies<T>& bd = a.bd;
+  const int nb = bd.nb, npo = bd.np + bd.no, nv = bd.nv;
+  const int nt = nb + npo, words = (nt + 31) >> 5;
+  const int ptile = poly_tile(npo, nv);
+  const T maxd = a.max_dist;
+  const long long items = (long long)a.B * chunks;
+  for (long long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int sc = (int)(it / chunks);
+    const int r = (int)(it - (long long)sc * chunks) * nth + tid;
+    const bool live = r < a.Q;
+    const size_t ri = (size_t)sc * a.Q + (live ? r : 0);
+    const size_t pi = a.shared_points ? (size_t)(live ? r : 0) : ri;
+    T px = T(0), py = T(0);
+    if (live) { px = a.points[2 * pi]; py = a.points[2 * pi + 1]; }
+    const bool valid = live && isfinite(px) && isfinite(py);
+    const uint32_t* aw = a.active ? a.active + (size_t)sc * words : nullptr;
+    // the best body's normal is (bnx, bny) / blen: blen = |x - q| outside, 1 inside a polygon, 0 at a circle's centre
+    T best = maxd, bnx = T(0), bny = T(0), blen = T(0);
+    int bbody = -1, bfeat = -1;
+    // ---- circles
+    for (int c0 = 0; c0 < nb; c0 += TC) {
+      const int n = nb - c0 < TC ? nb - c0 : TC;
+      __syncthreads();                                   // the previous tile (or work item) is done with the smem
+      stage_circles(bd, nb, sc, c0, n, aw, s_cx, s_cy, s_cr, s_con, tid, nth);
+      __syncthreads();
+      if (valid) {
+        for (int k = 0; k < n; ++k) {
+          if (!s_con[k]) continue;
+          const T dx = px - s_cx[k], dy = py - s_cy[k];
+          const T d = sqrt(dx * dx + dy * dy);
+          const T s = d - s_cr[k];
+          if (bbody < 0 ? s <= best : s < best) {
+            best = s; bbody = c0 + k; bfeat = -1;
+            bnx = dx; bny = dy; blen = d;
+          }
+        }
+      }
+    }
+    // ---- polygons, then obstacles (polygon q is body nb + q)
+    for (int q0 = 0; q0 < npo; q0 += ptile) {
+      const int n = npo - q0 < ptile ? npo - q0 : ptile;
+      __syncthreads();
+      stage_polygons(bd, nb, nv, sc, q0, n, aw, s_pv, s_pn, s_eok, s_po, tid, nth);
+      __syncthreads();
+      if (valid) {
+        for (int q = 0; q < n; ++q) {
+          if (!s_po[q]) continue;
+          const T* P = &s_pv[2 * q * nv];
+          const T* N = &s_pn[2 * q * nv];
+          const unsigned char* ok = &s_eok[q * nv];
+          T smax = T(-INFINITY), dmin = T(INFINITY), qdx = T(0), qdy = T(0);
+          int emax = -1, emin = -1;
+          for (int e = 0; e < nv; ++e) {
+            if (!ok[e]) continue;
+            const int f = e + 1 == nv ? 0 : e + 1;
+            const T vx = P[2 * e], vy = P[2 * e + 1];
+            const T wx = px - vx, wy = py - vy;
+            const T s = N[2 * e] * wx + N[2 * e + 1] * wy;
+            if (s > smax) { smax = s; emax = e; }
+            const T ex = P[2 * f] - vx, ey = P[2 * f + 1] - vy;
+            const T t = (wx * ex + wy * ey) / (ex * ex + ey * ey);
+            T dx, dy;
+            if (t <= T(0)) { dx = wx; dy = wy; }
+            else if (t >= T(1)) { dx = px - P[2 * f]; dy = py - P[2 * f + 1]; }
+            else { dx = px - (vx + t * ex); dy = py - (vy + t * ey); }
+            const T d2 = dx * dx + dy * dy;
+            if (d2 < dmin) { dmin = d2; emin = e; qdx = dx; qdy = dy; }
+          }
+          if (emax < 0) continue;                        // no edge of non-zero length
+          const bool inside = smax <= T(0);
+          const T s = inside ? smax : sqrt(dmin);
+          if (bbody < 0 ? s <= best : s < best) {
+            best = s; bbody = nb + q0 + q;
+            if (inside) { bfeat = 256 + emax; bnx = N[2 * emax]; bny = N[2 * emax + 1]; blen = T(1); }
+            else { bfeat = emin; bnx = qdx; bny = qdy; blen = s; }
+          }
+        }
+      }
+    }
+    if (live) {
+      a.sdf[ri] = best;
+      a.body[ri] = bbody;
+      a.feat[ri] = bfeat;
+      if (a.normal) {
+        const bool nz = blen > T(0);
+        a.normal[2 * ri] = nz ? bnx / blen : T(0);
+        a.normal[2 * ri + 1] = nz ? bny / blen : T(0);
+      }
+    }
+  }
+}
+
+}  // namespace ray
+}  // namespace lcpb200

@@ -1205,6 +1205,51 @@ extern "C" int lcpb200_raycast(int dtype, int B, int nb, int np, int no, int nv,
   return 0;
 }
 
+// ------------------------------------------------------------------ signed distances
+extern "C" int lcpb200_signed_distance(int dtype, int B, int nb, int np, int no, int nv, int Q, double max_dist,
+                                       const void* pos, const void* rad, const void* pverts, const void* overts,
+                                       const void* points, int shared_points, const int32_t* active_words, void* sdf,
+                                       int32_t* body, int32_t* feat, void* normal, void* stream) {
+  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
+  if (B <= 0 || Q <= 0 || nb < 0 || np < 0 || no < 0)
+    return fail("signed_distance: need B, Q > 0 and nb, np, no >= 0");
+  const long long nt = (long long)nb + np + no;
+  if (nt == 0) return fail("signed_distance: no body (nb + np + no == 0)");
+  if (nt > 0x7fffffffLL) return fail("signed_distance: too many bodies");
+  if (nv > cts::MAX_NV || (np + no > 0 && nv < 3)) return fail("signed_distance: polygons need 3 <= nv <= 256 vertices");
+  if (!std::isfinite(max_dist) || max_dist < 0 || (dtype == LCPB200_F32 && max_dist > FLT_MAX))
+    return fail("signed_distance: need a finite max_dist >= 0");
+  if ((nb > 0 && (!pos || !rad)) || (np > 0 && !pverts) || (no > 0 && !overts) || !points || !sdf || !body || !feat)
+    return fail("signed_distance: NULL argument");
+  if (active_words && nt > cts::MAX_ACTIVE_NT)
+    return fail("signed_distance: at most 8192 bodies (nb + np + no) with active");
+  if ((long long)B * Q > 0x7fffffffLL) return fail("signed_distance: B * Q points exceed int32 indexing");
+  int dev = 0, sms = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == LCPB200_F32) {
+    ray::SdfArgs<float> a{};
+    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
+    a.bd.pos = (const float*)pos; a.bd.rad = (const float*)rad;
+    a.bd.pverts = (const float*)pverts; a.bd.overts = (const float*)overts;
+    a.B = B; a.Q = Q; a.max_dist = (float)max_dist;
+    a.points = (const float*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
+    a.sdf = (float*)sdf; a.body = body; a.feat = feat; a.normal = (float*)normal;
+    CK(ray::launch_sdf<float>(a, sms, st));
+  } else {
+    ray::SdfArgs<double> a{};
+    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
+    a.bd.pos = (const double*)pos; a.bd.rad = (const double*)rad;
+    a.bd.pverts = (const double*)pverts; a.bd.overts = (const double*)overts;
+    a.B = B; a.Q = Q; a.max_dist = max_dist;
+    a.points = (const double*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
+    a.sdf = (double*)sdf; a.body = body; a.feat = feat; a.normal = (double*)normal;
+    CK(ray::launch_sdf<double>(a, sms, st));
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------ assembly
 extern "C" int lcpb200_assemble(int dtype, int B, int nb, int nc, double dt, const void* mass, const void* inertia,
                                 const void* v, const void* fext, const void* normal, const void* p1,

@@ -319,6 +319,21 @@ def pack_bits(mask):
     return torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32).contiguous()
 
 
+def pixel_centres(height, width, lo, hi):
+    """Centres of a height x width pixel grid over the window [lo, hi] (BatchedWorld.render): pixel (i, j) sits at
+    (lo_x + (j + 1/2) (hi_x - lo_x) / width, lo_y + (i + 1/2) (hi_y - lo_y) / height), so row i grows with y (the
+    reference's screen, gravity along +y). lo / hi [2] give [height * width, 2], [B, 2] give [B, height * width, 2],
+    row-major (point i * width + j); differentiable in lo and hi."""
+    j = torch.arange(width, dtype=lo.dtype, device=lo.device) + 0.5
+    i = torch.arange(height, dtype=lo.dtype, device=lo.device) + 0.5
+    span = hi - lo
+    x = lo[..., 0:1] + j * span[..., 0:1] / width                                   # [..., W]
+    y = lo[..., 1:2] + i * span[..., 1:2] / height                                  # [..., H]
+    shape = lo.shape[:-1] + (height, width)
+    grid = torch.stack([x.unsqueeze(-2).expand(shape), y.unsqueeze(-1).expand(shape)], -1)
+    return grid.reshape(lo.shape[:-1] + (height * width, 2))
+
+
 def _pad_vertices(v, V):
     """[B, n, V0, 2] -> [B, n, V, 2] (V >= V0) by repeating the last vertex: a zero-length edge, skipped by every rule."""
     if v.shape[2] == V:
@@ -958,6 +973,153 @@ class BatchedWorld:
         direction = torch.stack([torch.cos(ang), torch.sin(ang)], 2)
         origin = self.p[:, body, 1:].unsqueeze(1).expand(-1, n_rays, -1)
         return self.raycast(origin, direction, max_dist)
+
+    # ------------------------------------------------------------------ signed distances and images
+    def signed_distance(self, points, max_dist):
+        """Signed distance from query points to every scene's bodies at the current state (lcpb200_signed_distance):
+        points [B, Q, 2], or [Q, 2] shared by the batch (read by every scene, not copied). Negative inside a body; the
+        min over the scene's bodies (exact outside every body, a bound inside where bodies overlap). Returns (sdf [B, Q],
+        body [B, Q] int64 indexing [circles, polygons, obstacles], -1 when no body lies within max_dist, normal [B, Q, 2],
+        the unit direction in which the distance grows); a point with no body within max_dist, or a non-finite point,
+        reads max_dist with zero gradient and a zero normal. Inactive bodies (`active`) are invisible.
+        The kernel makes every discrete choice (which body, which edge, inside or outside). When a gradient or tangent
+        is needed, sdf and normal are rebuilt from those choices with torch ops, so that gradients reach the points, p,
+        the radii, the polygons' initial vertices and the obstacles' vertices (and forward_ad / torch.func work)."""
+        return self._signed_distance(points, max_dist, True)
+
+    def _signed_distance(self, points, max_dist, with_normal):
+        if isinstance(points, torch.Tensor):
+            if not points.is_floating_point():
+                raise ValueError("points: need a floating-point tensor, got dtype %s" % (points.dtype,))
+            x = points.to(device=self.device, dtype=self.dtype)
+        else:
+            x = torch.as_tensor(points, dtype=self.dtype, device=self.device)
+        shared = x.dim() == 2
+        if not ((shared and x.shape[1] == 2 and x.shape[0] >= 1) or
+                (x.dim() == 3 and x.shape[0] == self.B and x.shape[2] == 2 and x.shape[1] >= 1)):
+            raise ValueError("points: need [B, Q, 2] or [Q, 2] with Q >= 1 (B = %d), got %s" % (self.B, tuple(x.shape)))
+        md = float(max_dist)
+        if not math.isfinite(md) or md < 0:
+            raise ValueError("max_dist: need a finite distance >= 0, got %r" % (max_dist,))
+        B, Q, nb, dev = self.B, int(x.shape[-2]), self.nb, self.device
+        if B * Q > 2 ** 31 - 1:
+            raise ValueError("points: B * Q = %d exceeds int32 indexing" % (B * Q))
+        lib = _lib.load()
+        pverts = self.polygon_vertices() if self.np else None
+        tracked = (x, self.p, self.rad) + ((self.plocal,) if self.np else ()) + ((self.ov,) if self.no else ())
+        needs_graph = (torch.is_grad_enabled() and any(t.requires_grad for t in tracked)) or any(
+            _has_tangent(t) for t in tracked)
+        dc = lambda t: t.detach().contiguous() if t is not None else None
+
+        def query(pos, rad, pv, ov, xx, aw):
+            sdf = torch.empty(B, Q, dtype=self.dtype, device=dev)
+            body = torch.empty(B, Q, dtype=torch.int32, device=dev)
+            feat = torch.empty(B, Q, dtype=torch.int32, device=dev)
+            normal = None if needs_graph or not with_normal else torch.empty(B, Q, 2, dtype=self.dtype, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.lcpb200_signed_distance(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, Q, md, _lib.ptr(pos), _lib.ptr(rad),
+                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(xx), int(shared), _lib.ptr(aw), _lib.ptr(sdf),
+                    _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
+            # tensors only: _DetectFn marks every output non-differentiable
+            return tuple(t for t in (sdf, body, feat, normal) if t is not None)
+        out = _detect(query, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), dc(x),
+                      self.active_words)
+        body = out[1].long()
+        if not needs_graph:
+            return out[0], body, out[3] if with_normal else None
+        sdf, normal = self._sdf_torch(x, body, out[2].long(), md, pverts)
+        return sdf, body, normal
+
+    def _sdf_torch(self, points, body, feat, max_dist, pverts):
+        """Torch mirror of csrc/lcp_sdf.cuh, REBUILT FROM THE KERNEL'S CHOICES body / feat [B, Q]: |x - c| - r and
+        (x - c) / |x - c| for a circle; n_e . (x - v_e) and n_e inside a polygon (feat 256 + e); outside (feat e) the
+        distance to the closest point q of edge e (v_e, v_f or v_e + t E) and (x - q) / |x - q|; max_dist (a constant)
+        and a zero normal where no body was chosen. points [B, Q, 2] or [Q, 2]. A zero distance (a point at a circle's
+        centre or on the closest point) gives a zero normal and finite gradients."""
+        nb, V = self.nb, self.nv
+        B, Q = body.shape
+        x = points.expand(B, Q, 2) if points.dim() == 2 else points
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+
+        def length(d):
+            """|d| and d / |d|, both 0 where d == 0 (no 0 / 0 in either pass)"""
+            n2 = (d * d).sum(2)
+            nz = n2 > 0
+            ln = torch.where(nz, n2, torch.ones_like(n2)).sqrt()
+            return torch.where(nz, ln, torch.zeros_like(ln)), torch.where(nz.unsqueeze(2), d / ln.unsqueeze(2),
+                                                                          torch.zeros_like(d))
+        is_c = (body >= 0) & (body < nb)
+        is_p = body >= nb
+        sdf = torch.full((B, Q), max_dist, dtype=x.dtype, device=x.device)
+        normal = torch.zeros_like(x)
+        if nb:
+            ci = torch.where(is_c, body, 0)
+            ln, n_c = length(x - take2(self.p[:, :nb, 1:], ci))
+            sdf = torch.where(is_c, ln - torch.gather(self.rad, 1, ci), sdf)
+            normal = torch.where(is_c.unsqueeze(2), n_c, normal)
+        if self.np or self.no:
+            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            W = torch.roll(polys, -1, dims=2)
+            area = (polys[..., 0] * W[..., 1] - polys[..., 1] * W[..., 0]).sum(2)
+            orient = torch.where(area > 0, 1.0, -1.0).to(x.dtype)                                       # [B, P]
+            k = torch.where(is_p, body - nb, 0)
+            inside = is_p & (feat >= 256)
+            e = torch.where(is_p, feat % 256, 0)
+            flat = polys.reshape(B, -1, 2)
+            ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
+            E = vf - ve
+            ee = torch.where(is_p, (E * E).sum(2), torch.ones_like(E[..., 0]))
+            ln = ee.sqrt()
+            sg = torch.gather(orient, 1, k)
+            n = torch.stack([sg * E[..., 1] / ln, -sg * E[..., 0] / ln], 2)
+            w = x - ve
+            t = ((w * E).sum(2) / ee).unsqueeze(2)
+            q = torch.where(t <= 0, ve, torch.where(t >= 1, vf, ve + t * E))
+            d_out, n_out = length(x - q)
+            sdf = torch.where(inside, (n * w).sum(2), torch.where(is_p, d_out, sdf))
+            normal = torch.where(inside.unsqueeze(2), n, torch.where(is_p.unsqueeze(2), n_out, normal))
+        return sdf, normal
+
+    def render(self, height, width, lo, hi, sigma=0.0, max_dist=None):
+        """An image of every scene on a height x width pixel grid over the window [lo, hi] (pixel_centres: row i grows
+        with y; lo = (0, 0), hi = (W, H) gives the reference's screen pixels). lo / hi [2] (one window for the batch) or
+        [B, 2] (one per scene, e.g. following a body: lo = w.p[:, k, 1:] - 50); both may require grad.
+        Returns (image [B, H, W], body [B, H, W] int64, sdf [B, H, W]) from signed_distance at the pixel centres:
+        sigma > 0 gives the soft silhouette sigmoid(-sdf / sigma), differentiable like sdf; sigma == 0 the hard one
+        (sdf <= 0) in the world's dtype, without gradient. body is the nearest body within max_dist (-1: none), so
+        that any per-body attribute can be painted with it. max_dist None: the largest window diagonal (read on the
+        host; pass max_dist explicitly under torch.func transforms)."""
+        for name, v in (("height", height), ("width", width)):
+            if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+                raise ValueError("%s: need an int >= 1, got %r" % (name, v))
+        if self.B * height * width > 2 ** 31 - 1:
+            raise ValueError("render: B * height * width = %d exceeds int32 indexing" % (self.B * height * width))
+        sg = float(sigma)
+        if not math.isfinite(sg) or sg < 0:
+            raise ValueError("sigma: need a finite value >= 0, got %r" % (sigma,))
+        win = []
+        for name, v in (("lo", lo), ("hi", hi)):
+            if isinstance(v, torch.Tensor):
+                if not v.is_floating_point():
+                    raise ValueError("%s: need a floating-point tensor, got dtype %s" % (name, v.dtype))
+                v = v.to(device=self.device, dtype=self.dtype)
+            else:
+                v = torch.as_tensor(v, dtype=self.dtype, device=self.device)
+            if v.shape not in ((2,), (self.B, 2)):
+                raise ValueError("%s: need [2] or [B, 2] (B = %d), got %s" % (name, self.B, tuple(v.shape)))
+            win.append(v)
+        lo, hi = win
+        if lo.dim() != hi.dim():
+            lo, hi = lo.expand(self.B, 2), hi.expand(self.B, 2)
+        if not bool((lo.detach() < hi.detach()).all()):
+            raise ValueError("render: need lo < hi in both coordinates")
+        if max_dist is None:
+            max_dist = float((hi.detach() - lo.detach()).norm(dim=-1).max())
+        sdf, body, _ = self._signed_distance(pixel_centres(height, width, lo, hi), max_dist, False)
+        image = torch.sigmoid(-sdf / sg) if sg > 0 else (sdf.detach() <= 0).to(self.dtype)
+        shape = (self.B, height, width)
+        return image.reshape(shape), body.reshape(shape), sdf.reshape(shape)
 
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
