@@ -6,14 +6,22 @@
 namespace lcpb200 {
 namespace ray {
 
+// Launch shape of n rays or points in each of B scenes: CTAs of nth threads, one ray or point per thread (short lists
+// use fewer threads), each CTA walking (scene, chunk) items; at most 16 CTAs per SM.
+struct Shape { int nth, chunks, grid; };
+
+static Shape launch_shape(int B, int n, int num_sms) {
+  const int nth = n >= NT ? NT : (n + 31) / 32 * 32;
+  const int chunks = (n + nth - 1) / nth;
+  const long long items = (long long)B * chunks;
+  const long long cap = 16LL * num_sms;
+  return {nth, chunks, (int)(items < cap ? items : cap)};
+}
+
 template <typename T>
 cudaError_t launch_raycast(const RayArgs<T>& a, int num_sms, cudaStream_t st) {
-  const int nth = a.R >= NT ? NT : (a.R + 31) / 32 * 32;    // one ray per thread; short ray lists use fewer threads
-  const int chunks = (a.R + nth - 1) / nth;
-  const long long items = (long long)a.B * chunks;
-  const long long cap = 16LL * num_sms;
-  const int grid = (int)(items < cap ? items : cap);
-  raycast_kernel<T><<<grid, nth, 0, st>>>(a, chunks);
+  const Shape s = launch_shape(a.B, a.R, num_sms);
+  raycast_kernel<T><<<s.grid, s.nth, 0, st>>>(a, s.chunks);
   return cudaGetLastError();
 }
 
@@ -22,12 +30,8 @@ template cudaError_t launch_raycast<double>(const RayArgs<double>&, int, cudaStr
 
 template <typename T>
 cudaError_t launch_sdf(const SdfArgs<T>& a, int num_sms, cudaStream_t st) {
-  const int nth = a.Q >= NT ? NT : (a.Q + 31) / 32 * 32;    // one point per thread; short point lists use fewer threads
-  const int chunks = (a.Q + nth - 1) / nth;
-  const long long items = (long long)a.B * chunks;
-  const long long cap = 16LL * num_sms;
-  const int grid = (int)(items < cap ? items : cap);
-  sdf_kernel<T><<<grid, nth, 0, st>>>(a, chunks);
+  const Shape s = launch_shape(a.B, a.Q, num_sms);
+  sdf_kernel<T><<<s.grid, s.nth, 0, st>>>(a, s.chunks);
   return cudaGetLastError();
 }
 

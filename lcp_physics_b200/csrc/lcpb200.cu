@@ -1064,6 +1064,14 @@ extern "C" int lcpb200_engine_backward(lcpb200_handle_t h, int B, int nb, int nc
 }
 
 // ------------------------------------------------------------------ contact detection
+// Multiprocessor count of the current device, which bounds the grids of the contact, ray and point kernels.
+static int current_sms(int& sms) {
+  int dev = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
+}
+
 // One body of lcpb200_contacts and lcpb200_contacts_active per dtype. The instantiation is chosen here and only here:
 // the active walk for lcpb200_contacts_active; else the mask walk when the caller passes no_contact, the polygon walk
 // (HULLS) when it passes feat, the circle walk otherwise; the geometry kernel follows the walk's HULLS.
@@ -1126,9 +1134,8 @@ static int contacts_entry(bool per_scene, int dtype, int B, int nb, int np, int 
   if (ngeo == 6 && ((nb > 0 && (!fric || !rest)) || (np > 0 && (!pfric || !prest)) || (no > 0 && (!ofric || !orest))))
     return fail("contacts: the geometry needs the friction and restitution of every body group");
   if (B == 0) return 0;
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
   (dtype == LCPB200_F32 ? contacts_t<float> : contacts_t<double>)(
       B, nb, np, no, nv, cap, eps, pos, rad, fric, rest, pverts, pcen, pfric, prest, overts, oref, ofric, orest, body1,
       body2, counts, feat, normal, p1, p2, pen, mu, rest_c, no_contact, per_scene, active, nc_stride, sms,
@@ -1161,92 +1168,85 @@ extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no,
                         no_contact, active, no_contact_stride, stream);
 }
 
-// ------------------------------------------------------------------ ray casts
+// ------------------------------------------------------------------ ray casts and signed distances
+// Argument checks shared by lcpb200_raycast and lcpb200_signed_distance. what prefixes the messages; N counts the
+// queries per scene, named n_name and counted as `items` in the messages. queries_set: the entry's own query pointers
+// (origin and dir, or points) are non-NULL, so that one message covers every NULL pointer.
+static int check_query(const char* what, const char* n_name, const char* items, int dtype, int B, int N, int nb,
+                       int np, int no, int nv, double max_dist, const void* pos, const void* rad, const void* pverts,
+                       const void* overts, bool queries_set, const void* value, const int32_t* body,
+                       const int32_t* feat, const int32_t* active_words) {
+  const std::string w(what);
+  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
+  if (B <= 0 || N <= 0 || nb < 0 || np < 0 || no < 0)
+    return fail(w + ": need B, " + n_name + " > 0 and nb, np, no >= 0");
+  const long long nt = (long long)nb + np + no;
+  if (nt == 0) return fail(w + ": no body (nb + np + no == 0)");
+  if (nt > 0x7fffffffLL) return fail(w + ": too many bodies");
+  if (nv > cts::MAX_NV || (np + no > 0 && nv < 3)) return fail(w + ": polygons need 3 <= nv <= 256 vertices");
+  if (!std::isfinite(max_dist) || max_dist < 0 || (dtype == LCPB200_F32 && max_dist > FLT_MAX))
+    return fail(w + ": need a finite max_dist >= 0");
+  if ((nb > 0 && (!pos || !rad)) || (np > 0 && !pverts) || (no > 0 && !overts) || !queries_set || !value || !body ||
+      !feat)
+    return fail(w + ": NULL argument");
+  if (active_words && nt > cts::MAX_ACTIVE_NT) return fail(w + ": at most 8192 bodies (nb + np + no) with active");
+  if ((long long)B * N > 0x7fffffffLL)
+    return fail(w + ": B * " + n_name + " " + items + " exceed int32 indexing");
+  return 0;
+}
+
+// The bodies of a ray or point query in the layout of cts::Bodies; neither kernel reads the material and centroid
+// pointers, which stay NULL.
+template <typename T>
+static cts::Bodies<T> query_bodies(int nb, int np, int no, int nv, const void* pos, const void* rad, const void* pverts,
+                                   const void* overts) {
+  cts::Bodies<T> bd{};
+  bd.nb = nb; bd.np = np; bd.no = no; bd.nv = nv;
+  bd.pos = (const T*)pos; bd.rad = (const T*)rad; bd.pverts = (const T*)pverts; bd.overts = (const T*)overts;
+  return bd;
+}
+
 extern "C" int lcpb200_raycast(int dtype, int B, int nb, int np, int no, int nv, int R, double max_dist,
                                const void* pos, const void* rad, const void* pverts, const void* overts,
                                const void* origin, const void* dir, const int32_t* active_words, void* t,
                                int32_t* body, int32_t* feat, void* normal, void* stream) {
-  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
-  if (B <= 0 || R <= 0 || nb < 0 || np < 0 || no < 0) return fail("raycast: need B, R > 0 and nb, np, no >= 0");
-  const long long nt = (long long)nb + np + no;
-  if (nt == 0) return fail("raycast: no body (nb + np + no == 0)");
-  if (nt > 0x7fffffffLL) return fail("raycast: too many bodies");
-  if (nv > cts::MAX_NV || (np + no > 0 && nv < 3)) return fail("raycast: polygons need 3 <= nv <= 256 vertices");
-  if (!std::isfinite(max_dist) || max_dist < 0 || (dtype == LCPB200_F32 && max_dist > FLT_MAX))
-    return fail("raycast: need a finite max_dist >= 0");
-  if ((nb > 0 && (!pos || !rad)) || (np > 0 && !pverts) || (no > 0 && !overts) || !origin || !dir || !t || !body ||
-      !feat)
-    return fail("raycast: NULL argument");
-  if (active_words && nt > cts::MAX_ACTIVE_NT) return fail("raycast: at most 8192 bodies (nb + np + no) with active");
-  if ((long long)B * R > 0x7fffffffLL) return fail("raycast: B * R rays exceed int32 indexing");
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32) {
-    ray::RayArgs<float> a{};
-    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
-    a.bd.pos = (const float*)pos; a.bd.rad = (const float*)rad;
-    a.bd.pverts = (const float*)pverts; a.bd.overts = (const float*)overts;
-    a.B = B; a.R = R; a.max_dist = (float)max_dist;
-    a.origin = (const float*)origin; a.dir = (const float*)dir; a.active = (const uint32_t*)active_words;
-    a.t = (float*)t; a.body = body; a.feat = feat; a.normal = (float*)normal;
-    CK(ray::launch_raycast<float>(a, sms, st));
-  } else {
-    ray::RayArgs<double> a{};
-    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
-    a.bd.pos = (const double*)pos; a.bd.rad = (const double*)rad;
-    a.bd.pverts = (const double*)pverts; a.bd.overts = (const double*)overts;
-    a.B = B; a.R = R; a.max_dist = max_dist;
-    a.origin = (const double*)origin; a.dir = (const double*)dir; a.active = (const uint32_t*)active_words;
-    a.t = (double*)t; a.body = body; a.feat = feat; a.normal = (double*)normal;
-    CK(ray::launch_raycast<double>(a, sms, st));
-  }
+  if (int rc = check_query("raycast", "R", "rays", dtype, B, R, nb, np, no, nv, max_dist, pos, rad, pverts, overts,
+                           origin && dir, t, body, feat, active_words))
+    return rc;
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
+  auto launch = [&](auto zero) {      // the body for T = the type of zero
+    using T = decltype(zero);
+    ray::RayArgs<T> a{};
+    a.bd = query_bodies<T>(nb, np, no, nv, pos, rad, pverts, overts);
+    a.B = B; a.R = R; a.max_dist = (T)max_dist;
+    a.origin = (const T*)origin; a.dir = (const T*)dir; a.active = (const uint32_t*)active_words;
+    a.t = (T*)t; a.body = body; a.feat = feat; a.normal = (T*)normal;
+    return ray::launch_raycast<T>(a, sms, (cudaStream_t)stream);
+  };
+  CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
   return 0;
 }
 
-// ------------------------------------------------------------------ signed distances
 extern "C" int lcpb200_signed_distance(int dtype, int B, int nb, int np, int no, int nv, int Q, double max_dist,
                                        const void* pos, const void* rad, const void* pverts, const void* overts,
                                        const void* points, int shared_points, const int32_t* active_words, void* sdf,
                                        int32_t* body, int32_t* feat, void* normal, void* stream) {
-  if (dtype != LCPB200_F32 && dtype != LCPB200_F64) return fail("bad dtype");
-  if (B <= 0 || Q <= 0 || nb < 0 || np < 0 || no < 0)
-    return fail("signed_distance: need B, Q > 0 and nb, np, no >= 0");
-  const long long nt = (long long)nb + np + no;
-  if (nt == 0) return fail("signed_distance: no body (nb + np + no == 0)");
-  if (nt > 0x7fffffffLL) return fail("signed_distance: too many bodies");
-  if (nv > cts::MAX_NV || (np + no > 0 && nv < 3)) return fail("signed_distance: polygons need 3 <= nv <= 256 vertices");
-  if (!std::isfinite(max_dist) || max_dist < 0 || (dtype == LCPB200_F32 && max_dist > FLT_MAX))
-    return fail("signed_distance: need a finite max_dist >= 0");
-  if ((nb > 0 && (!pos || !rad)) || (np > 0 && !pverts) || (no > 0 && !overts) || !points || !sdf || !body || !feat)
-    return fail("signed_distance: NULL argument");
-  if (active_words && nt > cts::MAX_ACTIVE_NT)
-    return fail("signed_distance: at most 8192 bodies (nb + np + no) with active");
-  if ((long long)B * Q > 0x7fffffffLL) return fail("signed_distance: B * Q points exceed int32 indexing");
-  int dev = 0, sms = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == LCPB200_F32) {
-    ray::SdfArgs<float> a{};
-    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
-    a.bd.pos = (const float*)pos; a.bd.rad = (const float*)rad;
-    a.bd.pverts = (const float*)pverts; a.bd.overts = (const float*)overts;
-    a.B = B; a.Q = Q; a.max_dist = (float)max_dist;
-    a.points = (const float*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
-    a.sdf = (float*)sdf; a.body = body; a.feat = feat; a.normal = (float*)normal;
-    CK(ray::launch_sdf<float>(a, sms, st));
-  } else {
-    ray::SdfArgs<double> a{};
-    a.bd.nb = nb; a.bd.np = np; a.bd.no = no; a.bd.nv = nv;
-    a.bd.pos = (const double*)pos; a.bd.rad = (const double*)rad;
-    a.bd.pverts = (const double*)pverts; a.bd.overts = (const double*)overts;
-    a.B = B; a.Q = Q; a.max_dist = max_dist;
-    a.points = (const double*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
-    a.sdf = (double*)sdf; a.body = body; a.feat = feat; a.normal = (double*)normal;
-    CK(ray::launch_sdf<double>(a, sms, st));
-  }
+  if (int rc = check_query("signed_distance", "Q", "points", dtype, B, Q, nb, np, no, nv, max_dist, pos, rad, pverts,
+                           overts, points != nullptr, sdf, body, feat, active_words))
+    return rc;
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
+  auto launch = [&](auto zero) {      // the body for T = the type of zero
+    using T = decltype(zero);
+    ray::SdfArgs<T> a{};
+    a.bd = query_bodies<T>(nb, np, no, nv, pos, rad, pverts, overts);
+    a.B = B; a.Q = Q; a.max_dist = (T)max_dist;
+    a.points = (const T*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
+    a.sdf = (T*)sdf; a.body = body; a.feat = feat; a.normal = (T*)normal;
+    return ray::launch_sdf<T>(a, sms, (cudaStream_t)stream);
+  };
+  CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
   return 0;
 }
 

@@ -127,6 +127,34 @@ def polygon_inertia(rel, mass):
     return mass * num / nc.sum(-1) / 6
 
 
+def _orientation(polys):
+    """Orientation sign of polygons [..., V, 2] in their dtype: 1 where the shoelace area is positive
+    (counter-clockwise), else -1 (poly_orient of csrc/lcp_contacts.cuh)."""
+    W = torch.roll(polys, -1, dims=-2)
+    area = (polys[..., 0] * W[..., 1] - polys[..., 1] * W[..., 0]).sum(-1)
+    return torch.where(area > 0, 1.0, -1.0).to(polys.dtype)
+
+
+def _edge_normal(E, orient, ln):
+    """Outward unit normal orient (E_y, -E_x) / ln of edges E [..., 2] of polygons of orientation sign orient [...];
+    ln is |E|, made non-zero by the caller where an edge is not used."""
+    return torch.stack([orient * E[..., 1] / ln, -orient * E[..., 0] / ln], -1)
+
+
+def _chosen_edge(polys, body, edge, nb):
+    """Edge `edge` of body `body` ([B, n] each) of a world whose polygons polys [B, P, V, 2] are bodies nb, nb + 1,
+    ...: (v_e, v_f = the next vertex, E = v_f - v_e, the polygon's orientation sign [B, n]). Slots whose body is not a
+    polygon read edge 0 of polygon 0, so that they stay finite."""
+    B, _, V, _ = polys.shape
+    is_p = body >= nb
+    k = torch.where(is_p, body - nb, 0)
+    e = torch.where(is_p, edge, 0)
+    take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+    flat = polys.reshape(B, -1, 2)
+    ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
+    return ve, vf, vf - ve, torch.gather(_orientation(polys), 1, k)
+
+
 # ------------------------------------------------------------------ constraints.py:13-173, by body index
 class Joint:
     """Revolute joint (constraints.py:13-53) between bodies i and j (j None: a joint to the world point `anchor`) at
@@ -232,6 +260,27 @@ def _has_tangent(t):
     """True when t carries a forward-mode tangent: an input of torch.func.jvp / jacfwd (a functorch-wrapped tensor) or
     a torch.autograd.forward_ad dual tensor. Forward mode leaves requires_grad False."""
     return t is not None and fwAD.unpack_dual(t).tangent is not None
+
+
+def _needs_graph(tensors):
+    """True when a result computed from `tensors` (None entries allowed) must be rebuilt with torch ops: one of them
+    requires grad under grad mode, or carries a forward-mode tangent."""
+    return (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)) or any(
+        _has_tangent(t) for t in tensors)
+
+
+def _max_dist(max_dist):
+    """max_dist of a ray cast or signed distance as a float, finite and >= 0."""
+    md = float(max_dist)
+    if not math.isfinite(md) or md < 0:
+        raise ValueError("max_dist: need a finite distance >= 0, got %r" % (max_dist,))
+    return md
+
+
+def _check_count(v, name):
+    """Rejects a count (rays, pixels) that is not an int >= 1; bool is not a count."""
+    if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+        raise ValueError("%s: need an int >= 1, got %r" % (name, v))
 
 
 MAX_ACTIVE_BODIES = 8192        # bodies of a world walked per scene (the kernel's shared-memory list of active bodies)
@@ -612,9 +661,7 @@ class BatchedWorld:
         pverts = self.polygon_vertices() if self.np else None
         poly = (self.plocal, self.pfric, self.prest) if self.np else (None,) * 3
         obst = (self.ov, self.oref, self.ofric, self.orest) if self.no else (None,) * 4
-        tracked = (self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst
-        needs_graph = (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tracked)) or any(
-            _has_tangent(t) for t in tracked)
+        needs_graph = _needs_graph((self.p, self.rad, self.fric_coeff, self.restitution) + poly + obst)
         # feat selects the polygon walk, which worlds with polygons, no_contact pairs or per-scene bodies need; the
         # others keep the circle walk
         with_feat = self.np > 0 or self.nc_mask is not None or self.per_scene
@@ -686,13 +733,9 @@ class BatchedWorld:
         take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         cr, ci = take2(ref, kr), take2(ref, ki)
         vtx = lambda Vx, e: torch.gather(Vx, 2, e.unsqueeze(2).unsqueeze(3).expand(-1, -1, 1, 2)).squeeze(2)
-        Wr = torch.roll(Vr, -1, dims=2)
-        area = (Vr[..., 0] * Wr[..., 1] - Vr[..., 1] * Wr[..., 0]).sum(2)
-        orient = torch.where(area > 0, 1.0, -1.0).to(verts.dtype)
         E = vtx(Vr, (re + 1) % V) - vtx(Vr, re)
         ln = E.norm(dim=2)
-        ln1 = torch.where(ln > 0, ln, torch.ones_like(ln))
-        n = torch.stack([orient * E[..., 1] / ln1, -orient * E[..., 0] / ln1], 2)   # outward normal of the reference edge
+        n = _edge_normal(E, _orientation(Vr), torch.where(ln > 0, ln, torch.ones_like(ln)))   # of the reference edge
         r = vtx(Vr, re) - cr
         h = (ln / 2).unsqueeze(2)
         v0, v1 = vtx(Vi, ie) - cr, vtx(Vi, (ie + 1) % V) - cr                        # incident edge, reference frame
@@ -720,14 +763,11 @@ class BatchedWorld:
         B, P = k.shape
         verts = self.ov if verts is None else verts
         V = torch.gather(verts, 1, k.reshape(B, P, 1, 1).expand(B, P, self.nv, 2))          # [B,P,V,2]
-        Wv = torch.roll(V, -1, dims=2)
-        E = Wv - V
-        area = (V[..., 0] * Wv[..., 1] - V[..., 1] * Wv[..., 0]).sum(2)
-        orient = torch.where(area > 0, 1.0, -1.0).to(V.dtype).unsqueeze(2)
+        E = torch.roll(V, -1, dims=2) - V
         ln = E.norm(dim=3)
         dg = ~(ln > 0)                                     # zero-length edges (repeated vertices): skipped, as the kernel
-        ln1 = torch.where(dg, torch.ones_like(ln), ln)     # keeps the skipped entries finite, gradients too
-        nrm = torch.stack([orient * E[..., 1] / ln1, -orient * E[..., 0] / ln1], 3)        # outward unit normals
+        # a length of 1 keeps the skipped entries finite, gradients too
+        nrm = _edge_normal(E, _orientation(V).unsqueeze(2), torch.where(dg, torch.ones_like(ln), ln))
         rel = c.unsqueeze(2) - V
         sp = torch.where(dg, torch.full_like(ln, -math.inf), (nrm * rel).sum(3))
         inside = ~(sp > 0).any(2)
@@ -854,20 +894,49 @@ class BatchedWorld:
         return self.c_pen.max(dim=1)[0]
 
     # ------------------------------------------------------------------ ray casts
-    def _ray_arg(self, x, name):
-        """A ray argument [B, R, 2] or [R, 2] (shared by the batch) as a [B, R, 2] tensor of the world's dtype / device."""
+    def _float_arg(self, x, name):
+        """x as a tensor of the world's dtype and device; a tensor must be floating-point."""
         if isinstance(x, torch.Tensor):
             if not x.is_floating_point():
                 raise ValueError("%s: need a floating-point tensor, got dtype %s" % (name, x.dtype))
-            x = x.to(device=self.device, dtype=self.dtype)
-        else:
-            x = torch.as_tensor(x, dtype=self.dtype, device=self.device)
+            return x.to(device=self.device, dtype=self.dtype)
+        return torch.as_tensor(x, dtype=self.dtype, device=self.device)
+
+    def _ray_arg(self, x, name):
+        """A ray argument [B, R, 2] or [R, 2] (shared by the batch) as a [B, R, 2] tensor of the world's dtype / device."""
+        x = self._float_arg(x, name)
         if x.dim() == 2:
             x = x.unsqueeze(0).expand(self.B, -1, -1)
         if x.dim() != 3 or x.shape[0] != self.B or x.shape[2] != 2 or x.shape[1] == 0:
             raise ValueError("%s: need [B, R, 2] or [R, 2] with R >= 1 (B = %d), got %s"
                              % (name, self.B, tuple(x.shape)))
         return x
+
+    def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts):
+        """One call of the ray or point kernel `entry` (lcpb200_raycast or lcpb200_signed_distance) over n rays or
+        points per scene at the current state. The entry's arguments between overts and active_words are the tensors
+        `queries`, then the ints `flags`. pverts: polygon_vertices() (worlds with polygons). Returns (value [B, n], body
+        [B, n] int64, feat [B, n] int32, normal [B, n, 2] when with_normal, else None)."""
+        lib = _lib.load()
+        B, nb, dev = self.B, self.nb, self.device
+        dc = lambda t: t.detach().contiguous() if t is not None else None
+
+        def call(pos, rad, pv, ov, aw, *qs):
+            value = torch.empty(B, n, dtype=self.dtype, device=dev)
+            body = torch.empty(B, n, dtype=torch.int32, device=dev)
+            feat = torch.empty(B, n, dtype=torch.int32, device=dev)
+            normal = torch.empty(B, n, 2, dtype=self.dtype, device=dev) if with_normal else None
+            with torch.cuda.device(dev):
+                _lib.check(getattr(lib, entry)(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, n, max_dist, _lib.ptr(pos),
+                    _lib.ptr(rad), _lib.ptr(pv), _lib.ptr(ov), *[_lib.ptr(q) for q in qs], *flags, _lib.ptr(aw),
+                    _lib.ptr(value), _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
+            # tensors only: _DetectFn marks every output non-differentiable
+            return tuple(t for t in (value, body, feat, normal) if t is not None)
+        # contiguous copies, arguments of the call until it returns
+        out = _detect(call, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None),
+                      self.active_words, *[dc(q) for q in queries])
+        return out[0], out[1].long(), out[2], out[3] if with_normal else None
 
     def raycast(self, origin, direction, max_dist):
         """Casts rays against every scene's bodies at the current state (lcpb200_raycast): origin / direction
@@ -883,44 +952,23 @@ class BatchedWorld:
         d = self._ray_arg(direction, "direction")
         if o.shape[1] != d.shape[1]:
             raise ValueError("direction: need as many rays as origin (%d), got %d" % (o.shape[1], d.shape[1]))
-        md = float(max_dist)
-        if not math.isfinite(md) or md < 0:
-            raise ValueError("max_dist: need a finite distance >= 0, got %r" % (max_dist,))
+        md = _max_dist(max_dist)
         nrm = d.norm(dim=2, keepdim=True)
         u = d / torch.where(nrm > 0, nrm, torch.ones_like(nrm))      # a zero direction stays zero: it hits nothing
-        lib = _lib.load()
-        B, R, nb, dev = self.B, int(o.shape[1]), self.nb, self.device
         pverts = self.polygon_vertices() if self.np else None
-        tracked = (o, u, self.p, self.rad) + ((self.plocal,) if self.np else ()) + ((self.ov,) if self.no else ())
-        needs_graph = (torch.is_grad_enabled() and any(t.requires_grad for t in tracked)) or any(
-            _has_tangent(t) for t in tracked)
-        dc = lambda t: t.detach().contiguous() if t is not None else None
-
-        def cast(pos, rad, pv, ov, oo, uu, aw):
-            t = torch.empty(B, R, dtype=self.dtype, device=dev)
-            body = torch.empty(B, R, dtype=torch.int32, device=dev)
-            feat = torch.empty(B, R, dtype=torch.int32, device=dev)
-            normal = None if needs_graph else torch.empty(B, R, 2, dtype=self.dtype, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_raycast(
-                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, R, md, _lib.ptr(pos), _lib.ptr(rad),
-                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(oo), _lib.ptr(uu), _lib.ptr(aw), _lib.ptr(t), _lib.ptr(body),
-                    _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
-            # tensors only: _DetectFn marks every output non-differentiable
-            return tuple(x for x in (t, body, feat, normal) if x is not None)
-        out = _detect(cast, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), dc(o),
-                      dc(u), self.active_words)
-        body = out[1].long()
-        if not needs_graph:
-            return out[0], body, out[3]
-        dist, normal = self._ray_torch(o, u, body, out[2].long(), md, pverts)
+        needs_graph = _needs_graph((o, u, self.p, self.rad, self.plocal if self.np else None,
+                                    self.ov if self.no else None))
+        dist, body, feat, normal = self._query("lcpb200_raycast", (o, u), (), int(o.shape[1]), md, not needs_graph,
+                                                 pverts)
+        if needs_graph:
+            dist, normal = self._ray_torch(o, u, body, feat.long(), md, pverts)
         return dist, body, normal
 
     def _ray_torch(self, o, u, body, feat, max_dist, pverts):
         """Torch mirror of csrc/lcp_raycast.cuh, REBUILT FROM THE KERNEL'S CHOICES body / feat [B, R]: the circle's
         entry t = k / (-b + sqrt(b^2 - k)) and normal (w + t u) / r, or the entering edge's t = n_e . (v_e - o) /
         n_e . u and normal n_e; max_dist (a constant) and a zero normal where nothing is hit."""
-        nb, V = self.nb, self.nv
+        nb = self.nb
         B, R = body.shape
         take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         zero = torch.zeros_like(o)
@@ -942,18 +990,9 @@ class BatchedWorld:
             normal = torch.where(is_c.unsqueeze(2), n_c, normal)
         if self.np or self.no:
             polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
-            W = torch.roll(polys, -1, dims=2)
-            area = (polys[..., 0] * W[..., 1] - polys[..., 1] * W[..., 0]).sum(2)
-            orient = torch.where(area > 0, 1.0, -1.0).to(o.dtype)                                       # [B, P]
-            k = torch.where(is_p, body - nb, 0)
-            e = torch.where(is_p, feat, 0)
-            flat = polys.reshape(B, -1, 2)
-            ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
-            E = vf - ve
+            ve, _, E, sg = _chosen_edge(polys, body, feat, nb)
             ln = E.norm(dim=2)
-            ln1 = torch.where(is_p, ln, torch.ones_like(ln))
-            sg = torch.gather(orient, 1, k)
-            n = torch.stack([sg * E[..., 1] / ln1, -sg * E[..., 0] / ln1], 2)
+            n = _edge_normal(E, sg, torch.where(is_p, ln, torch.ones_like(ln)))
             den = (n * u).sum(2)
             t_p = (n * (ve - o)).sum(2) / torch.where(is_p, den, -torch.ones_like(den))
             dist = torch.where(is_p, t_p, dist)
@@ -966,8 +1005,7 @@ class BatchedWorld:
         inside it, never appears in the readings. Returns what `raycast` returns."""
         if isinstance(body, bool) or not isinstance(body, int) or not 0 <= body < self.nd:
             raise ValueError("body: need the index of a dynamic body in [0, %d), got %r" % (self.nd, body))
-        if isinstance(n_rays, bool) or not isinstance(n_rays, int) or n_rays < 1:
-            raise ValueError("n_rays: need an int >= 1, got %r" % (n_rays,))
+        _check_count(n_rays, "n_rays")
         k = torch.arange(n_rays, dtype=self.dtype, device=self.device)
         ang = self.p[:, body, 0:1] + start + k * float(fov) / n_rays                           # [B, n_rays]
         direction = torch.stack([torch.cos(ang), torch.sin(ang)], 2)
@@ -988,47 +1026,22 @@ class BatchedWorld:
         return self._signed_distance(points, max_dist, True)
 
     def _signed_distance(self, points, max_dist, with_normal):
-        if isinstance(points, torch.Tensor):
-            if not points.is_floating_point():
-                raise ValueError("points: need a floating-point tensor, got dtype %s" % (points.dtype,))
-            x = points.to(device=self.device, dtype=self.dtype)
-        else:
-            x = torch.as_tensor(points, dtype=self.dtype, device=self.device)
+        x = self._float_arg(points, "points")
         shared = x.dim() == 2
         if not ((shared and x.shape[1] == 2 and x.shape[0] >= 1) or
                 (x.dim() == 3 and x.shape[0] == self.B and x.shape[2] == 2 and x.shape[1] >= 1)):
             raise ValueError("points: need [B, Q, 2] or [Q, 2] with Q >= 1 (B = %d), got %s" % (self.B, tuple(x.shape)))
-        md = float(max_dist)
-        if not math.isfinite(md) or md < 0:
-            raise ValueError("max_dist: need a finite distance >= 0, got %r" % (max_dist,))
-        B, Q, nb, dev = self.B, int(x.shape[-2]), self.nb, self.device
+        md = _max_dist(max_dist)
+        B, Q = self.B, int(x.shape[-2])
         if B * Q > 2 ** 31 - 1:
             raise ValueError("points: B * Q = %d exceeds int32 indexing" % (B * Q))
-        lib = _lib.load()
         pverts = self.polygon_vertices() if self.np else None
-        tracked = (x, self.p, self.rad) + ((self.plocal,) if self.np else ()) + ((self.ov,) if self.no else ())
-        needs_graph = (torch.is_grad_enabled() and any(t.requires_grad for t in tracked)) or any(
-            _has_tangent(t) for t in tracked)
-        dc = lambda t: t.detach().contiguous() if t is not None else None
-
-        def query(pos, rad, pv, ov, xx, aw):
-            sdf = torch.empty(B, Q, dtype=self.dtype, device=dev)
-            body = torch.empty(B, Q, dtype=torch.int32, device=dev)
-            feat = torch.empty(B, Q, dtype=torch.int32, device=dev)
-            normal = None if needs_graph or not with_normal else torch.empty(B, Q, 2, dtype=self.dtype, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_signed_distance(
-                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, Q, md, _lib.ptr(pos), _lib.ptr(rad),
-                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(xx), int(shared), _lib.ptr(aw), _lib.ptr(sdf),
-                    _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
-            # tensors only: _DetectFn marks every output non-differentiable
-            return tuple(t for t in (sdf, body, feat, normal) if t is not None)
-        out = _detect(query, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), dc(x),
-                      self.active_words)
-        body = out[1].long()
-        if not needs_graph:
-            return out[0], body, out[3] if with_normal else None
-        sdf, normal = self._sdf_torch(x, body, out[2].long(), md, pverts)
+        needs_graph = _needs_graph((x, self.p, self.rad, self.plocal if self.np else None,
+                                    self.ov if self.no else None))
+        sdf, body, feat, normal = self._query("lcpb200_signed_distance", (x,), (int(shared),), Q, md,
+                                              with_normal and not needs_graph, pverts)
+        if needs_graph:
+            sdf, normal = self._sdf_torch(x, body, feat.long(), md, pverts)
         return sdf, body, normal
 
     def _sdf_torch(self, points, body, feat, max_dist, pverts):
@@ -1037,7 +1050,7 @@ class BatchedWorld:
         distance to the closest point q of edge e (v_e, v_f or v_e + t E) and (x - q) / |x - q|; max_dist (a constant)
         and a zero normal where no body was chosen. points [B, Q, 2] or [Q, 2]. A zero distance (a point at a circle's
         centre or on the closest point) gives a zero normal and finite gradients."""
-        nb, V = self.nb, self.nv
+        nb = self.nb
         B, Q = body.shape
         x = points.expand(B, Q, 2) if points.dim() == 2 else points
         take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
@@ -1060,19 +1073,10 @@ class BatchedWorld:
             normal = torch.where(is_c.unsqueeze(2), n_c, normal)
         if self.np or self.no:
             polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
-            W = torch.roll(polys, -1, dims=2)
-            area = (polys[..., 0] * W[..., 1] - polys[..., 1] * W[..., 0]).sum(2)
-            orient = torch.where(area > 0, 1.0, -1.0).to(x.dtype)                                       # [B, P]
-            k = torch.where(is_p, body - nb, 0)
             inside = is_p & (feat >= 256)
-            e = torch.where(is_p, feat % 256, 0)
-            flat = polys.reshape(B, -1, 2)
-            ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
-            E = vf - ve
+            ve, vf, E, sg = _chosen_edge(polys, body, feat % 256, nb)
             ee = torch.where(is_p, (E * E).sum(2), torch.ones_like(E[..., 0]))
-            ln = ee.sqrt()
-            sg = torch.gather(orient, 1, k)
-            n = torch.stack([sg * E[..., 1] / ln, -sg * E[..., 0] / ln], 2)
+            n = _edge_normal(E, sg, ee.sqrt())
             w = x - ve
             t = ((w * E).sum(2) / ee).unsqueeze(2)
             q = torch.where(t <= 0, ve, torch.where(t >= 1, vf, ve + t * E))
@@ -1090,9 +1094,8 @@ class BatchedWorld:
         (sdf <= 0) in the world's dtype, without gradient. body is the nearest body within max_dist (-1: none), so
         that any per-body attribute can be painted with it. max_dist None: the largest window diagonal (read on the
         host; pass max_dist explicitly under torch.func transforms)."""
-        for name, v in (("height", height), ("width", width)):
-            if isinstance(v, bool) or not isinstance(v, int) or v < 1:
-                raise ValueError("%s: need an int >= 1, got %r" % (name, v))
+        _check_count(height, "height")
+        _check_count(width, "width")
         if self.B * height * width > 2 ** 31 - 1:
             raise ValueError("render: B * height * width = %d exceeds int32 indexing" % (self.B * height * width))
         sg = float(sigma)
@@ -1100,12 +1103,7 @@ class BatchedWorld:
             raise ValueError("sigma: need a finite value >= 0, got %r" % (sigma,))
         win = []
         for name, v in (("lo", lo), ("hi", hi)):
-            if isinstance(v, torch.Tensor):
-                if not v.is_floating_point():
-                    raise ValueError("%s: need a floating-point tensor, got dtype %s" % (name, v.dtype))
-                v = v.to(device=self.device, dtype=self.dtype)
-            else:
-                v = torch.as_tensor(v, dtype=self.dtype, device=self.device)
+            v = self._float_arg(v, name)
             if v.shape not in ((2,), (self.B, 2)):
                 raise ValueError("%s: need [2] or [B, 2] (B = %d), got %s" % (name, self.B, tuple(v.shape)))
             win.append(v)
