@@ -341,6 +341,52 @@ int lcpb200_signed_distance(int dtype, int B, int nb, int np, int no, int nv, in
                             int shared_points, const int32_t* active_words, void* sdf, int32_t* body, int32_t* feat,
                             void* normal, void* stream);
 
+/* Distances between bodies of B scenes (the body groups of lcpb200_contacts), K queries per scene (or K queries shared
+ * by every scene). Every pair (A, B) reduces to the signed distance of one feature point of one body (the source: a
+ * circle's centre, radius r, or a polygon's vertex, r = 0) to the other body (the target), minus r. Target distances
+ * and choices are those of lcpb200_signed_distance (feat -1 circle, e outside / nearest edge e, 256 + e face e):
+ *   circle i - circle j         source the centre of i: d = |c_i - c_j| - r_j - r_i
+ *   circle - polygon            source the circle's centre (either order): d = sdf(centre, polygon) - r
+ *   polygon - polygon           S = max over the faces e of both polygons of min over the other's vertices v of
+ *                               n_e . (v - v_e) (A's faces win a tie; either orientation, zero-length padding edges
+ *                               skipped). S > 0 (separated): d is the exact Euclidean distance, min over A's vertices
+ *                               of their outside distance to B and over B's vertices of theirs to A (the first vertex
+ *                               wins a tie, A's before B's), target feat e. S <= 0 (overlapping or touching): d = S,
+ *                               the minimum translation distance; source the support vertex of the SAT face (the last
+ *                               maximal vertex), target feat 256 + e.
+ * normal is the unit normal n from A towards B (moving B along n increases d): minus the target's sdf normal at the
+ * source when A is the source, that normal when B is; zero where the source is the target's closest point. point_a is
+ * the witness on A; point_b = point_a + d n is the witness on B. When separated both lie on the boundaries and
+ * |point_b - point_a| = d; when overlapping one is the support vertex and the other its projection onto the SAT face's
+ * supporting line, which need not lie on the face segment.
+ * Pair mode (body_b != NULL): query k reads the pair (body_a[k], body_b[k]) and body[k] = body_b[k] on a hit. Nearest
+ * mode (body_b == NULL): query k reads body_a[k] and finds the nearest other active body of its scene, obstacles
+ * included, skipping the pairs of no_contact; candidates in index order, from best = max_dist, body -1, a body
+ * replaces the best iff body < 0 ? d <= best : d < best. A hit iff d <= max_dist. A query whose body is inactive or out
+ * of range, that names one body twice, or with nothing within max_dist reads dist = max_dist, body -1, feat -1 and
+ * zero normal and point_a. Deterministic (no atomics); results do not depend on how the queries are split into CTAs.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb] pverts[B,np,nv,2] overts[B,no,nv,2]   the bodies, as in lcpb200_signed_distance
+ *   body_a[B,K] int32, or [K] with shared_queries = 1  the first body of each pair, or the query body (nearest mode)
+ *   body_b[B,K] int32, or [K] with shared_queries = 1  the second body of each pair; NULL: nearest mode
+ *   active_words[B, ceil(nt / 32)] int32              NULL, or the layout of lcpb200_contacts_active (nt <= 8192)
+ *   no_contact, nc_stride                             NULL, or the pair masks of lcpb200_contacts_active (bit
+ *                                                     i * nt + j for i < j; scene s at no_contact + s * nc_stride,
+ *                                                     nc_stride 0: one mask shared by the batch); nearest mode only
+ *   dist[B,K] body[B,K] feat[B,K] int32               OUT: distance, the other body (-1: a miss), and the choices:
+ *                                                     bits 0-8 the target's sdf feat (e or 256 + e; 0 for a circle
+ *                                                     target), bits 9-16 the source vertex (0 for a circle), bit 17
+ *                                                     set iff B is the source; -1 on a miss
+ *   normal[B,K,2] point_a[B,K,2]                      OUT: n and the witness on A
+ * Returns non-zero without launching on B <= 0, K <= 0, nb + np + no == 0, nv > 256 (or nv < 3 with polygons),
+ * max_dist < 0 or non-finite (in the dtype), a NULL required pointer (body_a, the bodies, every output),
+ * nc_stride < 0, active_words with nt > 8192, or B * K > 2^31 - 1. */
+int lcpb200_body_distance(int dtype, int B, int nb, int np, int no, int nv, int K, double max_dist, const void* pos,
+                          const void* rad, const void* pverts, const void* overts, const int32_t* body_a,
+                          const int32_t* body_b, int shared_queries, const int32_t* active_words,
+                          const int32_t* no_contact, long long nc_stride, void* dist, int32_t* body, int32_t* feat,
+                          void* normal, void* point_a, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

@@ -1,12 +1,14 @@
-// lcp_ray_kernels.cu -- the batched ray cast (lcp_raycast.cuh) and signed distance (lcp_sdf.cuh), fp32 and fp64, in a
-// translation unit of their own so that the contact, assembly and solver objects do not change.
+// lcp_ray_kernels.cu -- the batched ray cast (lcp_raycast.cuh), signed distance (lcp_sdf.cuh) and body distance
+// (lcp_distance.cuh), fp32 and fp64, in a translation unit of their own so that the contact, assembly and solver objects
+// do not change.
 #include "lcp_raycast.cuh"
 #include "lcp_sdf.cuh"
+#include "lcp_distance.cuh"
 
 namespace lcpb200 {
 namespace ray {
 
-// Launch shape of n rays or points in each of B scenes: CTAs of nth threads, one ray or point per thread (short lists
+// Launch shape of n rays, points or body queries in each of B scenes: CTAs of nth threads, one ray or point per thread (short lists
 // use fewer threads), each CTA walking (scene, chunk) items; at most 16 CTAs per SM.
 struct Shape { int nth, chunks, grid; };
 
@@ -37,6 +39,16 @@ cudaError_t launch_sdf(const SdfArgs<T>& a, int num_sms, cudaStream_t st) {
 
 template cudaError_t launch_sdf<float>(const SdfArgs<float>&, int, cudaStream_t);
 template cudaError_t launch_sdf<double>(const SdfArgs<double>&, int, cudaStream_t);
+
+template <typename T>
+cudaError_t launch_distance(const DistArgs<T>& a, int num_sms, cudaStream_t st) {
+  const Shape s = launch_shape(a.B, a.K, num_sms);
+  distance_kernel<T><<<s.grid, s.nth, 0, st>>>(a, s.chunks);
+  return cudaGetLastError();
+}
+
+template cudaError_t launch_distance<float>(const DistArgs<float>&, int, cudaStream_t);
+template cudaError_t launch_distance<double>(const DistArgs<double>&, int, cudaStream_t);
 
 }  // namespace ray
 }  // namespace lcpb200

@@ -1,5 +1,5 @@
-// lcp_ray_launch.h -- host-side launch interface of the batched ray cast and signed distance (lcp_ray_kernels.cu,
-// lcp_raycast.cuh, lcp_sdf.cuh).
+// lcp_ray_launch.h -- host-side launch interface of the batched ray cast, signed distance and body distance
+// (lcp_ray_kernels.cu, lcp_raycast.cuh, lcp_sdf.cuh, lcp_distance.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,6 +47,31 @@ struct SdfArgs {
 
 template <typename T>
 cudaError_t launch_sdf(const SdfArgs<T>& a, int num_sms, cudaStream_t st);
+
+// One batch of body-distance queries of lcpb200_body_distance, bd as in RayArgs. body_a [B,K], or [K] read by every
+// scene when shared_queries != 0; body_b likewise for pair mode, nullptr for nearest mode. active as in RayArgs;
+// no_contact: nullptr, or the pair bitmask of lcpb200_contacts_active (scene s at no_contact + s nc_stride), read in
+// nearest mode only. Outputs dist / body / feat [B,K], normal / point_a [B,K,2].
+template <typename T>
+struct DistArgs {
+  cts::Bodies<T> bd;
+  int B, K;
+  T max_dist;
+  const int32_t* body_a;
+  const int32_t* body_b;
+  int shared_queries;
+  const uint32_t* active;
+  const uint32_t* no_contact;
+  long long nc_stride;
+  T* dist;
+  int32_t* body;
+  int32_t* feat;
+  T* normal;
+  T* point_a;
+};
+
+template <typename T>
+cudaError_t launch_distance(const DistArgs<T>& a, int num_sms, cudaStream_t st);
 
 }  // namespace ray
 }  // namespace lcpb200

@@ -26,6 +26,66 @@
 namespace lcpb200 {
 namespace ray {
 
+// The edges of a polygon staged by stage_polygons: vertex e at P[2 e], edge flag ok[e] (edge_ok), outward unit normal
+// N[2 e].
+template <typename T>
+struct StagedEdges {
+  const T* P;
+  const T* N;
+  const unsigned char* ok_;
+  __device__ __forceinline__ bool ok(int e) const { return ok_[e]; }
+  __device__ __forceinline__ T nx(int e) const { return N[2 * e]; }
+  __device__ __forceinline__ T ny(int e) const { return N[2 * e + 1]; }
+};
+
+// The edges of a polygon whose normals were not staged (vertices P, orientation o from poly_orient): the flag and the
+// normal computed with the expressions of stage_polygons.
+template <typename T>
+struct LoadedEdges {
+  const T* P;
+  T o;
+  int nv;
+  __device__ __forceinline__ bool ok(int e) const { return cts::edge_ok(P, nv, e); }
+  __device__ __forceinline__ T ex(int e) const { return P[2 * (e + 1 == nv ? 0 : e + 1)] - P[2 * e]; }
+  __device__ __forceinline__ T ey(int e) const { return P[2 * (e + 1 == nv ? 0 : e + 1) + 1] - P[2 * e + 1]; }
+  __device__ __forceinline__ T nx(int e) const {
+    const T x = ex(e), y = ey(e);
+    return o * y / sqrt(x * x + y * y);
+  }
+  __device__ __forceinline__ T ny(int e) const {
+    const T x = ex(e), y = ey(e);
+    return -o * x / sqrt(x * x + y * y);
+  }
+};
+
+// The choices of the signed distance of point (px, py) to one convex polygon g (StagedEdges or LoadedEdges of nv
+// vertices), the rule above: smax / emax the largest s_e and its edge (emax < 0: no edge of non-zero length), dmin /
+// emin the smallest |x - q_e|^2 and its edge, (qdx, qdy) = x - q of that edge. Shared by sdf_kernel and distance_kernel
+// (lcp_distance.cuh).
+template <typename T, class G>
+__device__ __forceinline__ void point_polygon(const G& g, int nv, T px, T py, T& smax, int& emax, T& dmin, int& emin,
+                                              T& qdx, T& qdy) {
+  const T* P = g.P;
+  smax = T(-INFINITY); dmin = T(INFINITY); qdx = T(0); qdy = T(0);
+  emax = -1; emin = -1;
+  for (int e = 0; e < nv; ++e) {
+    if (!g.ok(e)) continue;
+    const int f = e + 1 == nv ? 0 : e + 1;
+    const T vx = P[2 * e], vy = P[2 * e + 1];
+    const T wx = px - vx, wy = py - vy;
+    const T s = g.nx(e) * wx + g.ny(e) * wy;
+    if (s > smax) { smax = s; emax = e; }
+    const T ex = P[2 * f] - vx, ey = P[2 * f + 1] - vy;
+    const T t = (wx * ex + wy * ey) / (ex * ex + ey * ey);
+    T dx, dy;
+    if (t <= T(0)) { dx = wx; dy = wy; }
+    else if (t >= T(1)) { dx = px - P[2 * f]; dy = py - P[2 * f + 1]; }
+    else { dx = px - (vx + t * ex); dy = py - (vy + t * ey); }
+    const T d2 = dx * dx + dy * dy;
+    if (d2 < dmin) { dmin = d2; emin = e; qdx = dx; qdy = dy; }
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(NT) sdf_kernel(SdfArgs<T> a, int chunks) {
   __shared__ T s_cx[TC], s_cy[TC], s_cr[TC];
@@ -85,24 +145,9 @@ __global__ void __launch_bounds__(NT) sdf_kernel(SdfArgs<T> a, int chunks) {
           const T* P = &s_pv[2 * q * nv];
           const T* N = &s_pn[2 * q * nv];
           const unsigned char* ok = &s_eok[q * nv];
-          T smax = T(-INFINITY), dmin = T(INFINITY), qdx = T(0), qdy = T(0);
-          int emax = -1, emin = -1;
-          for (int e = 0; e < nv; ++e) {
-            if (!ok[e]) continue;
-            const int f = e + 1 == nv ? 0 : e + 1;
-            const T vx = P[2 * e], vy = P[2 * e + 1];
-            const T wx = px - vx, wy = py - vy;
-            const T s = N[2 * e] * wx + N[2 * e + 1] * wy;
-            if (s > smax) { smax = s; emax = e; }
-            const T ex = P[2 * f] - vx, ey = P[2 * f + 1] - vy;
-            const T t = (wx * ex + wy * ey) / (ex * ex + ey * ey);
-            T dx, dy;
-            if (t <= T(0)) { dx = wx; dy = wy; }
-            else if (t >= T(1)) { dx = px - P[2 * f]; dy = py - P[2 * f + 1]; }
-            else { dx = px - (vx + t * ex); dy = py - (vy + t * ey); }
-            const T d2 = dx * dx + dy * dy;
-            if (d2 < dmin) { dmin = d2; emin = e; qdx = dx; qdy = dy; }
-          }
+          T smax, dmin, qdx, qdy;
+          int emax, emin;
+          point_polygon(StagedEdges<T>{P, N, ok}, nv, px, py, smax, emax, dmin, emin, qdx, qdy);
           if (emax < 0) continue;                        // no edge of non-zero length
           const bool inside = smax <= T(0);
           const T s = inside ? smax : sqrt(dmin);

@@ -1168,8 +1168,8 @@ extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no,
                         no_contact, active, no_contact_stride, stream);
 }
 
-// ------------------------------------------------------------------ ray casts and signed distances
-// Argument checks shared by lcpb200_raycast and lcpb200_signed_distance. what prefixes the messages; N counts the
+// ------------------------------------------------------------------ ray casts, signed distances and body distances
+// Argument checks shared by lcpb200_raycast, lcpb200_signed_distance and lcpb200_body_distance. what prefixes the messages; N counts the
 // queries per scene, named n_name and counted as `items` in the messages. queries_set: the entry's own query pointers
 // (origin and dir, or points) are non-NULL, so that one message covers every NULL pointer.
 static int check_query(const char* what, const char* n_name, const char* items, int dtype, int B, int N, int nb,
@@ -1245,6 +1245,33 @@ extern "C" int lcpb200_signed_distance(int dtype, int B, int nb, int np, int no,
     a.points = (const T*)points; a.shared_points = shared_points != 0; a.active = (const uint32_t*)active_words;
     a.sdf = (T*)sdf; a.body = body; a.feat = feat; a.normal = (T*)normal;
     return ray::launch_sdf<T>(a, sms, (cudaStream_t)stream);
+  };
+  CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
+  return 0;
+}
+
+extern "C" int lcpb200_body_distance(int dtype, int B, int nb, int np, int no, int nv, int K, double max_dist,
+                                     const void* pos, const void* rad, const void* pverts, const void* overts,
+                                     const int32_t* body_a, const int32_t* body_b, int shared_queries,
+                                     const int32_t* active_words, const int32_t* no_contact, long long nc_stride,
+                                     void* dist, int32_t* body, int32_t* feat, void* normal, void* point_a,
+                                     void* stream) {
+  if (int rc = check_query("body_distance", "K", "queries", dtype, B, K, nb, np, no, nv, max_dist, pos, rad, pverts,
+                           overts, body_a != nullptr, dist, body, feat, active_words))
+    return rc;
+  if (!normal || !point_a) return fail("body_distance: NULL argument");
+  if (nc_stride < 0) return fail("body_distance: need nc_stride >= 0");
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
+  auto launch = [&](auto zero) {      // the body for T = the type of zero
+    using T = decltype(zero);
+    ray::DistArgs<T> a{};
+    a.bd = query_bodies<T>(nb, np, no, nv, pos, rad, pverts, overts);
+    a.B = B; a.K = K; a.max_dist = (T)max_dist;
+    a.body_a = body_a; a.body_b = body_b; a.shared_queries = shared_queries != 0;
+    a.active = (const uint32_t*)active_words; a.no_contact = (const uint32_t*)no_contact; a.nc_stride = nc_stride;
+    a.dist = (T*)dist; a.body = body; a.feat = feat; a.normal = (T*)normal; a.point_a = (T*)point_a;
+    return ray::launch_distance<T>(a, sms, (cudaStream_t)stream);
   };
   CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
   return 0;

@@ -1119,6 +1119,123 @@ class BatchedWorld:
         shape = (self.B, height, width)
         return image.reshape(shape), body.reshape(shape), sdf.reshape(shape)
 
+    # ------------------------------------------------------------------ distances between bodies
+    def _body_arg(self, x, name, pair):
+        """Body indices [K] / [B, K] (pair: [K, 2] / [B, K, 2]) indexing [circles, polygons, obstacles], as an int32
+        tensor on the world's device; returns (indices, shared by the batch)."""
+        t = x if isinstance(x, torch.Tensor) else torch.as_tensor(x)
+        want = "[K, 2] or [B, K, 2]" if pair else "[K] or [B, K]"
+        d = t.dim() - (1 if pair else 0)
+        if d not in (1, 2) or (pair and t.shape[-1] != 2) or (d == 2 and t.shape[0] != self.B):
+            raise ValueError("%s: need %s (B = %d), got %s" % (name, want, self.B, tuple(t.shape)))
+        K = int(t.shape[d - 1])
+        if K == 0:
+            raise ValueError("%s: need K >= 1 queries, got %s" % (name, tuple(t.shape)))
+        if t.dtype == torch.bool or t.is_floating_point() or t.is_complex():
+            raise ValueError("%s: need integer body indices, got dtype %s" % (name, t.dtype))
+        if self.B * K > 2 ** 31 - 1:
+            raise ValueError("%s: B * K = %d exceeds int32 indexing" % (name, self.B * K))
+        nt = self.nd + self.no
+        lo, hi = int(t.min()), int(t.max())
+        if lo < 0 or hi >= nt:
+            raise ValueError("%s: body index %d out of range (%d bodies)" % (name, lo if lo < 0 else hi, nt))
+        if pair and bool((t[..., 0] == t[..., 1]).any()):
+            raise ValueError("%s: a pair names one body twice" % name)
+        return t.to(device=self.device, dtype=torch.int32), d == 1
+
+    def distance(self, pairs, max_dist):
+        """Distance between the bodies of each pair at the current state (lcpb200_body_distance, pair mode): pairs
+        [K, 2] (shared by the batch) or [B, K, 2] of indices into [circles, polygons, obstacles]. The rule (DESIGN.md
+        section 8): the signed distance of one feature point of one body (a circle's centre minus its radius, or a
+        polygon's vertex) to the other body; the exact Euclidean distance for separated bodies, and for overlapping
+        polygons minus the minimum translation distance. Returns (dist [B, K], body [B, K] int64: the pair's second body,
+        -1 when it is not within max_dist or a body is inactive, normal [B, K, 2]: the unit normal from the first body
+        towards the second, point_a / point_b [B, K, 2]: the witnesses on the two bodies, point_b = point_a + dist
+        normal). When separated the witnesses lie on the two boundaries; when overlapping one is the support vertex and
+        the other its projection onto the supporting line of the separating face, which need not lie on the face
+        segment. A miss reads max_dist, zero normal and witnesses, and zero gradient.
+        The kernel makes every discrete choice (source point, target edge or face). When a gradient or tangent is
+        needed, the outputs are rebuilt from those choices with torch ops (_distance_torch), so that gradients reach p,
+        the radii, the polygons' initial vertices and the obstacles' vertices (and forward_ad / torch.func work)."""
+        t, shared = self._body_arg(pairs, "pairs", True)
+        return self._body_distance(t[..., 0], t[..., 1], shared, max_dist)
+
+    def nearest(self, bodies, max_dist):
+        """The nearest other body of each query body at the current state (lcpb200_body_distance, nearest mode):
+        bodies [K] (shared by the batch) or [B, K] of indices into [circles, polygons, obstacles]. Candidates are every
+        other active body of the scene, obstacles included, except the world's `no_contact` pairs (so that a link of a
+        jointed chain does not read its neighbour at the joint); the lower index wins a tie. Returns what `distance`
+        returns for the pair (query, nearest), with body the nearest body (-1: none within max_dist, or an inactive
+        query body)."""
+        t, shared = self._body_arg(bodies, "bodies", False)
+        return self._body_distance(t, None, shared, max_dist)
+
+    def _body_distance(self, ba, bb, shared, max_dist):
+        md = _max_dist(max_dist)
+        lib = _lib.load()
+        B, nb, dev = self.B, self.nb, self.device
+        K = int(ba.shape[-1])
+        pverts = self.polygon_vertices() if self.np else None
+        needs_graph = _needs_graph((self.p, self.rad, self.plocal if self.np else None, self.ov if self.no else None))
+        dc = lambda t: t.detach().contiguous() if t is not None else None
+        nc_stride = self.nc_stride if bb is None else 0
+
+        def call(pos, rad, pv, ov, aw, qa, qb, nc):
+            new = lambda *s_: torch.empty(B, K, *s_, dtype=self.dtype, device=dev)
+            dist, normal, point_a = new(), new(2), new(2)
+            body = torch.empty(B, K, dtype=torch.int32, device=dev)
+            feat = torch.empty(B, K, dtype=torch.int32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.lcpb200_body_distance(
+                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, K, md, _lib.ptr(pos), _lib.ptr(rad),
+                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(qa), _lib.ptr(qb), int(shared), _lib.ptr(aw), _lib.ptr(nc),
+                    nc_stride, _lib.ptr(dist), _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.ptr(point_a),
+                    _lib.stream_ptr(dev)))
+            # tensors only: _DetectFn marks every output non-differentiable
+            return dist, body, feat, normal, point_a
+        # contiguous copies, arguments of the call until it returns
+        dist, body, feat, normal, point_a = _detect(
+            call, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), self.active_words,
+            ba.contiguous(), dc(bb), self.nc_mask if bb is None else None)
+        body = body.long()
+        if needs_graph:
+            dist, normal, point_a, point_b = self._distance_torch(ba.long().expand(B, K), body, feat.long(), md, pverts)
+            return dist, body, normal, point_a, point_b
+        return dist, body, normal, point_a, point_a + dist.unsqueeze(2) * normal
+
+    def _distance_torch(self, ba, bo, feat, max_dist, pverts):
+        """Torch mirror of csrc/lcp_distance.cuh, REBUILT FROM THE KERNEL'S CHOICES: ba [B, K] the first body, bo [B, K]
+        the kernel's other body (-1: a miss), feat its packed choices. The source point x and radius r (a circle's
+        centre and radius, or polygon vertex feat >> 9 & 255 and 0) of the source body (the other body iff bit 17),
+        then one _sdf_torch of x against the target with the target feat (bits 0-8): d = sdf - r, n = -m (the first body
+        the source) or m (the other), point_a = x - r m or x - sdf m, point_b = point_a + d n. A miss reads max_dist (a
+        constant) and zeros. Returns (dist, normal, point_a, point_b)."""
+        nb = self.nb
+        B, K = bo.shape
+        hit = bo >= 0
+        src_b = hit & (((feat >> 17) & 1) == 1)
+        src = torch.where(src_b, bo, ba)
+        tgt = torch.where(hit, torch.where(src_b, ba, bo), -1)
+        is_c = src < nb
+        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+        dt = self.dtype
+        x = torch.zeros(B, K, 2, dtype=dt, device=self.device)
+        r = torch.zeros(B, K, dtype=dt, device=self.device)
+        if nb:
+            ci = torch.where(is_c, src, 0)
+            x = take2(self.p[:, :nb, 1:], ci)
+            r = torch.where(is_c, torch.gather(self.rad, 1, ci), r)
+        if self.np or self.no:
+            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            vi = torch.where(is_c | ~hit, 0, (src - nb) * self.nv + ((feat >> 9) & 255))   # a miss's feat is -1
+            x = torch.where(is_c.unsqueeze(2), x, take2(polys.reshape(B, -1, 2), vi))
+        sdf, m = self._sdf_torch(x, tgt, feat & 511, max_dist, pverts)
+        dist = torch.where(hit, sdf - r, sdf)
+        normal = torch.where(src_b.unsqueeze(2), m, -m)
+        w = torch.where(src_b, sdf, r)
+        point_a = torch.where(hit.unsqueeze(2), x - w.unsqueeze(2) * m, torch.zeros_like(x))
+        return dist, normal, point_a, point_a + dist.unsqueeze(2) * normal
+
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
         mass, inertia, v = self.mass, self.inertia, self.v
