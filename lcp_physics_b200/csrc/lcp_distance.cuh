@@ -22,9 +22,9 @@
 //
 // Layout: that of sdf_kernel, one CTA per (scene, chunk of blockDim.x queries) work item, one query per thread. The
 // query's own body (both bodies in pair mode) is read from global memory; in nearest mode the candidates are staged
-// through shared memory in the tiles of raycast_kernel (stage_circles, stage_polygons). A staged candidate is read
-// through the same edge view as a body read from global memory (LoadedEdges over its staged vertices: the same
-// expressions for edge flags and normals), so that nearest mode equals pair mode bit for bit. No atomics.
+// through shared memory by SceneWalk (lcp_raycast.cuh). A staged candidate is read through the same edge view as a
+// body read from global memory (LoadedEdges over its staged vertices: the same expressions for edge flags and
+// normals), so that both modes run the same source expressions. No atomics.
 #pragma once
 #include "lcp_sdf.cuh"
 
@@ -148,17 +148,9 @@ __device__ __forceinline__ Side<T, LoadedEdges<T>> load_body(const cts::Bodies<T
 
 template <typename T>
 __global__ void __launch_bounds__(NT) distance_kernel(DistArgs<T> a, int chunks) {
-  __shared__ T s_cx[TC], s_cy[TC], s_cr[TC];
-  __shared__ unsigned char s_con[TC];
-  __shared__ T s_pv[2 * TV];
-  __shared__ T s_pn[2 * TV];
-  __shared__ unsigned char s_eok[TV];
-  __shared__ signed char s_po[TP];
-  const int tid = threadIdx.x, nth = blockDim.x;
+  const SceneWalk<T> walk(a.bd);
   const cts::Bodies<T>& bd = a.bd;
-  const int nb = bd.nb, npo = bd.np + bd.no, nv = bd.nv;
-  const int nt = nb + npo, words = (nt + 31) >> 5;
-  const int ptile = poly_tile(npo, nv);
+  const int tid = walk.tid, nth = walk.nth, nv = walk.nv, nt = walk.nt;
   const bool nearest = a.body_b == nullptr;
   const T maxd = a.max_dist;
   const long long items = (long long)a.B * chunks;
@@ -168,7 +160,7 @@ __global__ void __launch_bounds__(NT) distance_kernel(DistArgs<T> a, int chunks)
     const bool live = r < a.K;
     const size_t ri = (size_t)sc * a.K + (live ? r : 0);
     const size_t qi = a.shared_queries ? (size_t)(live ? r : 0) : ri;
-    const uint32_t* aw = a.active ? a.active + (size_t)sc * words : nullptr;
+    const uint32_t* aw = a.active ? a.active + (size_t)sc * walk.words : nullptr;
     auto on = [&](int b) { return b >= 0 && b < nt && (!aw || ((__ldg(aw + (b >> 5)) >> (b & 31)) & 1u)); };
     const int ia = live ? a.body_a[qi] : -1;
     const int ib = live && !nearest ? a.body_b[qi] : -1;
@@ -190,39 +182,19 @@ __global__ void __launch_bounds__(NT) distance_kernel(DistArgs<T> a, int chunks)
         const long long bit = (long long)(ia < j ? ia : j) * nt + (ia < j ? j : ia);
         return ((__ldg(nc + (bit >> 5)) >> (bit & 31)) & 1u) != 0u;
       };
-      // ---- circles
-      for (int c0 = 0; c0 < nb; c0 += TC) {
-        const int n = nb - c0 < TC ? nb - c0 : TC;
-        __syncthreads();                                 // the previous tile (or work item) is done with the smem
-        stage_circles(bd, nb, sc, c0, n, aw, s_cx, s_cy, s_cr, s_con, tid, nth);
-        __syncthreads();
-        if (valid) {
-          for (int k = 0; k < n; ++k) {
-            const int j = c0 + k;
-            if (!s_con[k] || j == ia || excluded(j)) continue;
-            const Side<T, LoadedEdges<T>> C{true, s_cx[k], s_cy[k], s_cr[k], LoadedEdges<T>{nullptr, T(0), nv}, T(0)};
-            const Pair<T> p = pair_distance(A, C, nv);
-            if (bbody < 0 ? p.d <= best : p.d < best) { best = p.d; bbody = j; bp = p; }
-          }
-        }
-      }
-      // ---- polygons, then obstacles (polygon q is body nb + q)
-      for (int q0 = 0; q0 < npo; q0 += ptile) {
-        const int n = npo - q0 < ptile ? npo - q0 : ptile;
-        __syncthreads();
-        stage_polygons(bd, nb, nv, sc, q0, n, aw, s_pv, s_pn, s_eok, s_po, tid, nth);
-        __syncthreads();
-        if (valid) {
-          for (int q = 0; q < n; ++q) {
-            const int j = nb + q0 + q;
-            if (!s_po[q] || j == ia || excluded(j)) continue;
-            const Side<T, LoadedEdges<T>> C{false, T(0), T(0), T(0),
-                                            LoadedEdges<T>{&s_pv[2 * q * nv], T(s_po[q]), nv}, T(s_po[q])};
-            const Pair<T> p = pair_distance(A, C, nv);
-            if (bbody < 0 ? p.d <= best : p.d < best) { best = p.d; bbody = j; bp = p; }
-          }
-        }
-      }
+      auto visit = [&](int j, const Side<T, LoadedEdges<T>>& C) {
+        const Pair<T> p = pair_distance(A, C, nv);
+        if (bbody < 0 ? p.d <= best : p.d < best) { best = p.d; bbody = j; bp = p; }
+      };
+      walk(sc, aw, valid,
+        [&](int j, T cx, T cy, T cr) {
+          if (j == ia || excluded(j)) return;
+          visit(j, Side<T, LoadedEdges<T>>{true, cx, cy, cr, LoadedEdges<T>{nullptr, T(0), nv}, T(0)});
+        },
+        [&](int j, const T* P, const T*, const unsigned char*, int o) {
+          if (j == ia || excluded(j)) return;
+          visit(j, Side<T, LoadedEdges<T>>{false, T(0), T(0), T(0), LoadedEdges<T>{P, T(o), nv}, T(o)});
+        });
     }
     if (live) {
       const bool hit = bbody >= 0;

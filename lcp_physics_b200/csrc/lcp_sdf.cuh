@@ -17,16 +17,15 @@
 // over overlapping bodies it is the min of their distances, exact outside every body and a bound inside.
 //
 // Layout: one CTA per (scene, chunk of blockDim.x points) work item, one point per thread, the best (sdf, body, feat,
-// normal) in registers; the bodies are staged through shared memory in the tiles of raycast_kernel (stage_circles,
-// stage_polygons). Every thread visits the bodies in index order, so the result depends neither on the chunking nor on
-// the tile sizes. No atomics.
+// normal) in registers; the bodies are staged through shared memory by SceneWalk (lcp_raycast.cuh). Every thread
+// visits the bodies in index order, so the result depends neither on the chunking nor on the tile sizes. No atomics.
 #pragma once
 #include "lcp_raycast.cuh"
 
 namespace lcpb200 {
 namespace ray {
 
-// The edges of a polygon staged by stage_polygons: vertex e at P[2 e], edge flag ok[e] (edge_ok), outward unit normal
+// The edges of a polygon staged by SceneWalk: vertex e at P[2 e], edge flag ok[e] (edge_ok), outward unit normal
 // N[2 e].
 template <typename T>
 struct StagedEdges {
@@ -39,7 +38,7 @@ struct StagedEdges {
 };
 
 // The edges of a polygon whose normals were not staged (vertices P, orientation o from poly_orient): the flag and the
-// normal computed with the expressions of stage_polygons.
+// normal computed with the expressions of SceneWalk.
 template <typename T>
 struct LoadedEdges {
   const T* P;
@@ -88,17 +87,8 @@ __device__ __forceinline__ void point_polygon(const G& g, int nv, T px, T py, T&
 
 template <typename T>
 __global__ void __launch_bounds__(NT) sdf_kernel(SdfArgs<T> a, int chunks) {
-  __shared__ T s_cx[TC], s_cy[TC], s_cr[TC];
-  __shared__ unsigned char s_con[TC];
-  __shared__ T s_pv[2 * TV];
-  __shared__ T s_pn[2 * TV];
-  __shared__ unsigned char s_eok[TV];
-  __shared__ signed char s_po[TP];
-  const int tid = threadIdx.x, nth = blockDim.x;
-  const cts::Bodies<T>& bd = a.bd;
-  const int nb = bd.nb, npo = bd.np + bd.no, nv = bd.nv;
-  const int nt = nb + npo, words = (nt + 31) >> 5;
-  const int ptile = poly_tile(npo, nv);
+  const SceneWalk<T> walk(a.bd);
+  const int tid = walk.tid, nth = walk.nth, nv = walk.nv;
   const T maxd = a.max_dist;
   const long long items = (long long)a.B * chunks;
   for (long long it = blockIdx.x; it < items; it += gridDim.x) {
@@ -110,55 +100,33 @@ __global__ void __launch_bounds__(NT) sdf_kernel(SdfArgs<T> a, int chunks) {
     T px = T(0), py = T(0);
     if (live) { px = a.points[2 * pi]; py = a.points[2 * pi + 1]; }
     const bool valid = live && isfinite(px) && isfinite(py);
-    const uint32_t* aw = a.active ? a.active + (size_t)sc * words : nullptr;
+    const uint32_t* aw = a.active ? a.active + (size_t)sc * walk.words : nullptr;
     // the best body's normal is (bnx, bny) / blen: blen = |x - q| outside, 1 inside a polygon, 0 at a circle's centre
     T best = maxd, bnx = T(0), bny = T(0), blen = T(0);
     int bbody = -1, bfeat = -1;
-    // ---- circles
-    for (int c0 = 0; c0 < nb; c0 += TC) {
-      const int n = nb - c0 < TC ? nb - c0 : TC;
-      __syncthreads();                                   // the previous tile (or work item) is done with the smem
-      stage_circles(bd, nb, sc, c0, n, aw, s_cx, s_cy, s_cr, s_con, tid, nth);
-      __syncthreads();
-      if (valid) {
-        for (int k = 0; k < n; ++k) {
-          if (!s_con[k]) continue;
-          const T dx = px - s_cx[k], dy = py - s_cy[k];
-          const T d = sqrt(dx * dx + dy * dy);
-          const T s = d - s_cr[k];
-          if (bbody < 0 ? s <= best : s < best) {
-            best = s; bbody = c0 + k; bfeat = -1;
-            bnx = dx; bny = dy; blen = d;
-          }
+    walk(sc, aw, valid,
+      [&](int j, T cx, T cy, T cr) {
+        const T dx = px - cx, dy = py - cy;
+        const T d = sqrt(dx * dx + dy * dy);
+        const T s = d - cr;
+        if (bbody < 0 ? s <= best : s < best) {
+          best = s; bbody = j; bfeat = -1;
+          bnx = dx; bny = dy; blen = d;
         }
-      }
-    }
-    // ---- polygons, then obstacles (polygon q is body nb + q)
-    for (int q0 = 0; q0 < npo; q0 += ptile) {
-      const int n = npo - q0 < ptile ? npo - q0 : ptile;
-      __syncthreads();
-      stage_polygons(bd, nb, nv, sc, q0, n, aw, s_pv, s_pn, s_eok, s_po, tid, nth);
-      __syncthreads();
-      if (valid) {
-        for (int q = 0; q < n; ++q) {
-          if (!s_po[q]) continue;
-          const T* P = &s_pv[2 * q * nv];
-          const T* N = &s_pn[2 * q * nv];
-          const unsigned char* ok = &s_eok[q * nv];
-          T smax, dmin, qdx, qdy;
-          int emax, emin;
-          point_polygon(StagedEdges<T>{P, N, ok}, nv, px, py, smax, emax, dmin, emin, qdx, qdy);
-          if (emax < 0) continue;                        // no edge of non-zero length
-          const bool inside = smax <= T(0);
-          const T s = inside ? smax : sqrt(dmin);
-          if (bbody < 0 ? s <= best : s < best) {
-            best = s; bbody = nb + q0 + q;
-            if (inside) { bfeat = 256 + emax; bnx = N[2 * emax]; bny = N[2 * emax + 1]; blen = T(1); }
-            else { bfeat = emin; bnx = qdx; bny = qdy; blen = s; }
-          }
+      },
+      [&](int j, const T* P, const T* N, const unsigned char* ok, int) {
+        T smax, dmin, qdx, qdy;
+        int emax, emin;
+        point_polygon(StagedEdges<T>{P, N, ok}, nv, px, py, smax, emax, dmin, emin, qdx, qdy);
+        if (emax < 0) return;                            // no edge of non-zero length
+        const bool inside = smax <= T(0);
+        const T s = inside ? smax : sqrt(dmin);
+        if (bbody < 0 ? s <= best : s < best) {
+          best = s; bbody = j;
+          if (inside) { bfeat = 256 + emax; bnx = N[2 * emax]; bny = N[2 * emax + 1]; blen = T(1); }
+          else { bfeat = emin; bnx = qdx; bny = qdy; blen = s; }
         }
-      }
-    }
+      });
     if (live) {
       a.sdf[ri] = best;
       a.body[ri] = bbody;

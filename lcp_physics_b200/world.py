@@ -141,6 +141,23 @@ def _edge_normal(E, orient, ln):
     return torch.stack([orient * E[..., 1] / ln, -orient * E[..., 0] / ln], -1)
 
 
+def _take2(t, idx):
+    """Rows idx [B, n] of t [B, m, 2]: [B, n, 2]."""
+    return torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
+
+
+def _polygons(pverts, ov):
+    """The polygon bodies [B, P, V, 2] of a world, dynamic polygons then obstacles, from pverts (polygon_vertices())
+    and ov (the obstacle vertices); either may be None, not both."""
+    return torch.cat([t for t in (pverts, ov) if t is not None], 1)
+
+
+def _detached(t):
+    """t detached and contiguous, None for None: a kernel argument that stays alive until the call returns (a
+    temporary's memory could be reused before the kernel runs)."""
+    return t.detach().contiguous() if t is not None else None
+
+
 def _chosen_edge(polys, body, edge, nb):
     """Edge `edge` of body `body` ([B, n] each) of a world whose polygons polys [B, P, V, 2] are bodies nb, nb + 1,
     ...: (v_e, v_f = the next vertex, E = v_f - v_e, the polygon's orientation sign [B, n]). Slots whose body is not a
@@ -149,9 +166,8 @@ def _chosen_edge(polys, body, edge, nb):
     is_p = body >= nb
     k = torch.where(is_p, body - nb, 0)
     e = torch.where(is_p, edge, 0)
-    take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
     flat = polys.reshape(B, -1, 2)
-    ve, vf = take2(flat, k * V + e), take2(flat, k * V + (e + 1) % V)
+    ve, vf = _take2(flat, k * V + e), _take2(flat, k * V + (e + 1) % V)
     return ve, vf, vf - ve, torch.gather(_orientation(polys), 1, k)
 
 
@@ -666,7 +682,6 @@ class BatchedWorld:
         # others keep the circle walk
         with_feat = self.np > 0 or self.nc_mask is not None or self.per_scene
         masks = (self.nc_mask, self.active_words) if self.per_scene else (self.nc_mask,)
-        d = lambda t: t.detach().contiguous() if t is not None else None
 
         def walk(*ins):
             i32 = lambda *s_: torch.empty(*s_, dtype=torch.int32, device=dev)
@@ -687,11 +702,9 @@ class BatchedWorld:
                         _lib.ptr(ins[-1]), _lib.stream_ptr(dev)))
             # tensors only: _DetectFn marks every output non-differentiable
             return tuple(t for t in (b1, b2, counts, feat, *geo) if t is not None)
-        # contiguous copies, arguments of the call until it returns (a temporary's memory could be reused before the
-        # kernel runs)
         pcen = self.p[:, nb:, 1:] if self.np else None
-        ins = [d(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen) + poly[1:]
-               + obst]
+        ins = [_detached(t) for t in (self.p[:, :nb, 1:], self.rad, self.fric_coeff, self.restitution, pverts, pcen)
+               + poly[1:] + obst]
         out = _detect(walk, *ins, *masks)
         b1, b2, counts = out[:3]
         feat = out[3] if with_feat else None
@@ -730,8 +743,7 @@ class BatchedWorld:
         kr, ki = torch.where(ref2, k2, k1), torch.where(ref2, k1, k2)
         poly = lambda k: torch.gather(verts, 1, k.unsqueeze(2).unsqueeze(3).expand(-1, -1, V, 2))   # [B,C,V,2]
         Vr, Vi = poly(kr), poly(ki)
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
-        cr, ci = take2(ref, kr), take2(ref, ki)
+        cr, ci = _take2(ref, kr), _take2(ref, ki)
         vtx = lambda Vx, e: torch.gather(Vx, 2, e.unsqueeze(2).unsqueeze(3).expand(-1, -1, 1, 2)).squeeze(2)
         E = vtx(Vr, (re + 1) % V) - vtx(Vr, re)
         ln = E.norm(dim=2)
@@ -791,7 +803,6 @@ class BatchedWorld:
         pos = self.p[:, :, 1:]
         i1, i2 = b1.long(), b2.long()
         take = lambda t, idx: torch.gather(t, 1, idx)
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         if self.np:                                  # polygon k of body nb + k: [dynamic polygons..., obstacles...]
             cat = lambda a, b: torch.cat([a, b], 1) if self.no else a
             polys, pref = cat(pverts, self.ov if self.no else None), cat(pos[:, nb:], self.oref if self.no else None)
@@ -812,13 +823,13 @@ class BatchedWorld:
         cc = i2 < nb
         j = torch.where(cc, i2, 0)
         k = torch.where(cc, 0, i2 - nb)
-        c = take2(pos, i1)
+        c = _take2(pos, i1)
         r1 = take(self.rad, i1)
         one = torch.zeros_like(c)
         one[..., 0] = 1.0
         # circle-circle (slots of obstacle pairs and the padding pair (0, 0) of a one-body world get a harmless unit
         # offset: no 0 / 0 in either pass)
-        dcc = torch.where((cc & (i1 != j)).unsqueeze(2), c - take2(pos, j), one)
+        dcc = torch.where((cc & (i1 != j)).unsqueeze(2), c - _take2(pos, j), one)
         dist = dcc.norm(dim=2)
         r2 = take(self.rad, j)
         pen_cc = r1 + r2 - dist
@@ -837,7 +848,7 @@ class BatchedWorld:
         pen_co = torch.where(inside, r1 - sep, r1 - dq_n)
         q_co = torch.where(inside.unsqueeze(2), c - n_in * sep.unsqueeze(2), q)   # best_pt2 = center - n (dist + rad)
         p1_co = q_co - c
-        p2_co = q_co - take2(pref, k)
+        p2_co = q_co - _take2(pref, k)
         w = cc.unsqueeze(2)
         normal = torch.where(w, n_cc, n_co)
         p1 = torch.where(w, p1_cc, p1_co)
@@ -912,31 +923,44 @@ class BatchedWorld:
                              % (name, self.B, tuple(x.shape)))
         return x
 
-    def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts):
-        """One call of the ray or point kernel `entry` (lcpb200_raycast or lcpb200_signed_distance) over n rays or
-        points per scene at the current state. The entry's arguments between overts and active_words are the tensors
-        `queries`, then the ints `flags`. pverts: polygon_vertices() (worlds with polygons). Returns (value [B, n], body
-        [B, n] int64, feat [B, n] int32, normal [B, n, 2] when with_normal, else None)."""
+    def _geometry_leaves(self):
+        """The tensors the world's geometry is differentiated in (None where the world has none): p, the radii, the
+        polygons' initial vertices and the obstacle vertices."""
+        return self.p, self.rad, self.plocal if self.np else None, self.ov if self.no else None
+
+    def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts, no_contact=None):
+        """One call of the ray, point or body-distance kernel `entry` (lcpb200_raycast, lcpb200_signed_distance or
+        lcpb200_body_distance) over n queries per scene at the current state. The entry's arguments between overts
+        and active_words are the tensors `queries` (None: NULL), then the ints `flags`. no_contact: for
+        lcpb200_body_distance, its arguments after active_words (the mask or None, its stride); that entry also writes
+        point_a. pverts: polygon_vertices() (worlds with polygons). Returns (value [B, n], body [B, n] int64, feat
+        [B, n] int32, normal [B, n, 2] when with_normal, else None, point_a [B, n, 2] with no_contact, else None)."""
         lib = _lib.load()
         B, nb, dev = self.B, self.nb, self.device
-        dc = lambda t: t.detach().contiguous() if t is not None else None
+        with_point = no_contact is not None
 
-        def call(pos, rad, pv, ov, aw, *qs):
-            value = torch.empty(B, n, dtype=self.dtype, device=dev)
+        def call(pos, rad, pv, ov, aw, nc, *qs):
+            new = lambda *s_: torch.empty(B, n, *s_, dtype=self.dtype, device=dev)
+            value = new()
             body = torch.empty(B, n, dtype=torch.int32, device=dev)
             feat = torch.empty(B, n, dtype=torch.int32, device=dev)
-            normal = torch.empty(B, n, 2, dtype=self.dtype, device=dev) if with_normal else None
+            normal = new(2) if with_normal else None
+            point_a = new(2) if with_point else None
             with torch.cuda.device(dev):
                 _lib.check(getattr(lib, entry)(
                     _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, n, max_dist, _lib.ptr(pos),
                     _lib.ptr(rad), _lib.ptr(pv), _lib.ptr(ov), *[_lib.ptr(q) for q in qs], *flags, _lib.ptr(aw),
-                    _lib.ptr(value), _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.stream_ptr(dev)))
+                    *((_lib.ptr(nc), no_contact[1]) if with_point else ()), _lib.ptr(value), _lib.ptr(body),
+                    _lib.ptr(feat), _lib.ptr(normal), *((_lib.ptr(point_a),) if with_point else ()),
+                    _lib.stream_ptr(dev)))
             # tensors only: _DetectFn marks every output non-differentiable
-            return tuple(t for t in (value, body, feat, normal) if t is not None)
-        # contiguous copies, arguments of the call until it returns
-        out = _detect(call, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None),
-                      self.active_words, *[dc(q) for q in queries])
-        return out[0], out[1].long(), out[2], out[3] if with_normal else None
+            return tuple(t for t in (value, body, feat, normal, point_a) if t is not None)
+        nc = no_contact[0] if with_point else None
+        out = _detect(call, _detached(self.p[:, :nb, 1:]), _detached(self.rad), _detached(pverts),
+                      _detached(self.ov if self.no else None), self.active_words, nc, *[_detached(q) for q in queries])
+        rest = iter(out[3:])
+        normal, point_a = next(rest) if with_normal else None, next(rest) if with_point else None
+        return out[0], out[1].long(), out[2], normal, point_a
 
     def raycast(self, origin, direction, max_dist):
         """Casts rays against every scene's bodies at the current state (lcpb200_raycast): origin / direction
@@ -956,10 +980,9 @@ class BatchedWorld:
         nrm = d.norm(dim=2, keepdim=True)
         u = d / torch.where(nrm > 0, nrm, torch.ones_like(nrm))      # a zero direction stays zero: it hits nothing
         pverts = self.polygon_vertices() if self.np else None
-        needs_graph = _needs_graph((o, u, self.p, self.rad, self.plocal if self.np else None,
-                                    self.ov if self.no else None))
-        dist, body, feat, normal = self._query("lcpb200_raycast", (o, u), (), int(o.shape[1]), md, not needs_graph,
-                                                 pverts)
+        needs_graph = _needs_graph((o, u) + self._geometry_leaves())
+        dist, body, feat, normal, _ = self._query("lcpb200_raycast", (o, u), (), int(o.shape[1]), md, not needs_graph,
+                                                    pverts)
         if needs_graph:
             dist, normal = self._ray_torch(o, u, body, feat.long(), md, pverts)
         return dist, body, normal
@@ -970,7 +993,6 @@ class BatchedWorld:
         n_e . u and normal n_e; max_dist (a constant) and a zero normal where nothing is hit."""
         nb = self.nb
         B, R = body.shape
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         zero = torch.zeros_like(o)
         is_c = (body >= 0) & (body < nb)
         is_p = body >= nb
@@ -978,7 +1000,7 @@ class BatchedWorld:
         normal = zero
         if nb:
             ci = torch.where(is_c, body, 0)
-            w = o - take2(self.p[:, :nb, 1:], ci)
+            w = o - _take2(self.p[:, :nb, 1:], ci)
             r = torch.gather(self.rad, 1, ci)
             b = (u * w).sum(2)
             k = (w * w).sum(2) - r * r
@@ -989,7 +1011,7 @@ class BatchedWorld:
             dist = torch.where(is_c, t_c, dist)
             normal = torch.where(is_c.unsqueeze(2), n_c, normal)
         if self.np or self.no:
-            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            polys = _polygons(pverts, self.ov if self.no else None)
             ve, _, E, sg = _chosen_edge(polys, body, feat, nb)
             ln = E.norm(dim=2)
             n = _edge_normal(E, sg, torch.where(is_p, ln, torch.ones_like(ln)))
@@ -1036,10 +1058,9 @@ class BatchedWorld:
         if B * Q > 2 ** 31 - 1:
             raise ValueError("points: B * Q = %d exceeds int32 indexing" % (B * Q))
         pverts = self.polygon_vertices() if self.np else None
-        needs_graph = _needs_graph((x, self.p, self.rad, self.plocal if self.np else None,
-                                    self.ov if self.no else None))
-        sdf, body, feat, normal = self._query("lcpb200_signed_distance", (x,), (int(shared),), Q, md,
-                                              with_normal and not needs_graph, pverts)
+        needs_graph = _needs_graph((x,) + self._geometry_leaves())
+        sdf, body, feat, normal, _ = self._query("lcpb200_signed_distance", (x,), (int(shared),), Q, md,
+                                                 with_normal and not needs_graph, pverts)
         if needs_graph:
             sdf, normal = self._sdf_torch(x, body, feat.long(), md, pverts)
         return sdf, body, normal
@@ -1053,7 +1074,6 @@ class BatchedWorld:
         nb = self.nb
         B, Q = body.shape
         x = points.expand(B, Q, 2) if points.dim() == 2 else points
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
 
         def length(d):
             """|d| and d / |d|, both 0 where d == 0 (no 0 / 0 in either pass)"""
@@ -1068,11 +1088,11 @@ class BatchedWorld:
         normal = torch.zeros_like(x)
         if nb:
             ci = torch.where(is_c, body, 0)
-            ln, n_c = length(x - take2(self.p[:, :nb, 1:], ci))
+            ln, n_c = length(x - _take2(self.p[:, :nb, 1:], ci))
             sdf = torch.where(is_c, ln - torch.gather(self.rad, 1, ci), sdf)
             normal = torch.where(is_c.unsqueeze(2), n_c, normal)
         if self.np or self.no:
-            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            polys = _polygons(pverts, self.ov if self.no else None)
             inside = is_p & (feat >= 256)
             ve, vf, E, sg = _chosen_edge(polys, body, feat % 256, nb)
             ee = torch.where(is_p, (E * E).sum(2), torch.ones_like(E[..., 0]))
@@ -1172,32 +1192,12 @@ class BatchedWorld:
 
     def _body_distance(self, ba, bb, shared, max_dist):
         md = _max_dist(max_dist)
-        lib = _lib.load()
-        B, nb, dev = self.B, self.nb, self.device
-        K = int(ba.shape[-1])
+        B, K = self.B, int(ba.shape[-1])
         pverts = self.polygon_vertices() if self.np else None
-        needs_graph = _needs_graph((self.p, self.rad, self.plocal if self.np else None, self.ov if self.no else None))
-        dc = lambda t: t.detach().contiguous() if t is not None else None
-        nc_stride = self.nc_stride if bb is None else 0
-
-        def call(pos, rad, pv, ov, aw, qa, qb, nc):
-            new = lambda *s_: torch.empty(B, K, *s_, dtype=self.dtype, device=dev)
-            dist, normal, point_a = new(), new(2), new(2)
-            body = torch.empty(B, K, dtype=torch.int32, device=dev)
-            feat = torch.empty(B, K, dtype=torch.int32, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(lib.lcpb200_body_distance(
-                    _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, K, md, _lib.ptr(pos), _lib.ptr(rad),
-                    _lib.ptr(pv), _lib.ptr(ov), _lib.ptr(qa), _lib.ptr(qb), int(shared), _lib.ptr(aw), _lib.ptr(nc),
-                    nc_stride, _lib.ptr(dist), _lib.ptr(body), _lib.ptr(feat), _lib.ptr(normal), _lib.ptr(point_a),
-                    _lib.stream_ptr(dev)))
-            # tensors only: _DetectFn marks every output non-differentiable
-            return dist, body, feat, normal, point_a
-        # contiguous copies, arguments of the call until it returns
-        dist, body, feat, normal, point_a = _detect(
-            call, dc(self.p[:, :nb, 1:]), dc(self.rad), dc(pverts), dc(self.ov if self.no else None), self.active_words,
-            ba.contiguous(), dc(bb), self.nc_mask if bb is None else None)
-        body = body.long()
+        needs_graph = _needs_graph(self._geometry_leaves())
+        no_contact = (self.nc_mask, self.nc_stride) if bb is None else (None, 0)     # nearest mode only
+        dist, body, feat, normal, point_a = self._query("lcpb200_body_distance", (ba, bb), (int(shared),), K, md, True,
+                                                        pverts, no_contact)
         if needs_graph:
             dist, normal, point_a, point_b = self._distance_torch(ba.long().expand(B, K), body, feat.long(), md, pverts)
             return dist, body, normal, point_a, point_b
@@ -1217,18 +1217,17 @@ class BatchedWorld:
         src = torch.where(src_b, bo, ba)
         tgt = torch.where(hit, torch.where(src_b, ba, bo), -1)
         is_c = src < nb
-        take2 = lambda t, idx: torch.gather(t, 1, idx.unsqueeze(2).expand(-1, -1, 2))
         dt = self.dtype
         x = torch.zeros(B, K, 2, dtype=dt, device=self.device)
         r = torch.zeros(B, K, dtype=dt, device=self.device)
         if nb:
             ci = torch.where(is_c, src, 0)
-            x = take2(self.p[:, :nb, 1:], ci)
+            x = _take2(self.p[:, :nb, 1:], ci)
             r = torch.where(is_c, torch.gather(self.rad, 1, ci), r)
         if self.np or self.no:
-            polys = torch.cat([t for t in (pverts, self.ov if self.no else None) if t is not None], 1)   # [B, P, V, 2]
+            polys = _polygons(pverts, self.ov if self.no else None)
             vi = torch.where(is_c | ~hit, 0, (src - nb) * self.nv + ((feat >> 9) & 255))   # a miss's feat is -1
-            x = torch.where(is_c.unsqueeze(2), x, take2(polys.reshape(B, -1, 2), vi))
+            x = torch.where(is_c.unsqueeze(2), x, _take2(polys.reshape(B, -1, 2), vi))
         sdf, m = self._sdf_torch(x, tgt, feat & 511, max_dist, pverts)
         dist = torch.where(hit, sdf - r, sdf)
         normal = torch.where(src_b.unsqueeze(2), m, -m)
