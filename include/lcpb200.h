@@ -88,9 +88,12 @@ size_t lcpb200_workspace_bytes(lcpb200_handle_t h);
 int lcpb200_describe(lcpb200_handle_t h, char* buf, size_t len);
 
 /* Development aid: per-phase SM cycle counters of the solver kernels, summed over CTAs.
- * enable=1 allocates/zeroes them, 0 frees; out (may be NULL) receives 24 values: the 14 dual-form phases below
- * followed by the 10 condensed-kernel phases {structure, block inverses, assembly of K, LU, solve: right-hand
- * side, solve: substitution, solve: back-substitution of the multipliers, residuals, step rules, gradients}:
+ * enable=1 allocates/zeroes them, 0 frees; out (may be NULL) receives 26 values: the 14 dual-form phases below,
+ * the 10 condensed-kernel phases {structure, block inverses, assembly of K, LU, solve: right-hand
+ * side, solve: substitution, solve: back-substitution of the multipliers, residuals, step rules, gradients}
+ * (the banded kernel's in the same slots), then two counts summed over every forward kernel that ran: the KKT
+ * factorisations and the KKT solves (one forward + one backward substitution each) it executed. The dual-form
+ * phases:
  * {prefactor, load T, LU, KKT solves, residuals, step rules,
  *  LU: diagonal blocks (look-ahead warp), LU: panel solves, LU: trailing updates,
  *  LU: diagonal-block inverses, number of diagonal blocks with row interchanges, number of

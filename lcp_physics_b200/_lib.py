@@ -121,13 +121,15 @@ class Handle:
         return buf.value.decode()
 
     def profile(self, enable=True):
-        """Read (then reset or disable) the per-phase cycle counters: dict name -> SM cycles."""
-        out = (ctypes.c_longlong * 24)()
+        """Read (then reset or disable) the per-phase cycle counters: dict name -> SM cycles, then the counts of
+        KKT factorisations and solves the forward kernels executed ("factorisations", "solves")."""
+        out = (ctypes.c_longlong * 26)()
         check(load().lcpb200_profile(self._h, 1 if enable else 0, out))
         return dict(zip(("prefactor", "load_T", "lu", "kkt_solve", "residual", "step", "lu_diag", "lu_panel",
                          "lu_update", "lu_inverse", "lu_slow_blocks", "lu_blocks", "lu_ahead", "lu_wait",
                          "c_structure", "c_block_inverse", "c_assemble", "c_lu", "c_solve_rhs", "c_solve_tri",
-                         "c_solve_post", "c_residual", "c_step", "c_gradients"), list(out)))
+                         "c_solve_post", "c_residual", "c_step", "c_gradients", "factorisations", "solves"),
+                        list(out)))
 
     @property
     def raw(self):

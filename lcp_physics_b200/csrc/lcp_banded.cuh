@@ -149,7 +149,8 @@ struct BJvpArgs {
 };
 
 #ifdef LCP_BAND_DEVICE        // device code: compiled by lcp_band_kernels.cu only
-enum { BPH_STRUCT = 0, BPH_WINV, BPH_ASSEMBLE, BPH_LU, BPH_RHS, BPH_SUBST, BPH_POST, BPH_RESID, BPH_STEP, BPH_GRADS, BPH_COUNT };   // same order as cnd::CPH_* (shared counter buffer)
+enum { BPH_STRUCT = 0, BPH_WINV, BPH_ASSEMBLE, BPH_LU, BPH_RHS, BPH_SUBST, BPH_POST, BPH_RESID, BPH_STEP, BPH_GRADS,
+       BPH_FACTORS, BPH_SOLVES, BPH_COUNT };   // same order as cnd::CPH_* (shared counter buffer)
 
 struct BProf {
   long long* dst;
@@ -157,6 +158,9 @@ struct BProf {
   __device__ __forceinline__ void start(long long* d) { dst = d; if (dst) t0 = clock64(); }
   __device__ __forceinline__ void lap(int ph) {
     if (dst && threadIdx.x == 0) { const long long t = clock64(); atomicAdd((unsigned long long*)&dst[ph], (unsigned long long)(t - t0)); t0 = t; }
+  }
+  __device__ __forceinline__ void count(int ph, int k = 1) {
+    if (dst && threadIdx.x == 0) atomicAdd((unsigned long long*)&dst[ph], (unsigned long long)k);
   }
 };
 
@@ -1251,6 +1255,8 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
   __syncthreads();
   factor_kkt(c, pf, mode, mu, false);
   solve_kkt(c, pf, c.rx, c.rs, c.rz, e > 0 ? c.ry : nullptr, c.x, c.s, c.z, c.y);
+  pf.count(BPH_FACTORS);
+  pf.count(BPH_SOLVES);
   if (m == 0) {                                                             // no contacts: engines.py:35-49
     for (int i = tid; i < n; i += NT) o_x[i] = c.x[i];
     for (int i = tid; i < e; i += NT) o_y[i] = c.y[i];
@@ -1347,6 +1353,7 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
     if (not_improved == a.not_improved_lim) { status = 1; ++it; break; }
     if (best < a.eps) { status = 2; ++it; break; }
     if (mu_ > 1e100) { status = 3; ++it; break; }
+    if (it + 1 == a.max_iter) { ++it; break; }                              // the step would never be read
     for (int r = 0; r < cs; ++r)
       for (int k = tid; k < nc; k += NT) { const int i = r * ncap + k; c.d[i] = c.z[i] / c.s[i]; }     // :98
     __syncthreads();
@@ -1382,6 +1389,8 @@ __device__ __forceinline__ void forward_scene(const BArgs& a, Ctx& c, BProf& pf,
     for (int i = tid; i < e; i += NT) c.y[i] += alpha * c.dy[i];
     __syncthreads();
     pf.lap(BPH_STEP);
+    pf.count(BPH_FACTORS);
+    pf.count(BPH_SOLVES, 2);
   }
   if (tid == 0) { a.status[sc] = status; a.iters[sc] = it; if (a.resid) a.resid[sc] = best; }
 }

@@ -142,8 +142,10 @@ struct Struct {
 // optional per-phase SM cycle counters (thread 0 of every CTA; lcpb200_profile). A compile-time switch: the
 // kernels are instantiated twice, and the production instantiation carries no profiling state (a pointer and a
 // timestamp live across every phase cost registers the LU and the solves need).
+// The last two slots are counts, not cycles: the factorisations and the solves (forward + backward substitution)
+// the forward kernel executed.
 enum { CPH_STRUCT = 0, CPH_WINV, CPH_ASSEMBLE, CPH_LU, CPH_SOLVE_RHS, CPH_SOLVE_TRI, CPH_SOLVE_POST, CPH_RESID,
-       CPH_STEP, CPH_GRADS, CPH_COUNT };
+       CPH_STEP, CPH_GRADS, CPH_FACTORS, CPH_SOLVES, CPH_COUNT };
 template <bool ON>
 struct Prof {
   long long* p;               // this CTA's CPH_COUNT counters
@@ -157,12 +159,16 @@ struct Prof {
       t = n;
     }
   }
+  __device__ __forceinline__ void count(int ph, int k = 1) {
+    if (threadIdx.x == 0) atomicAdd(reinterpret_cast<unsigned long long*>(p + ph), (unsigned long long)k);
+  }
 };
 template <>
 struct Prof<false> {
   __device__ __forceinline__ explicit Prof(long long*) {}
   __device__ __forceinline__ void start() {}
   __device__ __forceinline__ void lap(int) {}
+  __device__ __forceinline__ void count(int, int = 1) {}
 };
 
 // ------------------------------------------------------------------ structure detection
@@ -1297,6 +1303,8 @@ __device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S,
   }
   factor_kkt<T, NS, CS>(P, S, st, pf);
   solve_kkt<T, CS, NS>(P, S, st, pf, S.rx(), S.rs2(), S.rz(), P.e > 0 ? S.ry() : nullptr, S.x(), S.s(), S.z(), S.y());
+  pf.count(CPH_FACTORS);
+  pf.count(CPH_SOLVES);
   if (m == 0) {
     // engine path, a scene without contacts: no complementarity, the equality-constrained solve above is the
     // answer (engines.py:35-49 solves [[M, -Je^T], [Je, 0]] x = [M v + dt f; 0] directly in that case)
@@ -1337,6 +1345,9 @@ __device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S,
     if (not_improved == a.not_improved_lim) { status = 1; ++it; break; }
     if (best < a.eps) { status = 2; ++it; break; }
     if (mu > T(1e100)) { status = 3; ++it; break; }
+    // the step below would make an iterate no residual is formed for: it can never become `best`, so the last
+    // iteration ends here (status 0, iters == max_iter, as if it had run)
+    if (it + 1 == a.max_iter) { ++it; break; }
 
     for (int i = threadIdx.x; i < m; i += NT) S.d()[i] = S.z()[i] / S.s()[i];     // :98
     __syncthreads();
@@ -1351,6 +1362,8 @@ __device__ __forceinline__ void forward_scene(const CFwdArgs<T>& a, CSmem<T>& S,
     // NOTE: ds_c -> S.rz(), dz_c -> S.rs2() (solve_kkt reads rs before it writes dz/ds of the same row)
     fwd_step<T>(P, S, m);
     pf.lap(CPH_STEP);
+    pf.count(CPH_FACTORS);
+    pf.count(CPH_SOLVES, 2);
   }
   if (threadIdx.x == 0) { a.status[sc] = status; a.iters[sc] = it; if (a.resid) a.resid[sc] = best; }
 }

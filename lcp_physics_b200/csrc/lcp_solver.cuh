@@ -30,9 +30,10 @@ struct Plan {
   long long w_Qi, w_R, w_T, w_U12, w_X, w_XA, w_S11, w_V, w_W, w_Fell, w_Gell;
 };
 
-// phases for the optional cycle counters
+// phases for the optional cycle counters; the last two are counts of the factorisations and the solves
+// (forward + backward substitution) the forward kernel executed
 enum { PH_PREFACTOR = 0, PH_LOADT, PH_LU, PH_SOLVE, PH_RESID, PH_STEP, PH_LU_DIAG, PH_LU_PANEL, PH_LU_UPDATE,
-       PH_LU_DIAGWAIT, PH_LU_SLOWDIAG, PH_LU_BLOCKS, PH_LU_AHEAD, PH_LU_WAIT, PH_COUNT };
+       PH_LU_DIAGWAIT, PH_LU_SLOWDIAG, PH_LU_BLOCKS, PH_LU_AHEAD, PH_LU_WAIT, PH_FACTORS, PH_SOLVES, PH_COUNT };
 
 template <typename T>
 struct Vecs {
@@ -109,6 +110,10 @@ __device__ __forceinline__ void prof_start(C& c) { if (c.prof && threadIdx.x == 
 template <typename C>
 __device__ __forceinline__ void prof_lap(C& c, int ph) {
   if (c.prof && threadIdx.x == 0) { const long long t = clock64(); c.prof[ph] += t - c.t_last; c.t_last = t; }
+}
+template <typename C>
+__device__ __forceinline__ void prof_count(C& c, int ph, int k = 1) {
+  if (c.prof && threadIdx.x == 0) c.prof[ph] += k;
 }
 
 // ------------------------------------------------------------------ vector GEMVs
@@ -842,6 +847,8 @@ __global__ void __launch_bounds__(512, 1) lcp_forward_kernel(const FwdArgs<T> a)
     __syncthreads();
     factor_kkt(c);
     solve_kkt(c, off(v.rx), off(v.rs2), off(v.rz), e > 0 ? off(v.ry) : -1, off(v.x), off(v.s), off(v.z), off(v.y));
+    prof_count(c, PH_FACTORS);
+    prof_count(c, PH_SOLVES);
     {   // shift s and z to >= 1 where the row minimum is <= 0       :65-75
       T mn[2] = {INFINITY, INFINITY};
       for (int i = tid; i < m; i += NT) { mn[0] = nan_min(mn[0], v.s[i]); mn[1] = nan_min(mn[1], v.z[i]); }
@@ -907,7 +914,8 @@ __global__ void __launch_bounds__(512, 1) lcp_forward_kernel(const FwdArgs<T> a)
       const T mu = fabs(sz / T(m));                               // :91
       const T resid = (e > 0 ? sqrt(v.bcast[2]) : T(0)) + sqrt(v.bcast[1]) + sqrt(v.bcast[3]) + T(m) * mu;   // :92-96
       prof_lap(c, PH_RESID);
-      factor_kkt(c, overlap);                                // :100
+      const bool last = it + 1 == a.max_iter;    // no step follows: its direction would make an unread iterate
+      if (!last) { factor_kkt(c, overlap); prof_count(c, PH_FACTORS); }     // :100
 
       // ---- best iterate / termination (per scene)                 :107-136
       bool improved;
@@ -922,6 +930,7 @@ __global__ void __launch_bounds__(512, 1) lcp_forward_kernel(const FwdArgs<T> a)
       if (not_improved == a.not_improved_lim) { status = 1; ++it; break; }
       if (best < a.eps) { status = 2; ++it; break; }
       if (mu > T(1e100)) { status = 3; ++it; break; }
+      if (last) { ++it; break; }
 
       // ---- affine direction                                       :138-139   (rs = z)
       solve_kkt(c, off(v.rx), off(v.z), off(v.rz), e > 0 ? off(v.ry) : -1, off(v.dxa), off(v.dsa), off(v.dza), off(v.dya));
@@ -939,7 +948,10 @@ __global__ void __launch_bounds__(512, 1) lcp_forward_kernel(const FwdArgs<T> a)
       __syncthreads();
       prof_lap(c, PH_STEP);
       solve_kkt(c, -1, off(v.rs2), -1, -1, off(v.dxc), off(v.dsc), off(v.dzc), off(v.dyc));
-      if (it + 1 < a.max_iter && P.prefetch) prefetch_T(c);                     // the factors are dead from here on
+      // the factors are dead from here on. R goes to T for the last iteration too, although that one factors
+      // nothing: the prefetch is what splits its residuals over a team (above), and the same split keeps the
+      // last residual, and so `best`, bit for bit what a factoring iteration would compute
+      if (it + 1 < a.max_iter && P.prefetch) prefetch_T(c);
       prof_lap(c, PH_SOLVE);
       for (int i = tid; i < n; i += NT) v.dxa[i] += v.dxc[i];    // :160-163
       for (int i = tid; i < m; i += NT) { v.dsa[i] += v.dsc[i]; v.dza[i] += v.dzc[i]; }
@@ -952,8 +964,10 @@ __global__ void __launch_bounds__(512, 1) lcp_forward_kernel(const FwdArgs<T> a)
       for (int i = tid; i < e; i += NT) v.y[i] += alpha * v.dya[i];
       __syncthreads();
       prof_lap(c, PH_STEP);
+      prof_count(c, PH_SOLVES, 2);
     }
-    if (c.t_prefetched) { cp_async_wait_all(); c.t_prefetched = false; }   // early exit: drain before T's region is reused
+    // early exit or the last iteration (R prefetched, never factored): drain before T's region is reused
+    if (c.t_prefetched) { cp_async_wait_all(); c.t_prefetched = false; }
     if (tid == 0) { a.status[sc] = status; a.iters[sc] = it; if (a.resid) a.resid[sc] = best; }
     __syncthreads();
   }

@@ -601,24 +601,35 @@ extern "C" int lcpb200_jvp_batched(lcpb200_handle_t h, int R, int B, const void*
 
 extern "C" int lcpb200_profile(lcpb200_handle_t h, int enable, long long* out) {
   // Development aid: per-phase SM cycle counters (thread 0 of every CTA), summed over CTAs.
-  // enable = 1 allocates + zeroes the counters, 0 frees them; `out` receives 24 values: the 14
-  // dual-form phases (see the header) followed by the 10 condensed-kernel phases.
+  // enable = 1 allocates + zeroes the counters, 0 frees them; `out` receives 26 values: the 14
+  // dual-form phases (see the header), the 10 condensed-kernel phases, then the factorisations and
+  // the solves the forward kernels executed (every family's count summed into the same two slots).
   if (!h) return fail("null handle");
   DeviceGuard dg_;
   CK(dg_.set(h->device));
+  static_assert(PH_SOLVES == PH_FACTORS + 1 && PH_COUNT == PH_SOLVES + 1, "counts are the dual form's last slots");
+  static_assert(cnd::CPH_SOLVES == cnd::CPH_FACTORS + 1 && cnd::CPH_COUNT == cnd::CPH_SOLVES + 1,
+                "counts are the condensed kernels' last slots");
+  const int ocnt = PH_FACTORS + cnd::CPH_FACTORS;       // first count slot of `out`
   const size_t cnt = (size_t)lcpb200_handle_s::NSLOT * h->max_grid * PH_COUNT;
   const size_t ccnt = (size_t)lcpb200_handle_s::NSLOT * std::max(h->cond_grid, h->num_sms) * cnd::CPH_COUNT;
   if (out) {
-    for (int i = 0; i < PH_COUNT + cnd::CPH_COUNT; ++i) out[i] = 0;
+    for (int i = 0; i < ocnt + 2; ++i) out[i] = 0;
     if (h->prof) {
       std::vector<long long> tmp(cnt);
       CK(cudaMemcpy(tmp.data(), h->prof, cnt * sizeof(long long), cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < cnt; ++i) out[i % PH_COUNT] += tmp[i];
+      for (size_t i = 0; i < cnt; ++i) {
+        const int ph = (int)(i % PH_COUNT);
+        out[ph < PH_FACTORS ? ph : ocnt + ph - PH_FACTORS] += tmp[i];
+      }
     }
     if (h->cprof) {
       std::vector<long long> tmp(ccnt);
       CK(cudaMemcpy(tmp.data(), h->cprof, ccnt * sizeof(long long), cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < ccnt; ++i) out[PH_COUNT + i % cnd::CPH_COUNT] += tmp[i];
+      for (size_t i = 0; i < ccnt; ++i) {
+        const int ph = (int)(i % cnd::CPH_COUNT);
+        out[ph < cnd::CPH_FACTORS ? PH_FACTORS + ph : ocnt + ph - cnd::CPH_FACTORS] += tmp[i];
+      }
     }
   }
   if (enable && !h->prof) CK(cudaMalloc(&h->prof, cnt * sizeof(long long)));

@@ -68,6 +68,7 @@ if __name__ == "__main__":
     for k, v in pr.items():
         if k.startswith("c_") and v:
             print("   %-18s %5.1f %%  %9.0f" % (k, 100.0 * v / tot, v / B))
+    print("executed per scene: %.2f factorisations, %.2f solves" % (pr["factorisations"] / B, pr["solves"] / B))
     for Bs in (132, 264):
         sub = [t[:Bs].contiguous() for t in inp]
         solve_forward(*sub, max_iter=10)
@@ -77,7 +78,8 @@ if __name__ == "__main__":
         torch.cuda.synchronize(); t1 = time.time()
         pr = hd.profile(False)
         print("forward only, B=%d (%.2f ms): cycles per scene:" % (Bs, (t1 - t0) * 1e3),
-              " ".join("%s=%.0f" % (k[2:], v / Bs) for k, v in pr.items() if k.startswith("c_") and v))
+              " ".join("%s=%.0f" % (k[2:], v / Bs) for k, v in pr.items() if k.startswith("c_") and v),
+              "| per scene: %.2f factorisations, %.2f solves" % (pr["factorisations"] / Bs, pr["solves"] / Bs))
     B = 1024
     inp = [t.cuda() for t in make_scenes(B, 16, 32, fd=3, e=0, dtype=torch.float64, seed=7)]
     for rep in range(3):
