@@ -390,6 +390,65 @@ int lcpb200_body_distance(int dtype, int B, int nb, int np, int no, int nv, int 
                           const int32_t* no_contact, long long nc_stride, void* dist, int32_t* body, int32_t* feat,
                           void* normal, void* point_a, void* stream);
 
+/* Shape casts and translational sweeps against the bodies of B scenes (the body groups of lcpb200_contacts), K queries
+ * per scene. Every case reduces to one cast primitive: a ray from a point x along a unit direction s u (s = +-1)
+ * against a target feature inflated by a radius rho >= 0, hitting at the first entry into the Minkowski sum of the
+ * target and a disk of radius rho (the minimum t >= 0 over the target's features):
+ *   circle (c, R)                 the ray against the circle (c, R + rho), lcpb200_raycast's rule: w = x - c,
+ *                                 b = s u . w, k = |w|^2 - (R + rho)^2, a hit iff k >= 0, b < 0 and b^2 - k >= 0, at
+ *                                 t = k / (-b + sqrt(b^2 - k)); normal m = (w + t s u) / (R + rho); feat 0
+ *   polygon face e                every edge of non-zero length (outward unit normal n_e, start vertex v_e, E the
+ *                                 edge): the offset line n_e . (y - v_e) = rho, a hit iff den = n_e . s u < 0,
+ *                                 t = (n_e . (v_e - x) + rho) / den >= 0 and the hit point projects onto the edge
+ *                                 within [0, 1] (inclusive); m = n_e; feat e
+ *   polygon vertex v (rho > 0)    the circle (v, rho) with the circle rule; m = (x + t s u - v) / rho; feat 256 + v
+ * Within a polygon the faces come first, then the vertices, each in index order, and only a strictly nearer hit
+ * replaces the best. A target the swept shape overlaps at t = 0 is skipped; one it only touches gives t = 0 when the
+ * motion heads into it and no hit otherwise.
+ * Disk mode (body_q == NULL): query k sweeps a disk of radius radius[k] from origin[k] along dir[k] against every
+ * active body: x = origin, s = +1, rho = radius; a polygon is skipped when its signed distance at the origin (the rule
+ * of lcpb200_signed_distance) is < radius. A hit iff t <= max_dist. no_contact and limit are not read.
+ * Body mode (body_q != NULL): query k translates body q = body_q[k] along dir[k] by at most limit[k] against every other
+ * active body of its scene not excluded by no_contact, held still (no rotation):
+ *   circle q, circle j            x = c_q, s = +1, the circle j with rho = R_q
+ *   circle q, polygon j           x = c_q, s = +1, polygon j with rho = R_q (skipped when sdf(c_q, j) < R_q)
+ *   polygon q, circle j           x = c_j, s = -1, polygon q at its current pose with rho = R_j (skipped when
+ *                                 sdf(c_j, q) < R_j): the mover is the target
+ *   polygon q, polygon j          every vertex of q with s = +1 against j, then every vertex of j with s = -1 against
+ *                                 q, rho = 0 (q's vertices first, the first strictly nearest wins); skipped when the
+ *                                 separating-axis value of both polygons, taken both ways, is < 0
+ * Candidates in index order, from best = the limit (max_dist in disk mode), body -1: a body replaces the best iff
+ * body < 0 ? t <= best : t < best. A miss -- nothing hit, a zero or non-finite direction, a non-finite origin or limit,
+ * a negative or non-finite radius, an inactive or out-of-range mover -- reads dist = the limit, body -1, feat -1 and
+ * zero normal and point. Deterministic (no atomics); results do not depend on how the queries are split into CTAs.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb] pverts[B,np,nv,2] overts[B,no,nv,2]   the bodies, as in lcpb200_signed_distance
+ *   origin[B,K,2] radius[B,K]                         disk mode: the disks (NULL in body mode)
+ *   body_q[B,K] int32                                 body mode: the movers; NULL: disk mode
+ *   dir[B,K,2]                                        the unit directions (not normalised here)
+ *   limit[B,K]                                        body mode: the length of each translation (NULL in disk mode)
+ *   active_words[B, ceil(nt / 32)] int32              NULL, or the layout of lcpb200_contacts_active (nt <= 8192)
+ *   no_contact, nc_stride                             NULL, or the pair masks of lcpb200_body_distance; body mode only
+ *   dist[B,K] body[B,K] feat[B,K] int32               OUT: t, the hit body (-1: a miss), and the choices: bits 0-8 the
+ *                                                     target feature, bits 9-16 the source vertex (0 for a circle
+ *                                                     source), bit 17 set iff the source is the hit body (the mover
+ *                                                     is the target); -1 on a miss
+ *   normal[B,K,2]                                     OUT: disk mode, the hit body's outward normal m at the contact;
+ *                                                     body mode, the unit normal from the mover towards the hit body
+ *                                                     (-m, or m when the mover is the target)
+ *   point[B,K,2]                                      OUT: the contact point at the time of impact, x + s t u - R_src m
+ *                                                     plus t u when the mover is the target (R_src: the source
+ *                                                     circle's radius, 0 for a polygon vertex)
+ * The radius is not read on the host: a negative or non-finite one reads a miss. Returns non-zero without launching on
+ * B <= 0, K <= 0, nb + np + no == 0, nv > 256 (or nv < 3 with polygons), max_dist < 0 or non-finite (in the dtype), a
+ * NULL pointer the mode reads (dir, origin and radius or limit, the bodies, every output), nc_stride < 0, active_words
+ * with nt > 8192, or B * K > 2^31 - 1. */
+int lcpb200_shapecast(int dtype, int B, int nb, int np, int no, int nv, int K, double max_dist, const void* pos,
+                      const void* rad, const void* pverts, const void* overts, const void* origin, const void* radius,
+                      const int32_t* body_q, const void* dir, const void* limit, const int32_t* active_words,
+                      const int32_t* no_contact, long long nc_stride, void* dist, int32_t* body, int32_t* feat,
+                      void* normal, void* point, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

@@ -1,5 +1,5 @@
-// lcp_ray_launch.h -- host-side launch interface of the batched ray cast, signed distance and body distance
-// (lcp_ray_kernels.cu, lcp_raycast.cuh, lcp_sdf.cuh, lcp_distance.cuh).
+// lcp_ray_launch.h -- host-side launch interface of the batched ray cast, signed distance, body distance and shape cast
+// (lcp_ray_kernels.cu, lcp_raycast.cuh, lcp_sdf.cuh, lcp_distance.cuh, lcp_shapecast.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -72,6 +72,32 @@ struct DistArgs {
 
 template <typename T>
 cudaError_t launch_distance(const DistArgs<T>& a, int num_sms, cudaStream_t st);
+
+// One batch of shape casts or sweeps of lcpb200_shapecast, bd as in RayArgs. dir [B,K,2] (unit length). Disk mode
+// (body_q == nullptr): origin [B,K,2], radius [B,K] and max_dist are read. Body mode: body_q [B,K] and limit [B,K] are
+// read, and no_contact as in DistArgs. active as in RayArgs. Outputs dist / body / feat [B,K], normal / point [B,K,2].
+template <typename T>
+struct CastArgs {
+  cts::Bodies<T> bd;
+  int B, K;
+  T max_dist;
+  const T* origin;
+  const T* radius;
+  const int32_t* body_q;
+  const T* dir;
+  const T* limit;
+  const uint32_t* active;
+  const uint32_t* no_contact;
+  long long nc_stride;
+  T* dist;
+  int32_t* body;
+  int32_t* feat;
+  T* normal;
+  T* point;
+};
+
+template <typename T>
+cudaError_t launch_shapecast(const CastArgs<T>& a, int num_sms, cudaStream_t st);
 
 }  // namespace ray
 }  // namespace lcpb200

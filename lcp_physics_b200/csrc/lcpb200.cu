@@ -1179,8 +1179,9 @@ extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no,
                         no_contact, active, no_contact_stride, stream);
 }
 
-// ------------------------------------------------------------------ ray casts, signed distances and body distances
-// Argument checks shared by lcpb200_raycast, lcpb200_signed_distance and lcpb200_body_distance. what prefixes the messages; N counts the
+// ------------------------------------------------------------------ ray casts, signed distances, body distances, shape casts
+// Argument checks shared by lcpb200_raycast, lcpb200_signed_distance, lcpb200_body_distance and lcpb200_shapecast. what
+// prefixes the messages; N counts the
 // queries per scene, named n_name and counted as `items` in the messages. queries_set: the entry's own query pointers
 // (origin and dir, or points) are non-NULL, so that one message covers every NULL pointer.
 static int check_query(const char* what, const char* n_name, const char* items, int dtype, int B, int N, int nb,
@@ -1283,6 +1284,38 @@ extern "C" int lcpb200_body_distance(int dtype, int B, int nb, int np, int no, i
     a.active = (const uint32_t*)active_words; a.no_contact = (const uint32_t*)no_contact; a.nc_stride = nc_stride;
     a.dist = (T*)dist; a.body = body; a.feat = feat; a.normal = (T*)normal; a.point_a = (T*)point_a;
     return ray::launch_distance<T>(a, sms, (cudaStream_t)stream);
+  };
+  CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
+  return 0;
+}
+
+// The radius of disk mode lives in device memory, which this entry does not read: the kernel treats a negative or
+// non-finite radius as a miss (BatchedWorld.shapecast rejects one on the host).
+extern "C" int lcpb200_shapecast(int dtype, int B, int nb, int np, int no, int nv, int K, double max_dist,
+                                 const void* pos, const void* rad, const void* pverts, const void* overts,
+                                 const void* origin, const void* radius, const int32_t* body_q, const void* dir,
+                                 const void* limit, const int32_t* active_words, const int32_t* no_contact,
+                                 long long nc_stride, void* dist, int32_t* body, int32_t* feat, void* normal,
+                                 void* point, void* stream) {
+  const bool disk = body_q == nullptr;
+  if (int rc = check_query("shapecast", "K", "queries", dtype, B, K, nb, np, no, nv, max_dist, pos, rad, pverts,
+                           overts, dir && (disk ? origin && radius : limit != nullptr), dist, body, feat,
+                           active_words))
+    return rc;
+  if (!normal || !point) return fail("shapecast: NULL argument");
+  if (nc_stride < 0) return fail("shapecast: need nc_stride >= 0");
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
+  auto launch = [&](auto zero) {      // the body for T = the type of zero
+    using T = decltype(zero);
+    ray::CastArgs<T> a{};
+    a.bd = query_bodies<T>(nb, np, no, nv, pos, rad, pverts, overts);
+    a.B = B; a.K = K; a.max_dist = (T)max_dist;
+    a.origin = (const T*)origin; a.radius = (const T*)radius; a.body_q = body_q; a.dir = (const T*)dir;
+    a.limit = (const T*)limit; a.active = (const uint32_t*)active_words; a.no_contact = (const uint32_t*)no_contact;
+    a.nc_stride = nc_stride;
+    a.dist = (T*)dist; a.body = body; a.feat = feat; a.normal = (T*)normal; a.point = (T*)point;
+    return ray::launch_shapecast<T>(a, sms, (cudaStream_t)stream);
   };
   CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
   return 0;

@@ -929,12 +929,13 @@ class BatchedWorld:
         return self.p, self.rad, self.plocal if self.np else None, self.ov if self.no else None
 
     def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts, no_contact=None):
-        """One call of the ray, point or body-distance kernel `entry` (lcpb200_raycast, lcpb200_signed_distance or
-        lcpb200_body_distance) over n queries per scene at the current state. The entry's arguments between overts
-        and active_words are the tensors `queries` (None: NULL), then the ints `flags`. no_contact: for
-        lcpb200_body_distance, its arguments after active_words (the mask or None, its stride); that entry also writes
-        point_a. pverts: polygon_vertices() (worlds with polygons). Returns (value [B, n], body [B, n] int64, feat
-        [B, n] int32, normal [B, n, 2] when with_normal, else None, point_a [B, n, 2] with no_contact, else None)."""
+        """One call of the ray, point, body-distance or shape-cast kernel `entry` (lcpb200_raycast,
+        lcpb200_signed_distance, lcpb200_body_distance or lcpb200_shapecast) over n queries per scene at the current
+        state. The entry's arguments between overts and active_words are the tensors `queries` (None: NULL), then the
+        ints `flags`. no_contact: for lcpb200_body_distance and lcpb200_shapecast, their arguments after active_words
+        (the mask or None, its stride); those entries also write point_a (shapecast's point). pverts:
+        polygon_vertices() (worlds with polygons). Returns (value [B, n], body [B, n] int64, feat [B, n] int32, normal
+        [B, n, 2] when with_normal, else None, point_a [B, n, 2] with no_contact, else None)."""
         lib = _lib.load()
         B, nb, dev = self.B, self.nb, self.device
         with_point = no_contact is not None
@@ -987,38 +988,53 @@ class BatchedWorld:
             dist, normal = self._ray_torch(o, u, body, feat.long(), md, pverts)
         return dist, body, normal
 
-    def _ray_torch(self, o, u, body, feat, max_dist, pverts):
-        """Torch mirror of csrc/lcp_raycast.cuh, REBUILT FROM THE KERNEL'S CHOICES body / feat [B, R]: the circle's
-        entry t = k / (-b + sqrt(b^2 - k)) and normal (w + t u) / r, or the entering edge's t = n_e . (v_e - o) /
-        n_e . u and normal n_e; max_dist (a constant) and a zero normal where nothing is hit."""
+    def _ray_torch(self, x, u, body, feat, max_dist, pverts, rho=0.0):
+        """Torch mirror of the cast primitive of csrc/lcp_raycast.cuh and csrc/lcp_shapecast.cuh, REBUILT FROM THE
+        KERNEL'S CHOICES body / feat [B, K]: the ray x + t u (x, u [B, K, 2]) against the target inflated by rho ([B, K],
+        or 0.0 for a ray cast). A circle (c, R) and a polygon vertex v (feat 256 + v, a circle (v, 0)): the entry
+        t = k / (-b + sqrt(b^2 - k)) into the circle of radius R + rho and normal (w + t u) / (R + rho); a polygon face
+        e (feat e < 256; raycast's entering edge): t = (n_e . (v_e - x) + rho) / n_e . u and normal n_e; max_dist (a
+        constant) and a zero normal where nothing is hit. With rho = 0.0 the values are raycast's: R + 0.0 and
+        s + 0.0 are exact."""
         nb = self.nb
-        B, R = body.shape
-        zero = torch.zeros_like(o)
+        B, K = body.shape
         is_c = (body >= 0) & (body < nb)
         is_p = body >= nb
-        dist = torch.full((B, R), max_dist, dtype=o.dtype, device=o.device)
-        normal = zero
-        if nb:
-            ci = torch.where(is_c, body, 0)
-            w = o - _take2(self.p[:, :nb, 1:], ci)
-            r = torch.gather(self.rad, 1, ci)
+        is_v = is_p & (feat >= 256)
+        is_f = is_p & ~is_v
+        dist = torch.full((B, K), max_dist, dtype=x.dtype, device=x.device)
+        normal = torch.zeros_like(x)
+        polys = _polygons(pverts, self.ov if self.no else None) if self.np or self.no else None
+        is_d = is_c | is_v                                     # a disk: a circle, or a vertex inflated by rho
+        if nb or polys is not None:
+            c = torch.zeros_like(x)
+            R = torch.zeros_like(dist)
+            if nb:
+                ci = torch.where(is_c, body, 0)
+                c = _take2(self.p[:, :nb, 1:], ci)
+                R = torch.gather(self.rad, 1, ci)
+            if polys is not None:
+                vi = torch.where(is_v, (body - nb) * self.nv + feat - 256, 0)
+                c = torch.where(is_v.unsqueeze(2), _take2(polys.reshape(B, -1, 2), vi), c)
+                R = torch.where(is_v, torch.zeros_like(R), R)
+            rr = R + rho
+            w = x - c
             b = (u * w).sum(2)
-            k = (w * w).sum(2) - r * r
-            disc = torch.where(is_c, b * b - k, torch.ones_like(b))
-            den = torch.where(is_c, -b + disc.sqrt(), torch.ones_like(b))
+            k = (w * w).sum(2) - rr * rr
+            disc = torch.where(is_d, b * b - k, torch.ones_like(b))
+            den = torch.where(is_d, -b + disc.sqrt(), torch.ones_like(b))
             t_c = k / den
-            n_c = (w + t_c.unsqueeze(2) * u) / torch.where(is_c, r, torch.ones_like(r)).unsqueeze(2)
-            dist = torch.where(is_c, t_c, dist)
-            normal = torch.where(is_c.unsqueeze(2), n_c, normal)
-        if self.np or self.no:
-            polys = _polygons(pverts, self.ov if self.no else None)
-            ve, _, E, sg = _chosen_edge(polys, body, feat, nb)
+            n_c = (w + t_c.unsqueeze(2) * u) / torch.where(is_d, rr, torch.ones_like(rr)).unsqueeze(2)
+            dist = torch.where(is_d, t_c, dist)
+            normal = torch.where(is_d.unsqueeze(2), n_c, normal)
+        if polys is not None:
+            ve, _, E, sg = _chosen_edge(polys, body, torch.where(is_v, 0, feat), nb)
             ln = E.norm(dim=2)
-            n = _edge_normal(E, sg, torch.where(is_p, ln, torch.ones_like(ln)))
+            n = _edge_normal(E, sg, torch.where(is_f, ln, torch.ones_like(ln)))
             den = (n * u).sum(2)
-            t_p = (n * (ve - o)).sum(2) / torch.where(is_p, den, -torch.ones_like(den))
-            dist = torch.where(is_p, t_p, dist)
-            normal = torch.where(is_p.unsqueeze(2), n, normal)
+            t_p = ((n * (ve - x)).sum(2) + rho) / torch.where(is_f, den, -torch.ones_like(den))
+            dist = torch.where(is_f, t_p, dist)
+            normal = torch.where(is_f.unsqueeze(2), n, normal)
         return dist, normal
 
     def lidar(self, body, n_rays, max_dist, fov=2 * math.pi, start=0.0):
@@ -1234,6 +1250,115 @@ class BatchedWorld:
         w = torch.where(src_b, sdf, r)
         point_a = torch.where(hit.unsqueeze(2), x - w.unsqueeze(2) * m, torch.zeros_like(x))
         return dist, normal, point_a, point_a + dist.unsqueeze(2) * normal
+
+    # ------------------------------------------------------------------ shape casts and sweeps
+    def shapecast(self, origin, direction, radius, max_dist):
+        """Sweeps disks against every scene's bodies at the current state (lcpb200_shapecast, disk mode): a disk of
+        radius `radius` from `origin` along `direction` ([B, K, 2] or [K, 2] shared by the batch; direction is
+        normalised here). radius: a scalar, [K] or [B, K], finite and >= 0. The disk hits a body where it first touches
+        it within max_dist; a body the disk already overlaps at the origin is not seen (with radius 0 this is
+        `raycast`). Returns (dist [B, K], body [B, K] int64 indexing [circles, polygons, obstacles], -1 for no hit,
+        normal [B, K, 2]: the hit body's outward normal at the contact, point [B, K, 2]: the contact point on its
+        surface, origin + dist u - radius normal); a miss reads max_dist, zeros and zero gradient, as does a zero or
+        non-finite direction. Inactive bodies (`active`) are invisible.
+        The kernel makes every discrete choice (which body, which face or vertex). When a gradient or tangent is
+        needed, the outputs are rebuilt from those choices with torch ops, so that gradients reach the origins, the
+        directions, the radii of the disks, p, the bodies' radii, the polygons' initial vertices and the obstacles'
+        vertices (and forward_ad / torch.func work)."""
+        o = self._ray_arg(origin, "origin")
+        d = self._ray_arg(direction, "direction")
+        K = int(o.shape[1])
+        if d.shape[1] != K:
+            raise ValueError("direction: need as many queries as origin (%d), got %d" % (K, d.shape[1]))
+        r = self._float_arg(radius, "radius")
+        if r.dim() == 0 or (r.dim() == 1 and r.shape[0] == K):
+            r = r.expand(self.B, K)
+        elif tuple(r.shape) != (self.B, K):
+            raise ValueError("radius: need a scalar, [K] or [B, K] (B = %d, K = %d), got %s"
+                             % (self.B, K, tuple(r.shape)))
+        rd = r.detach()
+        # the kernel reads a bad radius as a miss; it is rejected here wherever the values can be read
+        if not torch._C._functorch.is_functorch_wrapped_tensor(rd) and not bool((torch.isfinite(rd) & (rd >= 0)).all()):
+            raise ValueError("radius: need finite radii >= 0")
+        md = _max_dist(max_dist)
+        nrm = d.norm(dim=2, keepdim=True)
+        u = d / torch.where(nrm > 0, nrm, torch.ones_like(nrm))      # a zero direction stays zero: it hits nothing
+        pverts = self.polygon_vertices() if self.np else None
+        needs_graph = _needs_graph((o, u, r) + self._geometry_leaves())
+        dist, body, feat, normal, point = self._query("lcpb200_shapecast", (o, r, None, u, None), (), K, md, True,
+                                                      pverts, (None, 0))
+        if needs_graph:
+            hit = body >= 0
+            dist, normal = self._ray_torch(o, u, body, feat.long() & 511, md, pverts, r)
+            point = torch.where(hit.unsqueeze(2), o + dist.unsqueeze(2) * u - r.unsqueeze(2) * normal,
+                                torch.zeros_like(o))
+        return dist, body, normal, point
+
+    def sweep(self, bodies, displacement):
+        """Translates each query body by `displacement` (no rotation) against every other body of its scene, held
+        still, at the current state (lcpb200_shapecast, body mode): the continuous-collision question of how far a body
+        can move before it touches something, e.g. sweep(ks, w.v.reshape(B, nd, 3)[:, ks, 1:] * w.dt). bodies [K]
+        (shared by the batch) or [B, K] of indices into [circles, polygons, obstacles]; displacement [B, K, 2] or
+        [K, 2]. Candidates are those of `nearest`: every other active body, obstacles included, except the world's
+        `no_contact` partners of the mover. A body the mover already overlaps is not seen, one it touches is seen only
+        when the motion heads into it: sweep reports new contacts, `distance` existing overlap.
+        Returns (frac [B, K] in [0, 1]: the fraction of the displacement travelled at the first contact, 1 when nothing
+        is hit, body [B, K] int64: the hit body, -1 for none (also for a zero displacement or an inactive mover),
+        normal [B, K, 2]: the unit normal from the mover towards the hit body, point [B, K, 2]: the contact point in
+        world coordinates at the time of impact); a miss reads frac 1, zeros and zero gradient.
+        The kernel makes every discrete choice; when a gradient or tangent is needed the outputs are rebuilt from them
+        with torch ops (_sweep_torch), so that gradients reach the displacement, p, the radii, the polygons' initial
+        vertices and the obstacles' vertices (and forward_ad / torch.func work)."""
+        bq, _ = self._body_arg(bodies, "bodies", False)
+        d = self._ray_arg(displacement, "displacement")
+        B, K = self.B, int(bq.shape[-1])
+        if d.shape[1] != K:
+            raise ValueError("displacement: need as many queries as bodies (%d), got %d" % (K, d.shape[1]))
+        bq = bq.expand(B, K)
+        L = d.norm(dim=2)
+        Ls = torch.where(L > 0, L, torch.ones_like(L))
+        u = d / Ls.unsqueeze(2)                                      # a zero displacement stays zero: it hits nothing
+        pverts = self.polygon_vertices() if self.np else None
+        needs_graph = _needs_graph((d,) + self._geometry_leaves())
+        dist, body, feat, normal, point = self._query("lcpb200_shapecast", (None, None, bq, u, L), (), K, 0.0, True,
+                                                      pverts, (self.nc_mask, self.nc_stride))
+        if needs_graph:
+            return self._sweep_torch(bq.long(), body, feat.long(), u, Ls, pverts)
+        return torch.where(body >= 0, dist / Ls, torch.ones_like(dist)), body, normal, point
+
+    def _sweep_torch(self, bq, bo, feat, u, L, pverts):
+        """Torch mirror of lcpb200_shapecast's body mode, REBUILT FROM THE KERNEL'S CHOICES: bq [B, K] the movers, bo
+        [B, K] the hit bodies (-1: a miss), feat their packed choices, u the unit directions, L the displacements'
+        lengths (1 where zero). The source (the hit body iff bit 17) gives the point x and rho (a circle's centre and
+        radius, or polygon vertex feat >> 9 & 255 and 0), cast along s u (s = -1 iff bit 17) against the target with
+        the target feat (bits 0-8), one _ray_torch: frac = t / L, normal -m (or m when the mover is the target), point
+        x + s t u - rho m, plus t u when the mover is the target. A miss reads frac 1 and zeros. Returns
+        (frac, body, normal, point)."""
+        nb = self.nb
+        B, K = bo.shape
+        hit = bo >= 0
+        src_b = hit & (((feat >> 17) & 1) == 1)
+        src = torch.where(src_b, bo, bq)
+        tgt = torch.where(hit, torch.where(src_b, bq, bo), -1)
+        is_c = src < nb
+        dt = self.dtype
+        x = torch.zeros(B, K, 2, dtype=dt, device=self.device)
+        rho = torch.zeros(B, K, dtype=dt, device=self.device)
+        if nb:
+            ci = torch.where(is_c, src, 0)
+            x = _take2(self.p[:, :nb, 1:], ci)
+            rho = torch.where(is_c, torch.gather(self.rad, 1, ci), rho)
+        if self.np or self.no:
+            polys = _polygons(pverts, self.ov if self.no else None)
+            vi = torch.where(is_c | ~hit, 0, (src - nb) * self.nv + ((feat >> 9) & 255))   # a miss's feat is -1
+            x = torch.where(is_c.unsqueeze(2), x, _take2(polys.reshape(B, -1, 2), vi))
+        su = torch.where(src_b.unsqueeze(2), -u, u)
+        t, m = self._ray_torch(x, su, tgt, torch.where(hit, feat & 511, -1), 0.0, pverts, rho)
+        frac = torch.where(hit, t / L, torch.ones_like(t))
+        normal = torch.where(src_b.unsqueeze(2), m, -m)
+        tu = torch.where(src_b, torch.zeros_like(t), t).unsqueeze(2) * u
+        point = torch.where(hit.unsqueeze(2), x + tu - rho.unsqueeze(2) * m, torch.zeros_like(x))
+        return frac, bo, normal, point
 
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
