@@ -449,6 +449,45 @@ int lcpb200_shapecast(int dtype, int B, int nb, int np, int no, int nv, int K, d
                       const int32_t* no_contact, long long nc_stride, void* dist, int32_t* body, int32_t* feat,
                       void* normal, void* point, void* stream);
 
+/* Times of impact between bodies that translate and rotate over a step, in B scenes (the body groups of
+ * lcpb200_contacts), K queries per scene. Over tau in [0, 1] dynamic body k moves as p_k + tau motion_k, motion =
+ * (dth, dx, dy) in the layout of p: a circle's centre moves (its rotation is irrelevant), a polygon's vertices are
+ * c + tau dc + R(tau dth)(v - c) (v its vertices, c its centre at tau = 0), obstacles stay. d(tau) is the body distance
+ * of lcpb200_body_distance between the two bodies at their poses at tau.
+ * Conservative advancement from tau = 0: at each iterate, with d = d(tau), its unit normal n (from A towards B) and
+ *   mu = -n . (dc_B - dc_A) + |dth_A| R_A + |dth_B| R_B      (R: the largest |v - c| of a polygon, 0 otherwise)
+ * a hit at tau iff d - gap <= tol; no hit iff mu <= 0 or tau + (d - gap) / mu > 1; else tau += (d - gap) / mu. mu bounds
+ * how fast d can fall, so the reported tau is never later than the first time d reaches gap. At most 64 evaluations:
+ * a pair that reaches the cap reports the tau it reached as a hit (dist then shows d - gap > tol). A pair with
+ * d(0) < skip is not seen, one with d(0) == skip only when mu > 0; nor is a pair whose bodies do not move or one with a
+ * non-finite motion row.
+ * Pair mode (body_b != NULL): query k is the pair (body_a[k], body_b[k]); a pair naming one body twice or an inactive
+ * body misses. First mode (body_b == NULL): query k is body_a[k] against every other active body of its scene not
+ * excluded by no_contact (the candidates of lcpb200_body_distance's nearest mode), in index order, from best = 1, body
+ * -1: a body replaces the best iff body < 0 ? tau <= best : tau < best. Deterministic (no atomics); results do not
+ * depend on how the queries are split into CTAs.
+ * Device pointers:
+ *   pos[B,nb,2] rad[B,nb] pverts[B,np,nv,2] overts[B,no,nv,2]   the bodies at tau = 0, as in lcpb200_signed_distance
+ *   pcen[B,np,2]                                      the polygons' centres c (NULL when np == 0)
+ *   motion[B,nb+np,3]                                 (dth, dx, dy) per dynamic body (NULL when nb + np == 0)
+ *   body_a[B,K] / body_b[B,K] int32                   as in lcpb200_body_distance ([K] when shared_queries != 0)
+ *   active_words, no_contact, nc_stride               as in lcpb200_body_distance; no_contact is read in first mode
+ *   frac[B,K] body[B,K] feat[B,K] int32               OUT: tau (1 on a miss), the hit body (-1: a miss) and the pair's
+ *                                                     dist_feat at tau (lcpb200_body_distance's packing; -1 on a miss)
+ *   dist[B,K]                                         OUT: d at tau (0 on a miss)
+ *   normal[B,K,2] point_a[B,K,2]                      OUT: n and the witness on A at tau, world coordinates (zero on a
+ *                                                     miss); the witness on B is point_a + dist normal
+ * gap >= 0 is the distance that counts as contact, skip >= 0 the overlap threshold above, tol >= 0 the tolerance of
+ * the stop. Returns non-zero without launching on B <= 0, K <= 0, nb + np + no == 0, nv > 256 (or nv < 3 with
+ * polygons), gap, skip or tol negative or non-finite (in the dtype), a NULL required pointer (body_a, the bodies,
+ * pcen, motion, every output), nc_stride < 0, active_words with nt > 8192, or B * K > 2^31 - 1. */
+int lcpb200_time_of_impact(int dtype, int B, int nb, int np, int no, int nv, int K, double gap, const void* pos,
+                           const void* rad, const void* pverts, const void* overts, const void* pcen,
+                           const void* motion, const int32_t* body_a, const int32_t* body_b, int shared_queries,
+                           double skip, double tol, const int32_t* active_words, const int32_t* no_contact,
+                           long long nc_stride, void* frac, int32_t* body, int32_t* feat, void* dist, void* normal,
+                           void* point_a, void* stream);
+
 /* Contact-list -> dense LCP assembly for B scenes of nb bodies (3 dofs each,
  * n = 3 nb), nc contacts, fd = 2 friction directions (world.py:191-192),
  * m = nc (2 + fd). Structure-of-arrays inputs:

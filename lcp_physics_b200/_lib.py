@@ -51,6 +51,8 @@ _SIGS = {
                               [_vp] * 2 + [ctypes.c_longlong] + [_vp] * 6),
     "lcpb200_shapecast": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 11 + [ctypes.c_longlong] +
                           [_vp] * 6),
+    "lcpb200_time_of_impact": (ctypes.c_int, [ctypes.c_int] * 7 + [ctypes.c_double] + [_vp] * 8 + [ctypes.c_int] +
+                               [ctypes.c_double] * 2 + [_vp] * 2 + [ctypes.c_longlong] + [_vp] * 7),
     "lcpb200_assemble": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 17),
     "lcpb200_assemble_backward": (ctypes.c_int, [ctypes.c_int] * 4 + [ctypes.c_double] + [_vp] * 25),
 }

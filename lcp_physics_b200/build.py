@@ -27,7 +27,7 @@ DUAL_DEPS = ["lcp_kernels.cu", "lcp_launch.h", "lcp_device.cuh", "lcp_lu.cuh", "
 COND_DEPS = ["lcp_cond_kernels.cu", "lcp_cond_launch.h", "lcp_device.cuh", "lcp_condensed.cuh"]
 BAND_DEPS = ["lcp_band_kernels.cu", "lcp_band_launch.h", "lcp_device.cuh", "lcp_condensed.cuh", "lcp_banded.cuh"]
 RAY_DEPS = ["lcp_ray_kernels.cu", "lcp_ray_launch.h", "lcp_raycast.cuh", "lcp_sdf.cuh", "lcp_distance.cuh",
-            "lcp_shapecast.cuh", "lcp_contacts.cuh"]
+            "lcp_shapecast.cuh", "lcp_toi.cuh", "lcp_contacts.cuh"]
 API_DEPS = (["lcpb200.cu", "lcp_assemble.cuh", "lcp_contacts.cuh", "lcp_ray_launch.h", "../../include/lcpb200.h"] +
             DUAL_DEPS[1:] + COND_DEPS[1:] + BAND_DEPS[1:])
 

@@ -133,11 +133,12 @@ __host__ __device__ __forceinline__ int pack_feat(int kind, int clip1, int ref2,
   return kind | clip1 << 2 | ref2 << 4 | re << 5 | ie << 13;
 }
 
-template <typename T>
-__host__ __device__ __forceinline__ bool edge_ok(const T* __restrict__ P, int nv, int e) {
+// P: the vertices, vertex v at P[2 v] -- a pointer, or a view that computes them on every read (ray::MovedVerts)
+template <class V>
+__host__ __device__ __forceinline__ bool edge_ok(V P, int nv, int e) {
   const int f = e + 1 == nv ? 0 : e + 1;
-  const T ex = P[2 * f] - P[2 * e], ey = P[2 * f + 1] - P[2 * e + 1];
-  return sqrt(ex * ex + ey * ey) > T(0);
+  const auto ex = P[2 * f] - P[2 * e], ey = P[2 * f + 1] - P[2 * e + 1];
+  return sqrt(ex * ex + ey * ey) > decltype(ex)(0);
 }
 
 template <typename T>
@@ -151,8 +152,9 @@ struct Sep {
 // n . (v2_sup - v1_e) to the edge; returns the edge of largest distance (first edge wins a tie: the reference
 // starts its scan at the edge that won last time). The pair is separated iff dist > eps (the early exit of :239-241
 // returns at the first edge that raises the running maximum above eps, so it fires iff the maximum is > eps).
-template <typename T>
-__host__ __device__ Sep<T> separation(const T* __restrict__ P1, T o1, const T* __restrict__ P2, int nv) {
+// P1 / P2: pointers or vertex views, as in edge_ok.
+template <typename T, class V1, class V2>
+__host__ __device__ Sep<T> separation(V1 P1, T o1, V2 P2, int nv) {
   Sep<T> s;
   s.dist = T(-INFINITY); s.edge = 0; s.sup = 0;
   for (int e = 0; e < nv; ++e) {

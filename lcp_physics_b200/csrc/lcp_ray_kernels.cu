@@ -1,10 +1,11 @@
 // lcp_ray_kernels.cu -- the batched ray cast (lcp_raycast.cuh), signed distance (lcp_sdf.cuh), body distance
-// (lcp_distance.cuh) and shape cast (lcp_shapecast.cuh), fp32 and fp64, in a translation unit of their own so that the contact, assembly and solver objects
-// do not change.
+// (lcp_distance.cuh), shape cast (lcp_shapecast.cuh) and time of impact (lcp_toi.cuh), fp32 and fp64, in a
+// translation unit of their own so that the contact, assembly and solver objects do not change.
 #include "lcp_raycast.cuh"
 #include "lcp_sdf.cuh"
 #include "lcp_distance.cuh"
 #include "lcp_shapecast.cuh"
+#include "lcp_toi.cuh"
 
 namespace lcpb200 {
 namespace ray {
@@ -60,6 +61,16 @@ cudaError_t launch_shapecast(const CastArgs<T>& a, int num_sms, cudaStream_t st)
 
 template cudaError_t launch_shapecast<float>(const CastArgs<float>&, int, cudaStream_t);
 template cudaError_t launch_shapecast<double>(const CastArgs<double>&, int, cudaStream_t);
+
+template <typename T>
+cudaError_t launch_toi(const ToiArgs<T>& a, int num_sms, cudaStream_t st) {
+  const Shape s = launch_shape(a.B, a.K, num_sms);
+  toi_kernel<T><<<s.grid, s.nth, 0, st>>>(a, s.chunks);
+  return cudaGetLastError();
+}
+
+template cudaError_t launch_toi<float>(const ToiArgs<float>&, int, cudaStream_t);
+template cudaError_t launch_toi<double>(const ToiArgs<double>&, int, cudaStream_t);
 
 }  // namespace ray
 }  // namespace lcpb200

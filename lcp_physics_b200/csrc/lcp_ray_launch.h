@@ -1,5 +1,5 @@
 // lcp_ray_launch.h -- host-side launch interface of the batched ray cast, signed distance, body distance and shape cast
-// (lcp_ray_kernels.cu, lcp_raycast.cuh, lcp_sdf.cuh, lcp_distance.cuh, lcp_shapecast.cuh).
+// and time of impact (lcp_ray_kernels.cu, lcp_raycast.cuh, lcp_sdf.cuh, lcp_distance.cuh, lcp_shapecast.cuh, lcp_toi.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -98,6 +98,33 @@ struct CastArgs {
 
 template <typename T>
 cudaError_t launch_shapecast(const CastArgs<T>& a, int num_sms, cudaStream_t st);
+
+// One batch of time-of-impact queries of lcpb200_time_of_impact, bd as in RayArgs plus pcen [B,np,2], the polygons'
+// centres. motion [B,nb+np,3] (dth, dx, dy). body_a / body_b / shared_queries as in DistArgs (body_b nullptr: first
+// mode); active and no_contact (first mode only) as in DistArgs. Outputs frac / body / feat / dist [B,K], normal /
+// point_a [B,K,2].
+template <typename T>
+struct ToiArgs {
+  cts::Bodies<T> bd;
+  int B, K;
+  T gap, skip, tol;
+  const T* motion;
+  const int32_t* body_a;
+  const int32_t* body_b;
+  int shared_queries;
+  const uint32_t* active;
+  const uint32_t* no_contact;
+  long long nc_stride;
+  T* frac;
+  int32_t* body;
+  int32_t* feat;
+  T* dist;
+  T* normal;
+  T* point_a;
+};
+
+template <typename T>
+cudaError_t launch_toi(const ToiArgs<T>& a, int num_sms, cudaStream_t st);
 
 }  // namespace ray
 }  // namespace lcpb200

@@ -37,11 +37,25 @@ struct StagedEdges {
   __device__ __forceinline__ T ny(int e) const { return N[2 * e + 1]; }
 };
 
-// The edges of a polygon whose normals were not staged (vertices P, orientation o from poly_orient): the flag and the
-// normal computed with the expressions of SceneWalk.
+// The vertices of a polygon moved rigidly on every read (time_of_impact, lcp_toi.cuh): stored vertex v maps to
+// v + (R(phi) - I)(v - c) + s, with cm1 = cos(phi) - 1 and sn = sin(phi). At phi = 0 and s = 0 every read returns the
+// stored value exactly.
 template <typename T>
-struct LoadedEdges {
+struct MovedVerts {
   const T* P;
+  T cm1, sn, cx, cy, sx, sy;
+  __device__ __forceinline__ T operator[](int i) const {
+    const int v = i >> 1;
+    const T wx = P[2 * v] - cx, wy = P[2 * v + 1] - cy;
+    return (i & 1) ? P[i] + ((sn * wx + cm1 * wy) + sy) : P[i] + ((cm1 * wx - sn * wy) + sx);
+  }
+};
+
+// The edges of a polygon whose normals were not staged (vertices P, orientation o from poly_orient): the flag and the
+// normal computed with the expressions of SceneWalk. V: the vertex access, a pointer or MovedVerts.
+template <typename T, class V = const T*>
+struct LoadedEdges {
+  V P;
   T o;
   int nv;
   __device__ __forceinline__ bool ok(int e) const { return cts::edge_ok(P, nv, e); }
@@ -58,13 +72,13 @@ struct LoadedEdges {
 };
 
 // The choices of the signed distance of point (px, py) to one convex polygon g (StagedEdges or LoadedEdges of nv
-// vertices), the rule above: smax / emax the largest s_e and its edge (emax < 0: no edge of non-zero length), dmin /
-// emin the smallest |x - q_e|^2 and its edge, (qdx, qdy) = x - q of that edge. Shared by sdf_kernel and distance_kernel
-// (lcp_distance.cuh).
+// vertices, read through g.P), the rule above: smax / emax the largest s_e and its edge (emax < 0: no edge of non-zero
+// length), dmin / emin the smallest |x - q_e|^2 and its edge, (qdx, qdy) = x - q of that edge. Shared by sdf_kernel,
+// distance_kernel (lcp_distance.cuh) and toi_kernel (lcp_toi.cuh).
 template <typename T, class G>
 __device__ __forceinline__ void point_polygon(const G& g, int nv, T px, T py, T& smax, int& emax, T& dmin, int& emin,
                                               T& qdx, T& qdy) {
-  const T* P = g.P;
+  const auto& P = g.P;
   smax = T(-INFINITY); dmin = T(INFINITY); qdx = T(0); qdy = T(0);
   emax = -1; emin = -1;
   for (int e = 0; e < nv; ++e) {

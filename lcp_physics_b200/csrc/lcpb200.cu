@@ -1180,8 +1180,8 @@ extern "C" int lcpb200_contacts_active(int dtype, int B, int nb, int np, int no,
 }
 
 // ------------------------------------------------------------------ ray casts, signed distances, body distances, shape casts
-// Argument checks shared by lcpb200_raycast, lcpb200_signed_distance, lcpb200_body_distance and lcpb200_shapecast. what
-// prefixes the messages; N counts the
+// Argument checks shared by lcpb200_raycast, lcpb200_signed_distance, lcpb200_body_distance, lcpb200_shapecast and
+// lcpb200_time_of_impact. what prefixes the messages; N counts the
 // queries per scene, named n_name and counted as `items` in the messages. queries_set: the entry's own query pointers
 // (origin and dir, or points) are non-NULL, so that one message covers every NULL pointer.
 static int check_query(const char* what, const char* n_name, const char* items, int dtype, int B, int N, int nb,
@@ -1316,6 +1316,41 @@ extern "C" int lcpb200_shapecast(int dtype, int B, int nb, int np, int no, int n
     a.nc_stride = nc_stride;
     a.dist = (T*)dist; a.body = body; a.feat = feat; a.normal = (T*)normal; a.point = (T*)point;
     return ray::launch_shapecast<T>(a, sms, (cudaStream_t)stream);
+  };
+  CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
+  return 0;
+}
+
+// The motion lives in device memory, which this entry does not read: the kernel treats a non-finite motion row as no
+// motion to test (BatchedWorld rejects one on the host). gap is checked as max_dist is; skip and tol here.
+extern "C" int lcpb200_time_of_impact(int dtype, int B, int nb, int np, int no, int nv, int K, double gap,
+                                      const void* pos, const void* rad, const void* pverts, const void* overts,
+                                      const void* pcen, const void* motion, const int32_t* body_a,
+                                      const int32_t* body_b, int shared_queries, double skip, double tol,
+                                      const int32_t* active_words, const int32_t* no_contact, long long nc_stride,
+                                      void* frac, int32_t* body, int32_t* feat, void* dist, void* normal,
+                                      void* point_a, void* stream) {
+  if (int rc = check_query("time_of_impact", "K", "queries", dtype, B, K, nb, np, no, nv, gap, pos, rad, pverts,
+                           overts, body_a && (nb + np == 0 || motion), frac, body, feat, active_words))
+    return rc;
+  const double big = dtype == LCPB200_F32 ? FLT_MAX : DBL_MAX;
+  if (!(std::isfinite(skip) && skip >= 0 && skip <= big && std::isfinite(tol) && tol >= 0 && tol <= big))
+    return fail("time_of_impact: need finite skip, tol >= 0");
+  if ((np > 0 && !pcen) || !dist || !normal || !point_a) return fail("time_of_impact: NULL argument");
+  if (nc_stride < 0) return fail("time_of_impact: need nc_stride >= 0");
+  int sms = 0;
+  if (int rc = current_sms(sms)) return rc;
+  auto launch = [&](auto zero) {      // the body for T = the type of zero
+    using T = decltype(zero);
+    ray::ToiArgs<T> a{};
+    a.bd = query_bodies<T>(nb, np, no, nv, pos, rad, pverts, overts);
+    a.bd.pcen = (const T*)pcen;
+    a.B = B; a.K = K; a.gap = (T)gap; a.skip = (T)skip; a.tol = (T)tol;
+    a.motion = (const T*)motion; a.body_a = body_a; a.body_b = body_b; a.shared_queries = shared_queries != 0;
+    a.active = (const uint32_t*)active_words; a.no_contact = (const uint32_t*)no_contact; a.nc_stride = nc_stride;
+    a.frac = (T*)frac; a.body = body; a.feat = feat; a.dist = (T*)dist; a.normal = (T*)normal;
+    a.point_a = (T*)point_a;
+    return ray::launch_toi<T>(a, sms, (cudaStream_t)stream);
   };
   CK(dtype == LCPB200_F32 ? launch(0.0f) : launch(0.0));
   return 0;

@@ -293,6 +293,18 @@ def _max_dist(max_dist):
     return md
 
 
+def _length(x, name):
+    """A distance parameter (gap, skip, tol) as a float, finite and >= 0."""
+    v = float(x)
+    if not math.isfinite(v) or v < 0:
+        raise ValueError("%s: need a finite value >= 0, got %r" % (name, x))
+    return v
+
+
+# default stop tolerance of time_of_impact / first_impact, in world units
+TOI_TOL = {torch.float64: 1e-9, torch.float32: 1e-4}
+
+
 def _check_count(v, name):
     """Rejects a count (rays, pixels) that is not an int >= 1; bool is not a count."""
     if isinstance(v, bool) or not isinstance(v, int) or v < 1:
@@ -412,7 +424,7 @@ class BatchedWorld:
                  strict_no_penetration=True, max_iter=10, contact_capacity=None, device=None, exact_adjoint=False,
                  obstacles=None, obstacle_fric=0.9, obstacle_rest=0.5, polygons=None, poly_rot=0.0, poly_vel=None,
                  poly_mass=1.0, poly_fric=0.9, poly_rest=0.5, constraints=None, no_contact=None,
-                 external_force=None, active=None):
+                 external_force=None, active=None, ccd=False):
         """pos [B,nb,2] (nb may be 0), rad [B,nb] (or [nb] / scalar), vel [B,nb,3] (rot, x, y) or None, mass /
         restitution / fric_coeff [B,nb] (or broadcastable).
         `polygons`: dynamic convex polygons, the reference's `Rect` / `Hull` bodies (bodies.py:154-301): world-frame
@@ -445,7 +457,10 @@ class BatchedWorld:
         unchanged, and it makes no contact (the contact walk of each scene visits its active bodies only). A
         constraint belongs to the scenes in which all its bodies are active; one with active and inactive bodies in
         the same scene raises ValueError (list, e.g., a 4-link and a 7-link chain and activate one of them per scene).
-        At most 8192 bodies in all (nb + npoly + no) with `active` or per-scene `no_contact`."""
+        At most 8192 bodies in all (nb + npoly + no) with `active` or per-scene `no_contact`.
+        `ccd`: continuous collision detection in `step()`: each scene's step ends at the first impact of its bodies'
+        motion v dt (first_impact with gap eps / 2 and skip eps), so that a fast body does not pass through a thin one
+        unseen; pairs already within eps are left to the contact solve. False (the default) steps as the reference."""
         _lib.require_cuda()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         pos = torch.as_tensor(pos)
@@ -504,6 +519,7 @@ class BatchedWorld:
         self.dt, self.eps, self.tol = float(dt), float(eps), float(tol)
         self.post_stab, self.strict_no_pen, self.max_iter = post_stab, strict_no_penetration, max_iter
         self.exact_adjoint = bool(exact_adjoint)
+        self.ccd = bool(ccd)
         self.no, self.nv = 0, 0
         if obstacles is not None:
             ov = check_obstacles(obstacles, B)
@@ -723,9 +739,13 @@ class BatchedWorld:
     def polygon_vertices(self):
         """World-frame vertices [B, npoly, V, 2] of the dynamic polygons at the current p: centroid + R(rot) local
         (Hull.set_p / rotate_verts, bodies.py:202-214), differentiable in p and the polygons' initial vertices."""
-        q = self.p[:, self.nb:]
+        return self._vertices_at(self.p, self.plocal)
+
+    def _vertices_at(self, p, plocal):
+        """polygon_vertices() at the poses p [B', nd, 3] of polygons plocal [B', npoly, V, 2]"""
+        q = p[:, self.nb:]
         c, s = torch.cos(q[:, :, 0:1]), torch.sin(q[:, :, 0:1])
-        lx, ly = self.plocal[..., 0], self.plocal[..., 1]
+        lx, ly = plocal[..., 0], plocal[..., 1]
         return torch.stack([q[:, :, 1:2] + (c * lx - s * ly), q[:, :, 2:3] + (s * lx + c * ly)], 3)
 
     def _hull_torch(self, i1, i2, feat, verts, ref):
@@ -928,14 +948,15 @@ class BatchedWorld:
         polygons' initial vertices and the obstacle vertices."""
         return self.p, self.rad, self.plocal if self.np else None, self.ov if self.no else None
 
-    def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts, no_contact=None):
+    def _query(self, entry, queries, flags, n, max_dist, with_normal, pverts, no_contact=None, with_dist=False):
         """One call of the ray, point, body-distance or shape-cast kernel `entry` (lcpb200_raycast,
         lcpb200_signed_distance, lcpb200_body_distance or lcpb200_shapecast) over n queries per scene at the current
         state. The entry's arguments between overts and active_words are the tensors `queries` (None: NULL), then the
         ints `flags`. no_contact: for lcpb200_body_distance and lcpb200_shapecast, their arguments after active_words
         (the mask or None, its stride); those entries also write point_a (shapecast's point). pverts:
         polygon_vertices() (worlds with polygons). Returns (value [B, n], body [B, n] int64, feat [B, n] int32, normal
-        [B, n, 2] when with_normal, else None, point_a [B, n, 2] with no_contact, else None)."""
+        [B, n, 2] when with_normal, else None, point_a [B, n, 2] with no_contact, else None). with_dist: the entry
+        writes a second value [B, n] after feat (lcpb200_time_of_impact's dist), appended to the result."""
         lib = _lib.load()
         B, nb, dev = self.B, self.nb, self.device
         with_point = no_contact is not None
@@ -947,20 +968,23 @@ class BatchedWorld:
             feat = torch.empty(B, n, dtype=torch.int32, device=dev)
             normal = new(2) if with_normal else None
             point_a = new(2) if with_point else None
+            value2 = new() if with_dist else None
             with torch.cuda.device(dev):
                 _lib.check(getattr(lib, entry)(
                     _lib.dtype_code(self.dtype), B, nb, self.np, self.no, self.nv, n, max_dist, _lib.ptr(pos),
                     _lib.ptr(rad), _lib.ptr(pv), _lib.ptr(ov), *[_lib.ptr(q) for q in qs], *flags, _lib.ptr(aw),
                     *((_lib.ptr(nc), no_contact[1]) if with_point else ()), _lib.ptr(value), _lib.ptr(body),
-                    _lib.ptr(feat), _lib.ptr(normal), *((_lib.ptr(point_a),) if with_point else ()),
-                    _lib.stream_ptr(dev)))
+                    _lib.ptr(feat), *((_lib.ptr(value2),) if with_dist else ()), _lib.ptr(normal),
+                    *((_lib.ptr(point_a),) if with_point else ()), _lib.stream_ptr(dev)))
             # tensors only: _DetectFn marks every output non-differentiable
-            return tuple(t for t in (value, body, feat, normal, point_a) if t is not None)
+            return tuple(t for t in (value, body, feat, normal, point_a, value2) if t is not None)
         nc = no_contact[0] if with_point else None
         out = _detect(call, _detached(self.p[:, :nb, 1:]), _detached(self.rad), _detached(pverts),
                       _detached(self.ov if self.no else None), self.active_words, nc, *[_detached(q) for q in queries])
         rest = iter(out[3:])
         normal, point_a = next(rest) if with_normal else None, next(rest) if with_point else None
+        if with_dist:
+            return out[0], out[1].long(), out[2], normal, point_a, next(rest)
         return out[0], out[1].long(), out[2], normal, point_a
 
     def raycast(self, origin, direction, max_dist):
@@ -1081,13 +1105,17 @@ class BatchedWorld:
             sdf, normal = self._sdf_torch(x, body, feat.long(), md, pverts)
         return sdf, body, normal
 
-    def _sdf_torch(self, points, body, feat, max_dist, pverts):
+    def _sdf_torch(self, points, body, feat, max_dist, pverts, cpos=None, rad=None, ov=None):
         """Torch mirror of csrc/lcp_sdf.cuh, REBUILT FROM THE KERNEL'S CHOICES body / feat [B, Q]: |x - c| - r and
         (x - c) / |x - c| for a circle; n_e . (x - v_e) and n_e inside a polygon (feat 256 + e); outside (feat e) the
         distance to the closest point q of edge e (v_e, v_f or v_e + t E) and (x - q) / |x - q|; max_dist (a constant)
         and a zero normal where no body was chosen. points [B, Q, 2] or [Q, 2]. A zero distance (a point at a circle's
-        centre or on the closest point) gives a zero normal and finite gradients."""
+        centre or on the closest point) gives a zero normal and finite gradients. cpos [B, nb, 2] / rad [B, nb] / ov
+        [B, no, V, 2]: the circles' centres and radii and the obstacles' vertices, the world's when None."""
         nb = self.nb
+        cpos = self.p[:, :nb, 1:] if cpos is None else cpos
+        rad = self.rad if rad is None else rad
+        ov = (self.ov if self.no else None) if ov is None else ov
         B, Q = body.shape
         x = points.expand(B, Q, 2) if points.dim() == 2 else points
 
@@ -1104,11 +1132,11 @@ class BatchedWorld:
         normal = torch.zeros_like(x)
         if nb:
             ci = torch.where(is_c, body, 0)
-            ln, n_c = length(x - _take2(self.p[:, :nb, 1:], ci))
-            sdf = torch.where(is_c, ln - torch.gather(self.rad, 1, ci), sdf)
+            ln, n_c = length(x - _take2(cpos, ci))
+            sdf = torch.where(is_c, ln - torch.gather(rad, 1, ci), sdf)
             normal = torch.where(is_c.unsqueeze(2), n_c, normal)
         if self.np or self.no:
-            polys = _polygons(pverts, self.ov if self.no else None)
+            polys = _polygons(pverts, ov)
             inside = is_p & (feat >= 256)
             ve, vf, E, sg = _chosen_edge(polys, body, feat % 256, nb)
             ee = torch.where(is_p, (E * E).sum(2), torch.ones_like(E[..., 0]))
@@ -1219,15 +1247,18 @@ class BatchedWorld:
             return dist, body, normal, point_a, point_b
         return dist, body, normal, point_a, point_a + dist.unsqueeze(2) * normal
 
-    def _distance_torch(self, ba, bo, feat, max_dist, pverts):
+    def _distance_torch(self, ba, bo, feat, max_dist, pverts, cpos=None, rad=None, ov=None):
         """Torch mirror of csrc/lcp_distance.cuh, REBUILT FROM THE KERNEL'S CHOICES: ba [B, K] the first body, bo [B, K]
         the kernel's other body (-1: a miss), feat its packed choices. The source point x and radius r (a circle's
         centre and radius, or polygon vertex feat >> 9 & 255 and 0) of the source body (the other body iff bit 17),
         then one _sdf_torch of x against the target with the target feat (bits 0-8): d = sdf - r, n = -m (the first body
         the source) or m (the other), point_a = x - r m or x - sdf m, point_b = point_a + d n. A miss reads max_dist (a
-        constant) and zeros. Returns (dist, normal, point_a, point_b)."""
+        constant) and zeros. Returns (dist, normal, point_a, point_b). cpos / rad / ov: as in _sdf_torch."""
         nb = self.nb
         B, K = bo.shape
+        cpos = self.p[:, :nb, 1:] if cpos is None else cpos
+        rad = self.rad if rad is None else rad
+        ov = (self.ov if self.no else None) if ov is None else ov
         hit = bo >= 0
         src_b = hit & (((feat >> 17) & 1) == 1)
         src = torch.where(src_b, bo, ba)
@@ -1238,13 +1269,13 @@ class BatchedWorld:
         r = torch.zeros(B, K, dtype=dt, device=self.device)
         if nb:
             ci = torch.where(is_c, src, 0)
-            x = _take2(self.p[:, :nb, 1:], ci)
-            r = torch.where(is_c, torch.gather(self.rad, 1, ci), r)
+            x = _take2(cpos, ci)
+            r = torch.where(is_c, torch.gather(rad, 1, ci), r)
         if self.np or self.no:
-            polys = _polygons(pverts, self.ov if self.no else None)
+            polys = _polygons(pverts, ov)
             vi = torch.where(is_c | ~hit, 0, (src - nb) * self.nv + ((feat >> 9) & 255))   # a miss's feat is -1
             x = torch.where(is_c.unsqueeze(2), x, _take2(polys.reshape(B, -1, 2), vi))
-        sdf, m = self._sdf_torch(x, tgt, feat & 511, max_dist, pverts)
+        sdf, m = self._sdf_torch(x, tgt, feat & 511, max_dist, pverts, cpos, rad, ov)
         dist = torch.where(hit, sdf - r, sdf)
         normal = torch.where(src_b.unsqueeze(2), m, -m)
         w = torch.where(src_b, sdf, r)
@@ -1360,6 +1391,109 @@ class BatchedWorld:
         point = torch.where(hit.unsqueeze(2), x + tu - rho.unsqueeze(2) * m, torch.zeros_like(x))
         return frac, bo, normal, point
 
+    # ------------------------------------------------------------------ times of impact
+    def time_of_impact(self, pairs, motion, gap=0.0, skip=None, tol=None):
+        """Time of impact of each pair of bodies, both translating and rotating over one motion, from the current state
+        (lcpb200_time_of_impact, pair mode): pairs [K, 2] (shared by the batch) or [B, K, 2] of indices into [circles,
+        polygons, obstacles]; motion [B, nd, 3] or [B, n], each dynamic body's displacement (rot, x, y) over the motion,
+        e.g. w.v.reshape(B, nd, 3) * w.dt. Over tau in [0, 1] body k sits at p_k + tau motion_k (the motion of a
+        step); obstacles stay. The first tau at which the pair's distance (`distance`) falls to `gap` is found by
+        conservative advancement (DESIGN.md section 8), never later than the true contact; within `tol` (world units;
+        default TOI_TOL of the dtype, 1e-9 in float64 and 1e-4 in float32). A pair closer than `skip` (default: gap) at
+        tau = 0 is not seen, one exactly at skip only when it closes: new contacts, not existing ones.
+        Returns (frac [B, K]: tau, 1 when nothing is hit, body [B, K] int64: the pair's second body, -1 for no hit, an
+        inactive body or two still bodies, dist [B, K]: the distance at tau, normal [B, K, 2]: the unit normal from the
+        first body towards the second at tau, point_a / point_b [B, K, 2]: the witnesses at tau, point_b = point_a +
+        dist normal); a miss reads frac 1 and zeros, with zero gradient.
+        The kernel makes every discrete choice; when a gradient or tangent is needed, the outputs are rebuilt from them
+        with torch ops (_impact_torch): frac through the implicit-function derivative of the level set d = d(tau) at
+        the hit, so that gradients reach the motion, p, the radii, the polygons' initial vertices and the obstacles'
+        vertices (and forward_ad / torch.func work). A hit at tau = 0, or one where d does not fall (a grazing touch),
+        carries no gradient of frac."""
+        t, shared = self._body_arg(pairs, "pairs", True)
+        return self._impact(t[..., 0], t[..., 1], shared, motion, gap, skip, tol)
+
+    def first_impact(self, bodies, motion, gap=0.0, skip=None, tol=None):
+        """The first impact of each query body over the motion (lcpb200_time_of_impact, first mode): bodies [K] (shared
+        by the batch) or [B, K]; candidates are those of `nearest` (every other active body, obstacles included,
+        except the world's `no_contact` partners), each moving by its own motion row; the lower index wins a tie.
+        Returns what `time_of_impact` returns for the pair (query, first body hit)."""
+        t, shared = self._body_arg(bodies, "bodies", False)
+        return self._impact(t, None, shared, motion, gap, skip, tol)
+
+    def _motion_arg(self, motion):
+        """motion [B, nd, 3] or [B, n] as a [B, nd, 3] tensor of the world's dtype / device; finite where readable"""
+        m = self._float_arg(motion, "motion")
+        if tuple(m.shape) == (self.B, self.n):
+            m = m.reshape(self.B, self.nd, 3)
+        if tuple(m.shape) != (self.B, self.nd, 3):
+            raise ValueError("motion: need [B, nd, 3] or [B, 3 nd] (B = %d, nd = %d), got %s"
+                             % (self.B, self.nd, tuple(m.shape)))
+        md = m.detach()
+        # the kernel reads a non-finite row as no motion; it is rejected here wherever the values can be read
+        if not torch._C._functorch.is_functorch_wrapped_tensor(md) and not bool(torch.isfinite(md).all()):
+            raise ValueError("motion: need finite values")
+        return m
+
+    def _impact(self, ba, bb, shared, motion, gap, skip, tol):
+        m = self._motion_arg(motion)
+        gap = _length(gap, "gap")
+        skip = gap if skip is None else _length(skip, "skip")
+        tol = TOI_TOL[self.dtype] if tol is None else _length(tol, "tol")
+        B, K = self.B, int(ba.shape[-1])
+        pverts = self.polygon_vertices() if self.np else None
+        pcen = self.p[:, self.nb:, 1:] if self.np else None
+        needs_graph = _needs_graph((m,) + self._geometry_leaves())
+        no_contact = (self.nc_mask, self.nc_stride) if bb is None else (None, 0)     # first mode only
+        frac, body, feat, normal, point_a, dist = self._query(
+            "lcpb200_time_of_impact", (pcen, m, ba, bb), (int(shared), skip, tol), K, gap, True, pverts, no_contact,
+            with_dist=True)
+        if needs_graph:
+            return self._impact_torch(ba.long().expand(B, K), body, feat.long(), frac, m)
+        return frac, body, dist, normal, point_a, point_a + dist.unsqueeze(2) * normal
+
+    def _impact_torch(self, ba, bo, feat, tau, motion):
+        """Torch mirror of lcpb200_time_of_impact, REBUILT FROM THE KERNEL'S CHOICES: ba [B, K] the first body, bo
+        [B, K] the hit body (-1: a miss), feat the pair's distance choices at the kernel's tau [B, K], motion
+        [B, nd, 3]. D(t) is _distance_torch of the pair at the poses p + t motion (each query at its own t). frac =
+        tau - (D(tau) - D(tau).detach()) / Ddot, with tau and Ddot = n . (u_B(point_b) - u_A(point_a)) detached
+        (u_k(x) = dc_k + dth_k perp(x - c_k(tau)), the velocity of body k's material point x; dth = 0 for a circle):
+        the value is tau, the derivative that of the level set through the hit. Hits at tau = 0 or with Ddot >= 0 keep
+        tau constant. dist, normal and the witnesses are D's at p + frac motion. A miss reads frac 1 and zeros.
+        Returns (frac, body, dist, normal, point_a, point_b)."""
+        nb, nd, no = self.nb, self.nd, self.no
+        B, K = bo.shape
+        hit = bo >= 0
+        tau = tau.detach()
+        circle = torch.zeros(nd, 1, dtype=torch.bool, device=motion.device)
+        circle[:nb] = True
+        mo = torch.cat([torch.where(circle, 0.0, motion[..., :1]), motion[..., 1:]], 2)   # a circle does not turn
+
+        def at(t):
+            """_distance_torch of every query at the poses p + t motion, t [B, K]; [B, K] / [B, K, 2] results"""
+            p = (self.p.unsqueeze(1) + t.reshape(B, K, 1, 1) * mo.unsqueeze(1)).reshape(B * K, nd, 3)
+            rep = lambda x: None if x is None else x.repeat_interleave(K, 0)
+            pv = self._vertices_at(p, rep(self.plocal)) if self.np else None
+            ov = rep(self.ov) if no else None
+            out = self._distance_torch(ba.reshape(-1, 1), bo.reshape(-1, 1), feat.reshape(-1, 1), 0.0, pv,
+                                       p[:, :nb, 1:], rep(self.rad), ov)
+            return [x.reshape((B, K) + x.shape[2:]) for x in out]
+        d, n, pa, pb = at(tau)
+        # the velocities of the witnesses, detached; obstacles (index >= nd) do not move
+        full = torch.cat([mo, mo.new_zeros(B, no, 3)], 1).detach()
+        cen = torch.cat([self.p[..., 1:], self.p.new_zeros(B, no, 2)], 1).detach()
+
+        def vel(k, x):
+            dk = torch.gather(full, 1, k.unsqueeze(2).expand(-1, -1, 3))
+            w = x.detach() - (_take2(cen, k) + tau.unsqueeze(2) * dk[..., 1:])
+            return dk[..., 1:] + dk[..., :1] * torch.stack([-w[..., 1], w[..., 0]], 2)
+        ddot = (n.detach() * (vel(torch.where(hit, bo, 0), pb) - vel(ba, pa))).sum(2)
+        moving = hit & (tau > 0) & (ddot < 0)
+        frac = tau - torch.where(moving, (d - d.detach()) / torch.where(moving, ddot, torch.ones_like(ddot)),
+                                 torch.zeros_like(d))
+        dist, normal, point_a, point_b = at(frac)
+        return frac, bo, dist, normal, point_a, point_b
+
     # ------------------------------------------------------------------ engine calls
     def _lcp(self, mode, dt, b, fext=None):
         mass, inertia, v = self.mass, self.inertia, self.v
@@ -1416,7 +1550,14 @@ class BatchedWorld:
         self.v = self.solve_dynamics(dt)
         if self.active is not None:
             self.v = torch.where(self.dof_active, self.v, start_v)                 # frozen bodies keep p and v
-        dts = self.v.new_full((self.B,), float(dt))
+        if self.ccd:
+            # end the step at the first impact: the pair then sits near eps / 2, inside the contact margin eps
+            dyn = torch.arange(self.nd, device=self.device)
+            toi = self.first_impact(dyn, self.v.reshape(self.B, self.nd, 3) * float(dt), gap=self.eps / 2,
+                                    skip=self.eps)[0]
+            dts = float(dt) * toi.min(dim=1).values
+        else:
+            dts = self.v.new_full((self.B,), float(dt))
         done = torch.zeros(self.B, dtype=torch.bool, device=self.device)
         while True:
             moved = start_p + self.v.reshape(self.B, self.nd, 3) * dts.reshape(self.B, 1, 1)      # body.move(dt)
